@@ -304,6 +304,11 @@ __global__ void __launch_bounds__(128)
         for (int c = 0; c < it.ncomp && !status; c++) {
             const int td = it.td[c], ta = 4 + it.ta[c];
             for (int j = 0; j < it.h[c] * it.v[c]; j++, blk += 64) {
+                if (inside) {  // this thread owns the whole block: clear it here instead of memsetting the array
+                    uint4* const z = reinterpret_cast<uint4*>(blk);
+#pragma unroll
+                    for (int i = 0; i < 8; i++) z[i] = make_uint4(0, 0, 0, 0);
+                }
                 int s = huff_symbol(b, hs, td);
                 if (s < 0 || s > 15) { status = -3; break; }
                 if (s) pred[c] += receive_extend(b, s);
@@ -812,7 +817,12 @@ __global__ void __launch_bounds__(128)
 
 int jpeg_decode_launch(const JpegDecodeBatch& b, cudaStream_t st, cudaEvent_t ev_after_huff) {
     if (b.n <= 0) return LP_OK;
-    LP_CUDA_OK(cudaMemsetAsync(b.coef, 0, b.coef_elems_total * sizeof(int16_t), st));
+    // The serial and multi-scan decoders store only the nonzero coefficients of a zeroed array.  The
+    // parallel decoders (self-synchronising and restart-interval) clear every block of the region of
+    // interest themselves as they open it, so their array is not cleared: at 4096 1080p images that
+    // memset alone would write 15 GB per batch.  Blocks of an image that fails are not read.
+    if (b.scans || !b.use_parallel_huffman)
+        LP_CUDA_OK(cudaMemsetAsync(b.coef, 0, b.coef_elems_total * sizeof(int16_t), st));
     if (b.scans) {
         jpeg_multiscan_kernel<<<1, 32, 0, st>>>(b.items, b.scans, b.nscans, b.tables, b.scan, b.coef);
         g_launches++;

@@ -14,7 +14,8 @@
 //                            until no exit state changes (a fixed point that is exact by induction
 //                            from subsequence 0).  A prefix sum of the per-subsequence coefficient
 //                            counts gives every subsequence its absolute output position, and one
-//                            last decode writes AC coefficients and DC differences;
+//                            last decode writes whole coefficient blocks (zero-filled by the thread
+//                            that opens them) and DC differences;
 //   3. the same kernel then turns DC differences into DC values with a per-component prefix sum.
 // (Scheme after Weissenberger & Schmidt, "Accelerating JPEG Decompression on GPUs", restated from
 // the published description.)
@@ -258,15 +259,25 @@ struct BitWin {
 // Decode symbols that START in [p, limit).  Returns the exit state and the number of coefficient
 // slots consumed.  WRITE: store coefficients (DC slot receives the DC *difference*) starting at
 // absolute slot `pos`.
+//
+// WRITE stores whole blocks: the coefficient array is not cleared beforehand.  The span that decodes
+// a block's DC symbol owns that block: it zero-fills the block's 128 bytes before its first
+// coefficient store and, if the block is still open at `limit`, decodes on past `limit` (at most to
+// `end_bits`, the end of the stream) until the block closes.  A span that starts inside a block
+// (z > 0) stores nothing until that block closes; its owner writes it.  So every block is written by
+// one thread and no ordering between threads is needed.
 template <bool WRITE, bool TWO>
 __device__ __forceinline__ void decode_span_t(const HuffShared& hs, const uint8_t* s, uint32_t& p, uint32_t limit,
-                                            uint32_t& phase, uint32_t& nslots, int nb,
+                                            uint32_t end_bits, uint32_t& phase, uint32_t& nslots, int nb,
                                             uint64_t pos, uint64_t total_slots, const JpegDecodeItem* it,
                                             int16_t* coef, int16_t* dcdiff, int* status) {
     uint32_t blk = phase >> 6, z = phase & 63;
     const uint32_t z_start = z;
     uint32_t closed = 0;                       // blocks completed in this span
     int32_t bits_left = (int32_t)(limit - p);  // symbols that START before `limit` belong to this span
+    // WRITE: an owned block that is still open at `limit` is decoded to its end, but not past the stream
+    const int32_t own_floor = (int32_t)limit - (int32_t)end_bits;
+    bool own = z_start == 0;  // WRITE: the current block was opened by this span
     BitWin bw;
     bw.init(s, p);
     // WRITE: running block position.  Coefficients of the region of interest are stored in MCU (scan)
@@ -316,7 +327,7 @@ __device__ __forceinline__ void decode_span_t(const HuffShared& hs, const uint8_
     // The symbol step uses selects instead of branches: lanes of a warp sit at unrelated places of
     // unrelated subsequences, so every branch here would be a divergent one.  Coefficient slots are
     // not counted per symbol: slots = 64 * blocks closed + z_end - z_start.
-    while (bits_left > 0) {
+    while (bits_left > 0 || (WRITE && own && z != 0 && bits_left > own_floor)) {
         bw.refill();
         const uint32_t top = bw.peek();
         const bool isdc = z == 0;
@@ -366,12 +377,18 @@ __device__ __forceinline__ void decode_span_t(const HuffShared& hs, const uint8_
             int16_t* const where = isdc ? dcp : dstblk + zi;  // DC difference: every block; AC: inside the ROI
             const bool inblk = zt <= 64;
             bad |= !ez && !inblk;  // coefficient index past 63: corrupt data
-            if (!ez && inblk && (isdc || inside)) *where = (int16_t)val;
+            if (isdc && inside) {  // opening a block (z == 0 implies own): clear it before its AC stores
+                uint4* const q = reinterpret_cast<uint4*>(dstblk);
+#pragma unroll
+                for (int k = 0; k < 8; k++) q[k] = make_uint4(0, 0, 0, 0);
+            }
+            if (!ez && inblk && own && (isdc || inside)) *where = (int16_t)val;
         }
         bw.skip(used);
         bits_left -= used;
         const bool fin = zt >= 64;  // block finished
         z = fin ? 0u : zt;
+        if (WRITE) own |= fin;
         if (!WRITE) {
             // lanes sit at unrelated places, so SOME lane closes a block in nearly every iteration: keep the
             // bookkeeping to selects instead of a branch the whole warp would walk through
@@ -406,13 +423,13 @@ __device__ __forceinline__ void decode_span_t(const HuffShared& hs, const uint8_
 // compare, anything else looks them up per block.  hs.two_tables is uniform across the CTA.
 template <bool WRITE>
 __device__ __forceinline__ void decode_span(const HuffShared& hs, const uint8_t* s, uint32_t& p, uint32_t limit,
-                                            uint32_t& phase, uint32_t& nslots, int nb,
+                                            uint32_t end_bits, uint32_t& phase, uint32_t& nslots, int nb,
                                             uint64_t pos, uint64_t total_slots, const JpegDecodeItem* it,
                                             int16_t* coef, int16_t* dcdiff, int* status) {
     if (hs.two_tables)
-        decode_span_t<WRITE, true>(hs, s, p, limit, phase, nslots, nb, pos, total_slots, it, coef, dcdiff, status);
+        decode_span_t<WRITE, true>(hs, s, p, limit, end_bits, phase, nslots, nb, pos, total_slots, it, coef, dcdiff, status);
     else
-        decode_span_t<WRITE, false>(hs, s, p, limit, phase, nslots, nb, pos, total_slots, it, coef, dcdiff, status);
+        decode_span_t<WRITE, false>(hs, s, p, limit, end_bits, phase, nslots, nb, pos, total_slots, it, coef, dcdiff, status);
 }
 
 // ---- 3. DC differences -> DC values
@@ -575,7 +592,7 @@ __global__ void __launch_bounds__(kHuffThreads, LP_HUFF_MIN_CTAS)
     for (uint32_t i = tid; i < nsub; i += kHuffThreads) {
         uint32_t p = i * kSubBits, phase = 0, n = 0;
         const uint32_t limit = min((i + 1) * kSubBits, total_bits);
-        decode_span<false>(hs, s, p, limit, phase, n, nb, 0, 0, nullptr, nullptr, nullptr, nullptr);
+        decode_span<false>(hs, s, p, limit, total_bits, phase, n, nb, 0, 0, nullptr, nullptr, nullptr, nullptr);
         st[i] = SubState{p, phase};
         ns[i] = n;
     }
@@ -602,7 +619,7 @@ __global__ void __launch_bounds__(kHuffThreads, LP_HUFF_MIN_CTAS)
             const SubState old = st[i];
             uint32_t p = in.p, phase = in.phase, n = 0;
             const uint32_t limit = min((i + 1) * kSubBits, total_bits);
-            if (p < limit) decode_span<false>(hs, s, p, limit, phase, n, nb, 0, 0, nullptr, nullptr, nullptr, nullptr);
+            if (p < limit) decode_span<false>(hs, s, p, limit, total_bits, phase, n, nb, 0, 0, nullptr, nullptr, nullptr, nullptr);
             ns[i] = n;  // slots consumed depend on the entry state even when the exit state does not
             if (p != old.p || phase != old.phase) {
                 // only an exit-state change can affect the right neighbour
@@ -642,7 +659,7 @@ __global__ void __launch_bounds__(kHuffThreads, LP_HUFF_MIN_CTAS)
                 (uint32_t)(pos % ((uint64_t)nb * 64)) != ((phase >> 6) * 64 + (phase & 63)))
                 status = -3;
             if (!status && p < limit)
-                decode_span<true>(hs, s, p, limit, phase, n, nb, pos, total_slots, &it, coef, dcdiff, &status);
+                decode_span<true>(hs, s, p, limit, total_bits, phase, n, nb, pos, total_slots, &it, coef, dcdiff, &status);
             if (status) s_status = status;
         }
     }
