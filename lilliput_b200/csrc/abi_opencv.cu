@@ -849,19 +849,17 @@ bool opencv_encoder_write(opencv_encoder e, const opencv_mat src, const int* opt
         return false;
     }
     int quality = 95;  // OpenCV's default
+    bool progressive = false;
     for (size_t i = 0; i + 1 < opt_len; i += 2) {
         if (opt[i] == CV_IMWRITE_JPEG_QUALITY) quality = std::min(std::max(opt[i + 1], 0), 100);
-        if (opt[i] == CV_IMWRITE_JPEG_PROGRESSIVE && opt[i + 1]) {
-            fprintf(stderr, "[lilliput_b200] progressive JPEG output is not supported\n");
-            return false;
-        }
+        if (opt[i] == CV_IMWRITE_JPEG_PROGRESSIVE) progressive = opt[i + 1] != 0;
     }
     if (ensure_dev(s)) return false;
     cudaStream_t st = thread_stream();
     const int W = s->cols, H = s->rows, C = s->channels();
     // worst case is bounded by the raw size for sane inputs; give generous room
     const size_t cap = round_up((size_t)W * H * 3 + 4096, (size_t)256);
-    const size_t scratch_bytes = jpeg_encode_scratch_bytes(W, H, C, 1, cap);
+    const size_t scratch_bytes = jpeg_encode_scratch_bytes(W, H, C, 1, cap, progressive);
     uint8_t* buf = nullptr;
     if (cudaMallocAsync(&buf, scratch_bytes + cap + 256, st) != cudaSuccess) return false;
     JpegEncodeBatch b;
@@ -877,6 +875,7 @@ bool opencv_encoder_write(opencv_encoder e, const opencv_mat src, const int* opt
     b.out_cap = cap;
     b.out_len = reinterpret_cast<uint32_t*>(buf + scratch_bytes);
     b.scratch = buf;
+    b.progressive = progressive;
     bool ok = jpeg_encode_launch(b, st, nullptr) == LP_OK;
     uint32_t n = 0;
     if (ok) ok = cudaMemcpyAsync(&n, b.out_len, 4, cudaMemcpyDeviceToHost, st) == cudaSuccess && !sync_stream();

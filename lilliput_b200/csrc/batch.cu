@@ -22,6 +22,7 @@ using namespace lp;
 
 struct lp_batch {
     lp_batch_config cfg;
+    bool progressive = false;        // JPEG output is progressive (lp_xbatch with JpegProgressive)
     cudaStream_t st = nullptr;       // kernels
     cudaStream_t st_h2d = nullptr;   // input copies (pipelined transform)
     cudaStream_t st_d2h = nullptr;   // output copies (pipelined transform)
@@ -114,20 +115,21 @@ static void batch_free(lp_batch* b) {
 
 namespace lp {
 lp_batch* batch_create_in(const lp_batch_config* cfg, uint8_t* dev_arena, size_t dev_bytes, uint8_t* host_arena,
-                          size_t host_bytes);
+                          size_t host_bytes, bool progressive_jpeg = false);
 }
 extern "C" lp_batch* lp_batch_create(const lp_batch_config* cfg) { return lp::batch_create_in(cfg, nullptr, 0, nullptr, 0); }
 
 // dev_arena / host_arena non-null: every device / pinned buffer is carved from them (nothing is allocated or
-// freed by the context); returns nullptr when they are too small.
+// freed by the context); returns nullptr when they are too small.  progressive_jpeg: write progressive JPEG files.
 lp_batch* lp::batch_create_in(const lp_batch_config* cfg, uint8_t* dev_arena, size_t dev_bytes, uint8_t* host_arena,
-                              size_t host_bytes) {
+                              size_t host_bytes, bool progressive_jpeg) {
     if (!cfg || cfg->max_images < 1 || cfg->src_width < 1 || cfg->src_height < 1) return nullptr;
     if (ensure_device()) return nullptr;
     DeviceGuard dev_guard(cfg->device);
     if (!dev_guard.ok) return nullptr;
     lp_batch* b = new lp_batch;
     b->cfg = *cfg;
+    b->progressive = progressive_jpeg;
     b->owns_mem = dev_arena == nullptr;
     size_t dev_used = 0, host_used = 0;
     b->W = cfg->src_width;
@@ -194,7 +196,7 @@ lp_batch* lp::batch_create_in(const lp_batch_config* cfg, uint8_t* dev_arena, si
     BALLOC(b->d_planes, (size_t)b->chunk * max_blocks * 64);
     BALLOC(b->d_frames, (size_t)b->chunk * b->frame_bytes + 256);
     BALLOC(b->d_resized, N * b->resized_bytes + 256);
-    BALLOC(b->d_enc_scratch, jpeg_encode_scratch_bytes(b->out_w, b->out_h, 3, b->chunk, cfg->out_cap));
+    BALLOC(b->d_enc_scratch, jpeg_encode_scratch_bytes(b->out_w, b->out_h, 3, b->chunk, cfg->out_cap, b->progressive));
     BALLOC(b->d_clean, cfg->max_in_bytes + 64 * N + 4096);
     b->state_cap = (cfg->max_in_bytes / 128 + 2 * N + 16) * 2;
     BALLOC(b->d_states, b->state_cap * 8);
@@ -506,6 +508,7 @@ static int batch_launch_chunk(lp_batch* b, int i0, int cnt, cudaStream_t st, cud
     e.out_cap = b->cfg.out_cap;
     e.out_len = b->d_out_len + i0;
     e.scratch = b->d_enc_scratch;
+    e.progressive = b->progressive;
     rc = jpeg_encode_launch(e, st, ev ? ev[4] : nullptr);
     if (rc) return rc;
     // the encoded bytes leave packed: slots are out_cap (64 KB) apart but hold a few KB each, so a compaction

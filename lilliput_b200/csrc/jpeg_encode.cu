@@ -1,6 +1,6 @@
-// jpeg_encode.cu -- baseline JPEG encode on sm_90a: BGR->YCbCr + 4:2:0 downsample + ISLOW FDCT
+// jpeg_encode.cu -- JPEG encode on sm_90a: BGR->YCbCr + 4:2:0 downsample + ISLOW FDCT
 // + quantisation, then Huffman coding with a per-image prefix sum over MCU bit lengths,
-// bit packing and 0xFF byte stuffing.
+// bit packing and 0xFF byte stuffing.  Baseline, or progressive (T.81 Annex G) when asked.
 //
 // Replaces: opencv_encoder_write for ".jpeg"/".jpg" (ref opencv.cpp:185-194), i.e. what
 // cv::ImageEncoder::write asks of libjpeg-turbo 3.1.0 defaults.  Arithmetic and bitstream
@@ -13,6 +13,8 @@
 //                            store int16 coefficients in zig-zag order.
 //   jpeg_entropy_kernel      one CTA per image: per-MCU bit counts -> block scan -> packed
 //                            bitstream (atomicOr at MCU boundaries) -> stuffed bytes + header/EOI.
+//   jpeg_prog_entropy_kernel one CTA per image, progressive output: the scans of jpeg_simple_progression's
+//                            script in turn, each with its own optimal Huffman tables (jpeg_prog_core.h).
 #include <cstring>
 #include <map>
 #include <mutex>
@@ -20,6 +22,7 @@
 #include <vector>
 
 #include "common.cuh"
+#include "jpeg_prog_core.h"
 #include "kernels.cuh"
 
 namespace lp {
@@ -486,6 +489,47 @@ __device__ __forceinline__ uint32_t block_exclusive_scan(uint32_t v, uint32_t* t
     return base + inc - v;
 }
 
+// 0xFF byte stuffing (T.81 F.1.2.3) of nbytes packed big-endian bytes from words into body; each thread owns 16 bytes
+// per round.  Returns the stuffed length, or -1 where it does not fit in room.  kEntThreads threads; s_carry (shared)
+// is 0 on entry.  This is phase 4 of jpeg_entropy_kernel, which keeps its own copy so that the baseline kernel's code
+// is unchanged by the progressive path.
+__device__ __forceinline__ long long stuff_bytes(const uint32_t* words, uint32_t nbytes, uint8_t* body, size_t room,
+                                                uint32_t* warp_sums, uint32_t& s_carry) {
+    const int tid = threadIdx.x;
+    bool overflow = false;
+    for (uint32_t base = 0; base < nbytes; base += kEntThreads * 16) {
+        const uint32_t b0 = base + tid * 16;
+        uint32_t w[4] = {0, 0, 0, 0};
+        uint32_t cnt = 0, have = 0;
+        if (b0 < nbytes) {
+            have = min(16u, nbytes - b0);
+#pragma unroll
+            for (int i = 0; i < 4; i++) w[i] = words[(b0 >> 2) + i];  // reads <= nwords (zeroed slack)
+            for (uint32_t i = 0; i < have; i++)
+                cnt += ((w[i >> 2] >> (24 - 8 * (i & 3))) & 0xff) == 0xff;
+        }
+        uint32_t total;
+        const uint32_t ex = block_exclusive_scan(cnt, &total, warp_sums);
+        size_t o = (size_t)b0 + s_carry + ex;
+        if (b0 < nbytes) {
+            if (o + have + cnt > room) {
+                overflow = true;
+            } else {
+                for (uint32_t i = 0; i < have; i++) {
+                    const uint8_t v = (w[i >> 2] >> (24 - 8 * (i & 3))) & 0xff;
+                    body[o++] = v;
+                    if (v == 0xff) body[o++] = 0;
+                }
+            }
+        }
+        __syncthreads();
+        if (tid == 0) s_carry += total;
+        __syncthreads();
+    }
+    if (__syncthreads_or(overflow)) return -1;
+    return (long long)nbytes + s_carry;
+}
+
 __global__ void __launch_bounds__(kEntThreads)
     jpeg_entropy_kernel(const int16_t* coef_all, EncGeom g, const EncConst* ec, uint32_t* mcu_bits_all,
                         uint32_t* words_all, size_t words_per_img, uint8_t* out_all, size_t out_cap,
@@ -605,6 +649,163 @@ __global__ void __launch_bounds__(kEntThreads)
     }
 }
 
+// ------------------------------------------------------------------ progressive entropy coding
+
+// jpeg_prog_core.h's table builder on one warp
+struct WarpLanes {
+    __device__ int lane() const { return threadIdx.x & 31; }
+    __device__ int lanes() const { return 32; }
+    __device__ void sync() const { __syncwarp(); }
+    __device__ uint64_t min(uint64_t v) const {
+#pragma unroll
+        for (int o = 16; o; o >>= 1) {
+            const uint64_t t = __shfl_xor_sync(0xffffffffu, v, o);
+            v = t < v ? t : v;
+        }
+        return v;
+    }
+};
+struct SharedCounts {
+    uint32_t (*hist)[257];
+    __device__ void sym(int t, int s) { atomicAdd(&hist[t][s], 1u); }
+    __device__ void bits(uint32_t, int) {}
+};
+struct AtomicOrWord {
+    __device__ void operator()(uint32_t* w, uint32_t v) const { atomicOr(w, v); }
+};
+
+// One CTA per image writes the whole progressive file: the baseline frame header with SOF2, then each scan of the
+// script in turn -- symbol counts over the scan's blocks, EOB runs resolved by one thread, optimal tables built by
+// warp 0, per-block bit counts and a block scan for offsets, bits packed as in jpeg_entropy_kernel, 1-padding and
+// stuffing straight after the scan's DHT/SOS -- then EOI.  summ / runs: per-block scratch, reused by every scan.
+__global__ void __launch_bounds__(kEntThreads)
+    jpeg_prog_entropy_kernel(const int16_t* coef_all, EncGeom g, const EncConst* ec, uint32_t* summ_all,
+                             uint32_t* runs_all, uint32_t* words_all, size_t words_per_img, uint8_t* out_all,
+                             size_t out_cap, uint32_t* out_len) {
+    __shared__ uint32_t hist[2][257];
+    __shared__ uint32_t huff[2][256];
+    __shared__ int tbl_work[2][257];
+    __shared__ uint8_t bits[2][17], vals[2][256];
+    __shared__ uint32_t warp_sums[kEntThreads / 32];
+    __shared__ uint32_t s_carry;
+    __shared__ int s_fail;
+    const int img = blockIdx.x;
+    const int tid = threadIdx.x;
+    const bool gray = g.blocks_per_mcu == 1;
+    const jprog::Geom pg{g.mcus_x, g.mcus_y, g.blocks_per_mcu, g.ybw, g.ybh};
+    const size_t nblk = (size_t)g.mcus_x * g.mcus_y * g.blocks_per_mcu;
+    const int16_t* coef = coef_all + (size_t)img * nblk * 64;
+    uint32_t* summ = summ_all + (size_t)img * nblk;
+    uint32_t* runs = runs_all + (size_t)img * nblk;
+    uint32_t* words = words_all + (size_t)img * words_per_img;
+    uint8_t* out = out_all + (size_t)img * out_cap;
+    const int flen = jprog::frame_len(gray);
+    if (out_cap < (size_t)flen + 2) {
+        if (tid == 0) out_len[img] = 0;
+        return;
+    }
+    const int sof = jprog::sof_type_at(gray);
+    for (int i = tid; i < flen; i += kEntThreads) out[i] = i == sof ? 0xC2 : ec->header[i];
+    if (tid == 0) s_fail = 0;
+    size_t pos = flen;
+    const int nscans = gray ? jprog::kGrayScans : jprog::kColorScans;
+    for (int si = 0; si < nscans; si++) {
+        const jprog::Scan s = jprog::scan_of(gray, si);
+        const int nb = jprog::scan_blocks(pg, s);
+        const int nt = jprog::scan_tables(gray, s);
+        for (int i = tid; i < 2 * 257; i += kEntThreads) hist[i / 257][i % 257] = 0;
+        __syncthreads();
+        SharedCounts cnt{hist};
+        for (int i = tid; i < nb; i += kEntThreads) {
+            summ[i] = jprog::code_block(coef, pg, s, i, 0, cnt);
+            runs[i] = 0;
+        }
+        __syncthreads();
+        if (s.Ss && tid == 0)
+            jprog::resolve_runs(summ, nb, [&](int start, int run) {
+                runs[start] = (uint32_t)run;
+                hist[0][(jprog::nbits((unsigned)run) - 1) << 4]++;
+            });
+        __syncthreads();
+        if (tid < 32) {
+            for (int t = 0; t < nt; t++) {
+                const int n = jprog::gen_optimal_table(WarpLanes{}, hist[t], tbl_work[0], tbl_work[1], bits[t], vals[t]);
+                if (tid == 0) {
+                    if (n < 0) s_fail = 1;
+                    jprog::make_codes(bits[t], vals[t], huff[t]);
+                }
+                __syncwarp();
+            }
+            if (tid == 0) {
+                const int hl = jprog::scan_header_len(gray, s, bits);
+                if (pos + hl + 2 > out_cap) {
+                    s_fail = 1;
+                } else {
+                    jprog::put_scan_header(out + pos, gray, s, bits, vals);
+                    s_carry = (uint32_t)hl;
+                }
+            }
+        }
+        __syncthreads();
+        if (s_fail) {
+            if (tid == 0) out_len[img] = 0;
+            return;
+        }
+        pos += s_carry;
+        __syncthreads();
+        if (tid == 0) s_carry = 0;
+        __syncthreads();
+        // bit offset of every block
+        for (int base = 0; base < nb; base += kEntThreads) {
+            const int i = base + tid;
+            jprog::CountBits c{huff[0], huff[1], 0};
+            if (i < nb) jprog::code_block(coef, pg, s, i, (int)runs[i], c);
+            uint32_t total;
+            const uint32_t ex = block_exclusive_scan(c.total, &total, warp_sums);
+            if (i < nb) summ[i] = s_carry + ex;
+            __syncthreads();
+            if (tid == 0) s_carry += total;
+            __syncthreads();
+        }
+        const uint32_t total_bits = s_carry;
+        const uint32_t nbytes = (total_bits + 7) >> 3;
+        const uint32_t nwords = (nbytes + 3) >> 2;
+        const size_t room = out_cap - pos - 2;
+        if ((size_t)nbytes > room || nwords + 1 > words_per_img) {  // cannot fit even unstuffed
+            if (tid == 0) out_len[img] = 0;
+            return;
+        }
+        for (uint32_t i = tid; i <= nwords; i += kEntThreads) words[i] = 0;
+        __syncthreads();
+        for (int i = tid; i < nb; i += kEntThreads) {
+            jprog::BitPacker<AtomicOrWord> p(words, summ[i], AtomicOrWord{});
+            jprog::WriteBits<jprog::BitPacker<AtomicOrWord>> e{huff[0], huff[1], &p};
+            jprog::code_block(coef, pg, s, i, (int)runs[i], e);
+            p.finish();
+        }
+        __syncthreads();
+        if (tid == 0 && (total_bits & 7)) {  // pad the last byte with 1-bits
+            const uint32_t padn = 8 - (total_bits & 7);
+            const uint32_t at = total_bits & 31;
+            atomicOr(&words[total_bits >> 5], ((1u << padn) - 1) << (32 - at - padn));
+        }
+        if (tid == 0) s_carry = 0;
+        __syncthreads();
+        const long long stuffed = stuff_bytes(words, nbytes, out + pos, room, warp_sums, s_carry);
+        if (stuffed < 0) {
+            if (tid == 0) out_len[img] = 0;
+            return;
+        }
+        pos += (size_t)stuffed;
+        __syncthreads();
+    }
+    if (tid == 0) {
+        out[pos] = 0xFF;
+        out[pos + 1] = 0xD9;
+        out_len[img] = (uint32_t)(pos + 2);
+    }
+}
+
 // ------------------------------------------------------------------ launcher
 
 static EncGeom make_geom(int W, int H, int C) {
@@ -625,13 +826,19 @@ static EncGeom make_geom(int W, int H, int C) {
 
 static size_t words_per_image(size_t out_cap) { return (out_cap + 3) / 4 + 8; }
 
-size_t jpeg_encode_scratch_bytes(int W, int H, int C, int n, size_t out_cap) {
+// progressive output: per-block summaries / offsets and EOB run starts, one uint32 each
+static size_t prog_block_bytes(const EncGeom& g) {
+    return round_up((size_t)g.mcus_x * g.mcus_y * g.blocks_per_mcu * sizeof(uint32_t), (size_t)256);
+}
+
+size_t jpeg_encode_scratch_bytes(int W, int H, int C, int n, size_t out_cap, bool progressive) {
     EncGeom g = make_geom(W, H, C);
     const size_t nmcu = (size_t)g.mcus_x * g.mcus_y;
     size_t coef = nmcu * g.blocks_per_mcu * 64 * sizeof(int16_t);
     size_t bits = round_up(nmcu * sizeof(uint32_t), (size_t)256);
     size_t words = round_up(words_per_image(out_cap) * sizeof(uint32_t), (size_t)256);
-    return (size_t)n * (round_up(coef, (size_t)256) + bits + words);
+    size_t prog = progressive ? 2 * prog_block_bytes(g) : 0;
+    return (size_t)n * (round_up(coef, (size_t)256) + bits + words + prog);
 }
 
 int jpeg_encode_launch(const JpegEncodeBatch& b, cudaStream_t st, cudaEvent_t ev_after_transform) {
@@ -667,8 +874,16 @@ int jpeg_encode_launch(const JpegEncodeBatch& b, cudaStream_t st, cudaEvent_t ev
     g_launches++;
     LP_CUDA_OK(cudaGetLastError());
     if (ev_after_transform) LP_CUDA_OK(cudaEventRecord(ev_after_transform, st));
-    jpeg_entropy_kernel<<<b.n, kEntThreads, 0, st>>>(coef, g, ec, mcu_bits, words, wpi, b.out, b.out_cap,
-                                                    b.out_len, header_len);
+    if (b.progressive) {
+        const size_t words_bytes = round_up(wpi * sizeof(uint32_t), (size_t)256);
+        uint32_t* summ = reinterpret_cast<uint32_t*>(s + (size_t)b.n * (coef_bytes + bits_bytes + words_bytes));
+        uint32_t* runs = summ + (size_t)b.n * prog_block_bytes(g) / sizeof(uint32_t);
+        jpeg_prog_entropy_kernel<<<b.n, kEntThreads, 0, st>>>(coef, g, ec, summ, runs, words, wpi, b.out, b.out_cap,
+                                                             b.out_len);
+    } else {
+        jpeg_entropy_kernel<<<b.n, kEntThreads, 0, st>>>(coef, g, ec, mcu_bits, words, wpi, b.out, b.out_cap,
+                                                        b.out_len, header_len);
+    }
     g_launches++;
     LP_CUDA_OK(cudaGetLastError());
     return LP_OK;

@@ -250,8 +250,10 @@ struct JpegEncodeBatch {
     uint32_t* out_len;       // device, n (0 on overflow)
     // scratch (device), sized by jpeg_encode_scratch_bytes
     void* scratch;
+    // progressive output (libjpeg-turbo's jpeg_simple_progression script, optimal tables per scan)
+    bool progressive = false;
 };
-size_t jpeg_encode_scratch_bytes(int width, int height, int channels, int n, size_t out_cap);
+size_t jpeg_encode_scratch_bytes(int width, int height, int channels, int n, size_t out_cap, bool progressive = false);
 int jpeg_encode_launch(const JpegEncodeBatch& b, cudaStream_t st, cudaEvent_t ev_after_transform);
 
 // ---- webp_encode.cu -------------------------------------------------------------------------

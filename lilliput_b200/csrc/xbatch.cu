@@ -13,7 +13,7 @@
 //        GIF   -> every frame of every animation: LZW (one warp per frame), per-pixel compositor over the
 //                 frame sequence (gif_decode.cu), resize of every composited canvas
 //      and the sinks: JPEG (jpeg_encode.cu), lossy WebP still / animation (webp_encode.cu);
-//   3. anything the grid path does not cover (progressive JPEG, EXIF-rotated sources, ICC profiles to carry,
+//   3. anything the grid path does not cover (progressive JPEG sources, EXIF-rotated sources, ICC profiles to carry,
 //      lossless WebP output, PNG / GIF output ...) and any item whose grid stage fails goes through
 //      lp_transform on a worker thread -- still this library's device kernels, one image per call -- so the
 //      status and bytes of EVERY item are what lp_transform would have returned.
@@ -41,7 +41,7 @@ using namespace lp;
 
 namespace lp {
 lp_batch* batch_create_in(const lp_batch_config* cfg, uint8_t* dev_arena, size_t dev_bytes, uint8_t* host_arena,
-                          size_t host_bytes);
+                          size_t host_bytes, bool progressive_jpeg);
 }  // namespace lp
 
 namespace {
@@ -114,6 +114,7 @@ struct lp_xbatch {
     lp_image_options opt;
     Sink sink = S_NONE;
     int quality = 0;
+    bool progressive = false;  // S_JPEG: progressive files (JpegProgressive)
     std::vector<XItem> items;
     std::vector<int> fallback;
     std::mutex fb_mu;
@@ -249,7 +250,7 @@ static void sink_encode(lp_xbatch* X, Lane& L, Bump& bump, const std::vector<int
         uint32_t* d_len = bump.take<uint32_t>((size_t)n * 4);
         uint8_t* d_packed = bump.take<uint8_t>((size_t)n * slot + 16);
         auto* d_off = bump.take<unsigned long long>((size_t)(n + 1) * 8);
-        void* scratch = bump.take<uint8_t>(jpeg_encode_scratch_bytes(ow, oh, ch, n, slot));
+        void* scratch = bump.take<uint8_t>(jpeg_encode_scratch_bytes(ow, oh, ch, n, slot, X->progressive));
         if (!d_out || !d_len || !d_packed || !d_off || !scratch) {
             failed->insert(failed->end(), idx.begin(), idx.end());
             return;
@@ -269,6 +270,7 @@ static void sink_encode(lp_xbatch* X, Lane& L, Bump& bump, const std::vector<int
         e.out_cap = slot;
         e.out_len = d_len;
         e.scratch = scratch;
+        e.progressive = X->progressive;
         int rc = jpeg_encode_launch(e, L.st, nullptr);
         if (!rc) rc = compact_launch(d_out, slot, d_len, (uint32_t)slot, n, d_packed, d_off, L.st);
         std::vector<unsigned long long> off((size_t)n + 1);
@@ -738,7 +740,7 @@ static void run_jpeg(lp_xbatch* X, Lane& L, const std::vector<int>& idx) {
     int chunk = (int)std::min<long>(fit, 3L * std::max(slots, 1));
     if (slots > 0 && chunk > slots) chunk = chunk / slots * slots;
     c.chunk = std::max(1, std::min(chunk, n));
-    lp_batch* b = batch_create_in(&c, L.dev, L.dev_bytes, L.host, L.host_bytes);
+    lp_batch* b = batch_create_in(&c, L.dev, L.dev_bytes, L.host, L.host_bytes, X->progressive);
     if (!b) {
         for (int i : idx) push_fallback(X, i);
         return;
@@ -902,10 +904,11 @@ extern "C" int lp_xbatch_transform(lp_xbatch* X, const uint8_t* const* in, const
     std::string ext = opt->file_type ? opt->file_type : "";
     for (auto& c : ext) c = (char)tolower((unsigned char)c);
     X->sink = S_NONE;
+    X->progressive = false;
     if (ext == ".jpeg" || ext == ".jpg") {
         X->sink = S_JPEG;
         X->quality = option_value(*opt, CV_IMWRITE_JPEG_QUALITY, 95);  // OpenCV's default
-        if (option_value(*opt, 2 /* JpegProgressive */, 0)) X->sink = S_NONE;
+        X->progressive = option_value(*opt, CV_IMWRITE_JPEG_PROGRESSIVE, 0) != 0;
     } else if (ext == ".webp") {
         const int q = option_value(*opt, CV_IMWRITE_WEBP_QUALITY, 100);
         X->quality = q < 1 ? 1 : q;
