@@ -227,8 +227,8 @@ static int decode_jpeg_into(const Decoder* d, Mat* m) {
         it.td[c] = h.comp[c].td;
         it.ta[c] = h.comp[c].ta;
     }
-    uint32_t plane_bytes = 0;
-    const uint32_t blocks = jpeg_item_set_window(&it, 0, 0, h.width, h.height, false, &plane_bytes);  // whole image
+    uint32_t tiles = 0;
+    const uint32_t blocks = jpeg_item_set_window(&it, 0, 0, h.width, h.height, false, &tiles);  // whole image
     it.frame_channels = h.ncomp == 1 ? 1 : 3;
     JpegHuffSet hs;
     jpeg_build_huff_set(h, &hs);
@@ -239,21 +239,19 @@ static int decode_jpeg_into(const Decoder* d, Mat* m) {
     const size_t sets_b = round_up(sizeof(JpegHuffSet) * (size_t)(h.multiscan ? nsets : 1), (size_t)256);
     const size_t scans_b = round_up(sizeof(JpegScanDesc) * (size_t)nscans + 16, (size_t)256);
     const size_t coef_bytes = round_up((size_t)blocks * 64 * sizeof(int16_t), (size_t)256);
-    const size_t plane_b = round_up((size_t)plane_bytes, (size_t)256);
     const bool parallel = h.restart_interval == 0 && !h.multiscan;
     const size_t clean_b = parallel ? round_up(huff_clean_bytes(h.scan_length), (size_t)256) : 0;
     const size_t states_b = parallel ? round_up(2 * huff_nsub(h.scan_length) * 8, (size_t)256) : 0;
     const size_t nslots_b = parallel ? round_up(2 * huff_nsub(h.scan_length) * 4, (size_t)256) : 0;
     const size_t dcdiff_b = parallel ? round_up((size_t)total_blocks * 2, (size_t)256) : 0;
-    const size_t total = 1024 + sets_b + scan_bytes + coef_bytes + plane_b + clean_b + states_b + nslots_b +
+    const size_t total = 1024 + sets_b + scan_bytes + coef_bytes + clean_b + states_b + nslots_b +
                          dcdiff_b + scans_b;
     LP_CUDA_OK(cudaMallocAsync(&scratch, total, st));
     JpegDecodeItem* d_item = reinterpret_cast<JpegDecodeItem*>(scratch);
     JpegHuffSet* d_hs = reinterpret_cast<JpegHuffSet*>(scratch + 1024);
     uint8_t* d_scan = scratch + 1024 + sets_b;
     int16_t* d_coef = reinterpret_cast<int16_t*>(d_scan + scan_bytes);
-    uint8_t* d_planes = reinterpret_cast<uint8_t*>(d_coef) + coef_bytes;
-    uint8_t* d_clean = d_planes + plane_b;
+    uint8_t* d_clean = reinterpret_cast<uint8_t*>(d_coef) + coef_bytes;
     uint8_t* d_states = d_clean + clean_b;
     uint8_t* d_nslots = d_states + states_b;
     uint8_t* d_dcdiff = d_nslots + nslots_b;
@@ -272,13 +270,10 @@ static int decode_jpeg_into(const Decoder* d, Mat* m) {
     b.tables = d_hs;
     b.scan = d_scan;
     b.coef = d_coef;
-    b.planes = d_planes;
     b.frames = m->dptr();
     b.n = 1;
     b.coef_elems_total = (size_t)blocks * 64;
-    b.max_blocks_per_image = (int)blocks;
-    b.max_width = h.width;
-    b.max_height = h.height;
+    b.max_tiles_per_image = (int)tiles;
     b.use_parallel_huffman = parallel;
     b.clean = d_clean;
     b.states = d_states;

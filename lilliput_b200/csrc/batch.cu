@@ -39,7 +39,7 @@ struct lp_batch {
     int crop_x = 0, crop_y = 0, crop_w = 0, crop_h = 0;
     // per-image scratch layout, fixed by the first image staged into this context
     bool layout_known = false;
-    uint32_t blocks = 0, plane_bytes = 0;
+    uint32_t blocks = 0;
     size_t max_blocks_alloc = 0;
     size_t frame_bytes = 0, resized_bytes = 0;
     // device
@@ -47,7 +47,6 @@ struct lp_batch {
     JpegDecodeItem* d_items = nullptr;
     JpegHuffSet* d_tables = nullptr;
     int16_t* d_coef = nullptr;
-    uint8_t* d_planes = nullptr;
     uint8_t* d_frames = nullptr;
     uint8_t* d_resized = nullptr;
     uint8_t* d_enc_scratch = nullptr;
@@ -73,7 +72,7 @@ struct lp_batch {
     uint32_t* h_out_len = nullptr;  // pinned
     unsigned long long* h_off = nullptr;  // pinned + device-mapped: packed offsets, (cnt + 1) per chunk at [i0 + chunk ordinal]
     struct ChunkLayout {
-        uint32_t blocks = 0, plane_bytes = 0, total_blocks = 0;
+        uint32_t blocks = 0, tiles = 0, total_blocks = 0;
         int ordinal = 0;
         std::vector<uint2> rst_work;  // (image in chunk, restart interval) of the chunk's DRI images
         uint2* d_rst_work = nullptr;  // stream-ordered allocation, freed after the chunk's launches
@@ -96,7 +95,7 @@ static void batch_free(lp_batch* b) {
         if (kv.second.d_rst_work) cudaFree(kv.second.d_rst_work);
     if (b->owns_mem) {
     cudaFree(b->d_scan); cudaFree(b->d_items); cudaFree(b->d_tables); cudaFree(b->d_coef);
-    cudaFree(b->d_planes); cudaFree(b->d_frames); cudaFree(b->d_resized); cudaFree(b->d_enc_scratch);
+    cudaFree(b->d_frames); cudaFree(b->d_resized); cudaFree(b->d_enc_scratch);
     cudaFree(b->d_out); cudaFree(b->d_out_len);
     cudaFree(b->d_clean); cudaFree(b->d_states); cudaFree(b->d_nslots); cudaFree(b->d_dcdiff);
     if (b->h_out) cudaFreeHost(b->h_out);
@@ -193,7 +192,6 @@ lp_batch* lp::batch_create_in(const lp_batch_config* cfg, uint8_t* dev_arena, si
     b->max_tables = (int)N;
     BALLOC(b->d_tables, (size_t)b->max_tables * sizeof(JpegHuffSet));
     BALLOC(b->d_coef, (size_t)b->chunk * max_blocks * 64 * sizeof(int16_t));
-    BALLOC(b->d_planes, (size_t)b->chunk * max_blocks * 64);
     BALLOC(b->d_frames, (size_t)b->chunk * b->frame_bytes + 256);
     BALLOC(b->d_resized, N * b->resized_bytes + 256);
     BALLOC(b->d_enc_scratch, jpeg_encode_scratch_bytes(b->out_w, b->out_h, 3, b->chunk, cfg->out_cap, b->progressive));
@@ -305,7 +303,7 @@ static int batch_layout_chunk(lp_batch* b, const uint8_t* const* in, const size_
 // batch may mix 4:2:0 / 4:2:2 / 4:4:4 files in any order (the per-chunk scratch is sized for 4:4:4 anyway).
 static int batch_parse_chunk(lp_batch* b, const uint8_t* const* in, const size_t* in_len, int i0, int cnt, int ordinal) {
     std::vector<JpegHeader> hdr((size_t)cnt);
-    std::vector<uint32_t> blocks_of((size_t)cnt, 0), planes_of((size_t)cnt, 0), total_of((size_t)cnt, 0);
+    std::vector<uint32_t> blocks_of((size_t)cnt, 0), tiles_of((size_t)cnt, 0), total_of((size_t)cnt, 0);
     auto pass1 = [&](int k0, int k1) {
         for (int k = k0; k < k1; k++) {
             JpegHeader& h = hdr[k - i0];
@@ -333,13 +331,13 @@ static int batch_parse_chunk(lp_batch* b, const uint8_t* const* in, const size_t
                 }
                 it.frame_channels = 3;
                 // decode only what Fit will read: the crop window (+ the chroma-upsampling margin)
-                uint32_t plane_bytes = 0;
+                uint32_t tiles = 0;
                 const uint32_t blocks = jpeg_item_set_window(&it, b->crop_x, b->crop_y, b->crop_x + b->crop_w,
-                                                             b->crop_y + b->crop_h, true, &plane_bytes);
+                                                             b->crop_y + b->crop_h, true, &tiles);
                 blocks_of[k - i0] = blocks;
-                planes_of[k - i0] = plane_bytes;
+                tiles_of[k - i0] = tiles;
                 total_of[k - i0] = total_blocks;
-                if (blocks > b->max_blocks_alloc || total_blocks > b->max_blocks_alloc || plane_bytes > b->max_blocks_alloc * 64)
+                if (blocks > b->max_blocks_alloc || total_blocks > b->max_blocks_alloc)
                     rc = LP_ERR_UNSUPPORTED;  // beyond what the context was created for
             }
             b->parse_status[k] = rc;
@@ -363,7 +361,7 @@ static int batch_parse_chunk(lp_batch* b, const uint8_t* const* in, const size_t
         if (b->parse_status[k]) continue;
         const JpegDecodeItem& it = b->items[k];
         lay.blocks = std::max(lay.blocks, blocks_of[k - i0]);
-        lay.plane_bytes = std::max(lay.plane_bytes, planes_of[k - i0]);
+        lay.tiles = std::max(lay.tiles, tiles_of[k - i0]);
         lay.total_blocks = std::max(lay.total_blocks, total_of[k - i0]);
         if (!b->layout_known) {  // the decoded window depends on the geometry only, which the context fixes
             b->win_w = it.win_w;
@@ -373,7 +371,6 @@ static int batch_parse_chunk(lp_batch* b, const uint8_t* const* in, const size_t
             b->layout_known = true;
         }
     }
-    lay.plane_bytes = round_up(lay.plane_bytes, 256u);
     b->blocks = std::max(b->blocks, lay.blocks);
     b->total_blocks = std::max(b->total_blocks, lay.total_blocks);
     b->chunk_layout[i0] = lay;
@@ -405,7 +402,6 @@ static int batch_parse_chunk(lp_batch* b, const uint8_t* const* in, const size_t
         }
         it.scan_off = b->file_dev_off[k] + hdr[k - i0].scan_offset;
         it.coef_off = (uint64_t)slot * lay.blocks * 64;
-        it.plane_off = (uint64_t)slot * lay.plane_bytes;
         it.frame_off = (uint64_t)slot * b->frame_bytes;
         it.dcdiff_off = (uint64_t)slot * lay.total_blocks;
         it.clean_off = b->clean_off;
@@ -467,13 +463,10 @@ static int batch_launch_chunk(lp_batch* b, int i0, int cnt, cudaStream_t st, cud
     d.tables = b->d_tables;
     d.scan = b->d_scan;
     d.coef = b->d_coef;
-    d.planes = b->d_planes;
     d.frames = b->d_frames;
     d.n = cnt;
     d.coef_elems_total = (size_t)cnt * lay.blocks * 64;
-    d.max_blocks_per_image = (int)lay.blocks;
-    d.max_width = b->win_w;
-    d.max_height = b->win_h;
+    d.max_tiles_per_image = (int)lay.tiles;
     d.dcdiff = b->d_dcdiff;
     d.use_parallel_huffman = b->parallel_huffman;
     d.clean = b->d_clean;

@@ -10,9 +10,10 @@
 //   jpeg_huff_decode_kernel   entropy-coded segment -> quantised coefficients (int16, natural
 //                             order, zero-initialised buffer).  Bit-serial by nature; this
 //                             first version runs one stream per thread.
-//   jpeg_idct_kernel          one thread per 8x8 block: dequantise, two 1-D passes in
-//                             registers, 8-byte row stores into the component plane.
-//   jpeg_upsample_color_kernel  triangle upsampling + fixed-point colour conversion, packed BGR.
+//   jpeg_idct_color_kernel    one CTA per tile of MCU rows x columns: dequantise + IDCT (one thread
+//                             per 8x8 block, two 1-D passes in registers) into shared-memory
+//                             component rows, then triangle upsampling + fixed-point colour
+//                             conversion from there into the packed BGR frame.
 #include "common.cuh"
 #include "kernels.cuh"
 
@@ -23,10 +24,46 @@ __constant__ uint8_t c_zigzag[64] = {0,  1,  8,  16, 9,  2,  3,  10, 17, 24, 32,
                                      35, 42, 49, 56, 57, 50, 43, 36, 29, 22, 15, 23, 30, 37, 44, 51,
                                      58, 59, 52, 45, 38, 31, 39, 46, 53, 60, 61, 54, 47, 55, 62, 63};
 
+// ------------------------------------------------------------------ tile layout (host and device)
+
+// Dynamic shared memory of one jpeg_idct_color_kernel CTA: a 4:2:0 span of up to 36 MCU columns (576 px).  Five
+// CTAs of 128 threads per SM (the register limit at 96 registers) then fit in shared memory as well.  On an H100
+// that beat a 46 KB budget (one span at the headline's 70-column ROI, four CTAs per SM) by 4 % in kernel time.
+constexpr uint32_t kTileSmemBytes = 24 * 1024;
+
+// libjpeg-turbo's fancy upsamplers (jdsample.c) read neighbouring samples: h2v2 and h1v2 the rows above and
+// below, h2v2 and h2v1 the columns left and right.  Every other ratio replicates.
+__host__ __device__ __forceinline__ bool fancy_rows(int hr, int vr) { return vr == 2 && hr <= 2; }
+__host__ __device__ __forceinline__ bool fancy_cols(int hr, int vr) { return hr == 2 && vr <= 2; }
+
+struct TileLayout {
+    uint32_t off[3], stride[3];  // component c's rows in shared memory: byte offset, row pitch
+    uint32_t bytes;
+};
+
+// Shared memory of a tile `cols` MCU columns wide.  Each component keeps rows of cols + 2 MCU columns (a halo
+// column on each side).  Components upsampled with rows above and below keep three MCU rows (a ring), the
+// others one.
+__host__ __device__ inline TileLayout tile_layout(const JpegDecodeItem& it, int cols) {
+    int maxh = 1, maxv = 1;
+    for (int c = 0; c < it.ncomp; c++) {
+        maxh = it.h[c] > maxh ? it.h[c] : maxh;
+        maxv = it.v[c] > maxv ? it.v[c] : maxv;
+    }
+    TileLayout L{};
+    for (int c = 0; c < it.ncomp; c++) {
+        const int rows = (fancy_rows(maxh / it.h[c], maxv / it.v[c]) ? 3 : 1) * 8 * it.v[c];
+        L.stride[c] = (uint32_t)(((cols + 2) * 8 * it.h[c] + 15) & ~15);
+        L.off[c] = L.bytes;
+        L.bytes += L.stride[c] * (uint32_t)rows;
+    }
+    return L;
+}
+
 // ------------------------------------------------------------------ ROI layout (host)
 
 uint32_t jpeg_item_set_window(JpegDecodeItem* it, int x0, int y0, int x1, int y1, bool align16,
-                              uint32_t* plane_bytes_out) {
+                              uint32_t* tiles_out) {
     int maxh = 1, maxv = 1;
     for (int c = 0; c < it->ncomp; c++) {
         maxh = it->h[c] > maxh ? it->h[c] : maxh;
@@ -59,16 +96,22 @@ uint32_t jpeg_item_set_window(JpegDecodeItem* it, int x0, int y0, int x1, int y1
     it->roi_my0 = py0 / mh;
     it->roi_mcx = px1 / mw - it->roi_mx0 + 1;
     it->roi_mcy = py1 / mh - it->roi_my0 + 1;
-    uint32_t blocks = 0, plane_bytes = 0;
+    uint32_t blocks = 0;
     for (int c = 0; c < it->ncomp; c++) {
         it->bw[c] = it->roi_mcx * it->h[c];
         it->bh[c] = it->roi_mcy * it->v[c];
         it->block_off[c] = blocks;
-        it->plane_rel[c] = plane_bytes;
         blocks += (uint32_t)it->bw[c] * it->bh[c];
-        plane_bytes += (uint32_t)it->bw[c] * it->bh[c] * 64;
     }
-    if (plane_bytes_out) *plane_bytes_out = plane_bytes;
+    // Tiles: spans as wide as the shared-memory budget allows, evened out over the ROI width, and four bands of
+    // MCU rows so that an image gives several CTAs.
+    const int mcx = it->roi_mcx > 0 ? it->roi_mcx : 1, mcy = it->roi_mcy > 0 ? it->roi_mcy : 1;
+    int span = mcx;
+    while (span > 1 && tile_layout(*it, span).bytes > kTileSmemBytes) span--;
+    it->tile_mcx = (mcx + (mcx + span - 1) / span - 1) / ((mcx + span - 1) / span);
+    it->tiles_x = (mcx + it->tile_mcx - 1) / it->tile_mcx;
+    it->tile_mcy = (mcy + 3) / 4;
+    if (tiles_out) *tiles_out = (uint32_t)(it->tiles_x * ((mcy + it->tile_mcy - 1) / it->tile_mcy));
     return blocks;
 }
 
@@ -603,84 +646,113 @@ __device__ __forceinline__ uint32_t pack_px(int a, int b, int c, int d) {
     return w ^ 0x80808080u;
 }
 
-__global__ void __launch_bounds__(128)
-    jpeg_idct_kernel(const JpegDecodeItem* items, const int16_t* coef, uint8_t* planes, int mcu_order) {
-    const JpegDecodeItem& it = items[blockIdx.y];
-    if (it.status != 0) return;
-    // the image's quantisation tables, once per CTA (read back 8 entries per load below)
-    __shared__ __align__(16) uint16_t s_qt[3][64];
-    for (int i = threadIdx.x; i < 3 * 64; i += blockDim.x) s_qt[i >> 6][i & 63] = it.qt[i >> 6][i & 63];
-    __syncthreads();
-    const int blk = blockIdx.x * blockDim.x + threadIdx.x;
-    int c = 0;
-    if (it.ncomp == 3) c = blk >= (int)it.block_off[2] ? 2 : (blk >= (int)it.block_off[1] ? 1 : 0);
-    const int nblk = (int)it.block_off[it.ncomp - 1] + it.bw[it.ncomp - 1] * it.bh[it.ncomp - 1];
-    if (blk >= nblk) return;
-    const int rel = blk - (int)it.block_off[c];
-    const int X = rel % it.bw[c], Y = rel / it.bw[c];
-    // The serial and multi-scan entropy decoders store blocks per component in raster order (index =
-    // blk); the parallel decoder stores them in scan order (jpeg_huff_parallel.cu): block (X % h, Y % v)
-    // of component c inside ROI MCU (X / h, Y / v).
-    size_t sblk = (size_t)blk;
-    if (mcu_order) {
-        const int h = it.h[c], vv = it.v[c];
-        int nb = 0, kfirst = 0;
-        for (int k = 0; k < it.ncomp; k++) {
-            if (k < c) kfirst += it.h[k] * it.v[k];
-            nb += it.h[k] * it.v[k];
-        }
-        sblk = ((size_t)(Y / vv) * it.roi_mcx + X / h) * nb + kfirst + (Y % vv) * h + X % h;
+// ------------------------------------------------------------------ fused dequant + IDCT + upsample + colour
+//
+// jpeg_idct_color_kernel runs one CTA per tile of an image: a band of ROI MCU rows x a span of ROI MCU columns
+// (jpeg_item_set_window sizes them).  The CTA walks its band top to bottom.  For each MCU row it dequantises and
+// IDCTs the row's blocks into shared-memory component rows, then upsamples and converts those rows straight into
+// the frame window.  Only the coefficients are read from HBM and only the window is written.
+//
+// Components that fancy upsampling reads vertically keep a ring of three MCU rows (m - 1, m, m + 1) and are
+// IDCT'd one MCU row ahead.  Fancy upsampling reads one sample beyond the window on every side.  At the ROI edge
+// that sample lies inside the ROI (jpeg_item_set_window adds the margin).  At an inner tile edge the CTA IDCTs the
+// neighbouring MCU row or column itself.
+
+constexpr int kIdctColorThreads = 128;
+
+// Per-component geometry of one tile, in shared memory.
+struct TileCtx {
+    int off[3], stride[3];  // shared-memory rows (TileLayout)
+    int h[3], v[3];         // sampling factors
+    int ring[3];            // 1: three MCU rows kept, IDCT'd one row ahead
+    int row0[3];            // full-image component row of ROI row 0
+    int col0[3];            // full-image component column of shared-memory column 0
+    int xb0[3];             // ROI block column of shared-memory column 0
+    int ca[3], nc[3];       // ROI MCU columns IDCT'd: [ca, ca + nc)
+    int kfirst[3];          // first block of the component inside a scan-order MCU
+    int nb;                 // blocks per MCU
+};
+
+// Offset in the tile of full-image component row cy, column 0 (add the column).
+__device__ __forceinline__ int tile_row(const TileCtx& t, int c, int cy) {
+    const int rows = 8 * t.v[c];
+    const int ry = cy - t.row0[c];
+    const int mr = ry / rows;
+    const int slot = t.ring[c] ? mr % 3 : 0;
+    return t.off[c] + (slot * rows + ry - mr * rows) * t.stride[c] - t.col0[c];
+}
+
+// Dequantise + IDCT ROI MCU row m_ring of the ring components and m_flat of the others (-1: none) over the
+// tile's columns into shared memory, one thread per block.  The serial and multi-scan entropy decoders store
+// blocks per component in raster order; the parallel decoders store them in scan order (jpeg_huff_parallel.cu):
+// block (X % h, Y % v) of component c inside ROI MCU (X / h, Y / v).
+__device__ __forceinline__ void idct_phase(const JpegDecodeItem& it, const TileCtx& t, const int16_t* coef,
+                                           int mcu_order, const uint16_t (*qt)[64], uint8_t* tile, int m_flat,
+                                           int m_ring) {
+    int end[3];
+    int total = 0;
+#pragma unroll
+    for (int c = 0; c < 3; c++) {
+        const int m = t.ring[c] ? m_ring : m_flat;
+        if (c < it.ncomp && m >= 0) total += t.nc[c] * t.h[c] * t.v[c];
+        end[c] = total;
     }
-    const uint4* src = reinterpret_cast<const uint4*>(coef + it.coef_off + sblk * 64);
-    const uint4* q4 = reinterpret_cast<const uint4*>(s_qt[c]);
-    int v[64];
+    for (int j = threadIdx.x; j < total; j += blockDim.x) {
+        const int c = j < end[0] ? 0 : (j < end[1] ? 1 : 2);
+        const int k = j - (c == 0 ? 0 : (c == 1 ? end[0] : end[1]));
+        const int h = t.h[c], vs = t.v[c];
+        const int m = t.ring[c] ? m_ring : m_flat;
+        const int per = t.nc[c] * h;  // blocks per block row
+        const int by = k / per, bx = k - by * per;
+        const int X = t.ca[c] * h + bx;  // ROI block column
+        const size_t sblk = mcu_order
+                                ? ((size_t)m * it.roi_mcx + X / h) * t.nb + t.kfirst[c] + by * h + X % h
+                                : (size_t)it.block_off[c] + (size_t)(m * vs + by) * it.bw[c] + X;
+        const uint4* src = reinterpret_cast<const uint4*>(coef + it.coef_off + sblk * 64);
+        const uint4* q4 = reinterpret_cast<const uint4*>(qt[c]);
+        int v[64];
 #pragma unroll
-    for (int r = 0; r < 8; r++) {
-        const uint4 u = __ldg(src + r);
-        const uint4 qq = q4[r];
-        const uint32_t w[4] = {u.x, u.y, u.z, u.w};
-        const uint32_t qw[4] = {qq.x, qq.y, qq.z, qq.w};
+        for (int r = 0; r < 8; r++) {
+            const uint4 u = __ldg(src + r);
+            const uint4 qq = q4[r];
+            const uint32_t w[4] = {u.x, u.y, u.z, u.w};
+            const uint32_t qw[4] = {qq.x, qq.y, qq.z, qq.w};
 #pragma unroll
-        for (int k = 0; k < 4; k++) {
-            // 16-bit wrapping multiply (pmullw), as libjpeg-turbo's SIMD dequantisation does
-            const int lo = (int16_t)(w[k] & 0xffff), hi = (int16_t)(w[k] >> 16);
-            v[r * 8 + 2 * k] = (int16_t)(lo * (int)(qw[k] & 0xffff));
-            v[r * 8 + 2 * k + 1] = (int16_t)(hi * (int)(qw[k] >> 16));
+            for (int q = 0; q < 4; q++) {
+                // 16-bit wrapping multiply (pmullw), as libjpeg-turbo's SIMD dequantisation does
+                const int lo = (int16_t)(w[q] & 0xffff), hi = (int16_t)(w[q] >> 16);
+                v[r * 8 + 2 * q] = (int16_t)(lo * (int)(qw[q] & 0xffff));
+                v[r * 8 + 2 * q + 1] = (int16_t)(hi * (int)(qw[q] >> 16));
+            }
         }
-    }
 #pragma unroll
-    for (int x = 0; x < 8; x++)
-        idct8<11, true>(v[x], v[8 + x], v[16 + x], v[24 + x], v[32 + x], v[40 + x], v[48 + x], v[56 + x]);
-    const int stride = it.bw[c] * 8;
-    uint8_t* dst = planes + it.plane_off + it.plane_rel[c] + (size_t)Y * 8 * stride + X * 8;
+        for (int x = 0; x < 8; x++)
+            idct8<11, true>(v[x], v[8 + x], v[16 + x], v[24 + x], v[32 + x], v[40 + x], v[48 + x], v[56 + x]);
+        const int stride = t.stride[c];
+        uint8_t* dst = tile + t.off[c] + ((t.ring[c] ? m % 3 : 0) * 8 * vs + by * 8) * stride + (X - t.xb0[c]) * 8;
 #pragma unroll
-    for (int r = 0; r < 8; r++) {
-        idct8<18, false>(v[r * 8], v[r * 8 + 1], v[r * 8 + 2], v[r * 8 + 3], v[r * 8 + 4], v[r * 8 + 5],
-                         v[r * 8 + 6], v[r * 8 + 7]);
-        uint2 o;
-        o.x = pack_px(v[r * 8], v[r * 8 + 1], v[r * 8 + 2], v[r * 8 + 3]);
-        o.y = pack_px(v[r * 8 + 4], v[r * 8 + 5], v[r * 8 + 6], v[r * 8 + 7]);
-        *reinterpret_cast<uint2*>(dst + (size_t)r * stride) = o;
+        for (int r = 0; r < 8; r++) {
+            idct8<18, false>(v[r * 8], v[r * 8 + 1], v[r * 8 + 2], v[r * 8 + 3], v[r * 8 + 4], v[r * 8 + 5],
+                             v[r * 8 + 6], v[r * 8 + 7]);
+            uint2 o;
+            o.x = pack_px(v[r * 8], v[r * 8 + 1], v[r * 8 + 2], v[r * 8 + 3]);
+            o.y = pack_px(v[r * 8 + 4], v[r * 8 + 5], v[r * 8 + 6], v[r * 8 + 7]);
+            *reinterpret_cast<uint2*>(dst + r * stride) = o;
+        }
     }
 }
 
-// ------------------------------------------------------------------ upsample + colour
-
 // Value of component c at full-resolution pixel (x, y): libjpeg-turbo jdsample.c.
-__device__ __forceinline__ int upsampled(const JpegDecodeItem& it, const uint8_t* planes, int c, int maxh,
-                                         int maxv, int x, int y) {
-    const int stride = it.bw[c] * 8;
-    // plane origin shifted so that full-image component coordinates index it directly
-    const uint8_t* pl = planes + it.plane_off + it.plane_rel[c] -
-                        ((size_t)(it.roi_my0 * it.v[c] * 8) * stride + (size_t)(it.roi_mx0 * it.h[c] * 8));
-    const int hr = maxh / it.h[c], vr = maxv / it.v[c];
+__device__ __forceinline__ int upsampled(const JpegDecodeItem& it, const TileCtx& t, const uint8_t* tile, int c,
+                                         int maxh, int maxv, int x, int y) {
+    const int hr = maxh / t.h[c], vr = maxv / t.v[c];
     const int cw = it.dw[c], ch = it.dh[c];
-    if (hr == 1 && vr == 1) return pl[(size_t)y * stride + x];
+    if (hr == 1 && vr == 1) return tile[tile_row(t, c, y) + x];
     if (hr == 2 && vr == 2) {
         const int cy = y >> 1, i = x >> 1;
         const int fy = min(max((y & 1) ? cy + 1 : cy - 1, 0), ch - 1);
-        const uint8_t* s0 = pl + (size_t)cy * stride;
-        const uint8_t* s1 = pl + (size_t)fy * stride;
+        const uint8_t* s0 = tile + tile_row(t, c, cy);
+        const uint8_t* s1 = tile + tile_row(t, c, fy);
         const int cs = 3 * s0[i] + s1[i];
         if (x & 1) {
             if (i == cw - 1) return (cs * 4 + 7) >> 4;
@@ -690,7 +762,7 @@ __device__ __forceinline__ int upsampled(const JpegDecodeItem& it, const uint8_t
         return (cs * 3 + 3 * s0[i - 1] + s1[i - 1] + 8) >> 4;
     }
     if (hr == 2 && vr == 1) {
-        const uint8_t* s = pl + (size_t)y * stride;
+        const uint8_t* s = tile + tile_row(t, c, y);
         const int i = x >> 1;
         if (x & 1) return (i == cw - 1) ? s[i] : (3 * s[i] + s[i + 1] + 2) >> 2;
         return (i == 0) ? s[0] : (3 * s[i] + s[i - 1] + 1) >> 2;
@@ -698,59 +770,17 @@ __device__ __forceinline__ int upsampled(const JpegDecodeItem& it, const uint8_t
     if (hr == 1 && vr == 2) {
         const int cy = y >> 1;
         const int fy = min(max((y & 1) ? cy + 1 : cy - 1, 0), ch - 1);
-        return (3 * pl[(size_t)cy * stride + x] + pl[(size_t)fy * stride + x] + ((y & 1) ? 2 : 1)) >> 2;
+        return (3 * tile[tile_row(t, c, cy) + x] + tile[tile_row(t, c, fy) + x] + ((y & 1) ? 2 : 1)) >> 2;
     }
-    return pl[(size_t)(y / vr) * stride + x / hr];  // int_upsample (replication)
+    return tile[tile_row(t, c, y / vr) + x / hr];  // int_upsample (replication)
 }
 
-// Thread = 16 consecutive output pixels of one row.  4:2:0 frames whose rows are 16-byte aligned take
-// the vector path (one 16-byte Y load, four 8-byte chroma loads, three 16-byte stores); everything
-// else (other samplings, grayscale, odd widths) goes pixel by pixel through upsampled().
-__global__ void __launch_bounds__(128)
-    jpeg_upsample_color_kernel(const JpegDecodeItem* items, const uint8_t* planes, uint8_t* frames) {
-    const JpegDecodeItem& it = items[blockIdx.y];
-    if (it.status != 0) return;
-    // flat index over (row, 16-pixel segment): a window row of 68 segments would leave half of a 128-thread
-    // block idle if blocks were tied to rows (ncu round 2: 23 of 32 lanes active)
-    const unsigned segs = (unsigned)(it.win_w + 15) >> 4;
-    const unsigned f = blockIdx.x * blockDim.x + threadIdx.x;
-    const unsigned row = f / segs;
-    if (row >= (unsigned)it.win_h) return;
-    const int x0 = it.win_x0 + (int)(f - row * segs) * 16;  // full-image coordinates
-    const int y = it.win_y0 + (int)row;
-    const int xe = it.win_x0 + it.win_w;
-    uint8_t* out = frames + it.frame_off + (size_t)(y - it.win_y0) * it.win_stride;  // this window row
-    if (it.ncomp == 1) {
-        const int stride = it.bw[0] * 8;
-        const uint8_t* pl = planes + it.plane_off + it.plane_rel[0] + (size_t)(y - it.roi_my0 * 8) * stride -
-                            (size_t)(it.roi_mx0 * 8);
-        for (int x = x0; x < min(x0 + 16, xe); x++) out[x - it.win_x0] = pl[x];
-        return;
-    }
-    const bool fast = it.h[0] == 2 && it.v[0] == 2 && it.h[1] == 1 && it.v[1] == 1 && it.h[2] == 1 &&
-                      it.v[2] == 1 && (it.width & 15) == 0 && (it.win_x0 & 15) == 0 && (it.win_w & 15) == 0 &&
-                      (it.win_stride & 15) == 0 && (it.frame_off & 15) == 0;
-    if (!fast) {
-        const int maxh = max(it.h[0], max(it.h[1], it.h[2])), maxv = max(it.v[0], max(it.v[1], it.v[2]));
-        for (int x = x0; x < min(x0 + 16, xe); x++) {
-            const int Y = upsampled(it, planes, 0, maxh, maxv, x, y);
-            const int cb = upsampled(it, planes, 1, maxh, maxv, x, y) - 128;
-            const int cr = upsampled(it, planes, 2, maxh, maxv, x, y) - 128;
-            const int r = Y + ((91881 * cr + 32768) >> 16);
-            const int g = Y + ((-22554 * cb + 32768 - 46802 * cr) >> 16);
-            const int b = Y + ((116130 * cb + 32768) >> 16);
-            uint8_t* o = out + (size_t)(x - it.win_x0) * 3;
-            o[0] = (uint8_t)min(max(b, 0), 255);
-            o[1] = (uint8_t)min(max(g, 0), 255);
-            o[2] = (uint8_t)min(max(r, 0), 255);
-        }
-        return;
-    }
-    const uint8_t* base = planes + it.plane_off;
-    const int sy = it.bw[0] * 8, sc = it.bw[1] * 8;
-    const int lx = it.roi_mx0 * 16, ly = it.roi_my0 * 16;  // luma / chroma plane origins (4:2:0)
-    const int cx_ = it.roi_mx0 * 8, cy_ = it.roi_my0 * 8;
-    const uint4 yv = *reinterpret_cast<const uint4*>(base + it.plane_rel[0] + (size_t)(y - ly) * sy + (x0 - lx));
+// 4:2:0, 16-byte aligned: 16 consecutive pixels of row y from x0 (one 16-byte Y load, four 8-byte chroma loads,
+// three 16-byte stores).
+__device__ __forceinline__ void color16_420(const JpegDecodeItem& it, const TileCtx& t, const uint8_t* tile,
+                                            uint8_t* out, int x0, int y) {
+    const uint4 yv = *reinterpret_cast<const uint4*>(tile + t.off[0] + ((y - t.row0[0]) & 15) * t.stride[0] +
+                                                     (x0 - t.col0[0]));
     const uint32_t yw[4] = {yv.x, yv.y, yv.z, yv.w};
     const int cw = it.dw[1], chh = it.dh[1];
     const int cy = y >> 1;
@@ -760,8 +790,10 @@ __global__ void __launch_bounds__(128)
     int cs[2][10];  // 3*near + far for chroma columns i0-1 .. i0+8, Cb and Cr
 #pragma unroll
     for (int c = 0; c < 2; c++) {
-        const uint8_t* pn = base + it.plane_rel[1 + c] + (size_t)(cy - cy_) * sc - cx_;
-        const uint8_t* pf = base + it.plane_rel[1 + c] + (size_t)(fy - cy_) * sc - cx_;
+        // the chroma ring: MCU row r of the ROI sits in slot r % 3
+        const int rn = cy - t.row0[1 + c], rf = fy - t.row0[1 + c];
+        const uint8_t* pn = tile + t.off[1 + c] + (((rn >> 3) % 3) * 8 + (rn & 7)) * t.stride[1 + c] - t.col0[1 + c];
+        const uint8_t* pf = tile + t.off[1 + c] + (((rf >> 3) % 3) * 8 + (rf & 7)) * t.stride[1 + c] - t.col0[1 + c];
         const uint2 n8 = *reinterpret_cast<const uint2*>(pn + i0);
         const uint2 f8 = *reinterpret_cast<const uint2*>(pf + i0);
         cs[c][0] = 3 * pn[il] + pf[il];
@@ -785,8 +817,8 @@ __global__ void __launch_bounds__(128)
     for (int q = 0; q < 4; q++) {  // 4 pixels -> 3 output words
         uint32_t B[4], G[4], R[4];
 #pragma unroll
-        for (int t = 0; t < 4; t++) {
-            const int k = 4 * q + t;
+        for (int p = 0; p < 4; p++) {
+            const int k = 4 * q + p;
             const int j = 1 + (k >> 1);
             int cb, cr;
             if (k & 1) {
@@ -796,11 +828,11 @@ __global__ void __launch_bounds__(128)
                 cb = (c3[0][j] + cs[0][j - 1] + 8) >> 4;
                 cr = (c3[1][j] + cs[1][j - 1] + 8) >> 4;
             }
-            const int Y = (int)__byte_perm(yw[q], 0, 0x4440 + t);  // byte t of the word, zero-extended
+            const int Y = (int)__byte_perm(yw[q], 0, 0x4440 + p);  // byte p of the word, zero-extended
             // (c * (x - 128) + 32768) >> 16 with the -128 folded into the addend
-            R[t] = (uint32_t)__vimin_s32_relu(Y + ((91881 * cr + (32768 - 91881 * 128)) >> 16), 255);
-            G[t] = (uint32_t)__vimin_s32_relu(Y + ((-22554 * cb - 46802 * cr + (32768 + (22554 + 46802) * 128)) >> 16), 255);
-            B[t] = (uint32_t)__vimin_s32_relu(Y + ((116130 * cb + (32768 - 116130 * 128)) >> 16), 255);
+            R[p] = (uint32_t)__vimin_s32_relu(Y + ((91881 * cr + (32768 - 91881 * 128)) >> 16), 255);
+            G[p] = (uint32_t)__vimin_s32_relu(Y + ((-22554 * cb - 46802 * cr + (32768 + (22554 + 46802) * 128)) >> 16), 255);
+            B[p] = (uint32_t)__vimin_s32_relu(Y + ((116130 * cb + (32768 - 116130 * 128)) >> 16), 255);
         }
         // bytes: B0 G0 R0 B1 | G1 R1 B2 G2 | R2 B3 G3 R3
         ow[3 * q + 0] = __byte_perm(__byte_perm(B[0], G[0], 0x0040), __byte_perm(R[0], B[1], 0x0040), 0x5410);
@@ -811,6 +843,97 @@ __global__ void __launch_bounds__(128)
     dst[0] = make_uint4(ow[0], ow[1], ow[2], ow[3]);
     dst[1] = make_uint4(ow[4], ow[5], ow[6], ow[7]);
     dst[2] = make_uint4(ow[8], ow[9], ow[10], ow[11]);
+}
+
+// Upsample + colour the window pixels of ROI MCU row m inside the span [c0, c1), one thread per 16 consecutive
+// pixels of a row.  4:2:0 frames whose rows are 16-byte aligned take color16_420; everything else (other
+// samplings, odd widths) goes pixel by pixel through upsampled(); grayscale is a copy.
+__device__ __forceinline__ void color_phase(const JpegDecodeItem& it, const TileCtx& t, const uint8_t* tile,
+                                            uint8_t* frames, int m, int c0, int c1, int maxh, int maxv, bool fast) {
+    const int mh = 8 * maxv, mw = 8 * maxh;
+    const int ya = max(it.win_y0, (it.roi_my0 + m) * mh), yb = min(it.win_y0 + it.win_h, (it.roi_my0 + m + 1) * mh);
+    const int xa = max(it.win_x0, (it.roi_mx0 + c0) * mw), xb = min(it.win_x0 + it.win_w, (it.roi_mx0 + c1) * mw);
+    if (ya >= yb || xa >= xb) return;
+    const int segs = (xb - xa + 15) >> 4;
+    const int n = (yb - ya) * segs;
+    for (int j = threadIdx.x; j < n; j += blockDim.x) {
+        const int r = j / segs;
+        const int y = ya + r, x0 = xa + (j - r * segs) * 16;
+        uint8_t* out = frames + it.frame_off + (size_t)(y - it.win_y0) * it.win_stride;
+        if (it.ncomp == 1) {
+            const int o = tile_row(t, 0, y);
+            for (int x = x0; x < min(x0 + 16, xb); x++) out[x - it.win_x0] = tile[o + x];
+        } else if (fast) {
+            color16_420(it, t, tile, out, x0, y);
+        } else {
+            for (int x = x0; x < min(x0 + 16, xb); x++) {
+                const int Y = upsampled(it, t, tile, 0, maxh, maxv, x, y);
+                const int cb = upsampled(it, t, tile, 1, maxh, maxv, x, y) - 128;
+                const int cr = upsampled(it, t, tile, 2, maxh, maxv, x, y) - 128;
+                const int r = Y + ((91881 * cr + 32768) >> 16);
+                const int g = Y + ((-22554 * cb + 32768 - 46802 * cr) >> 16);
+                const int b = Y + ((116130 * cb + 32768) >> 16);
+                uint8_t* o = out + (size_t)(x - it.win_x0) * 3;
+                o[0] = (uint8_t)min(max(b, 0), 255);
+                o[1] = (uint8_t)min(max(g, 0), 255);
+                o[2] = (uint8_t)min(max(r, 0), 255);
+            }
+        }
+    }
+}
+
+__global__ void __launch_bounds__(kIdctColorThreads, 5)
+    jpeg_idct_color_kernel(const JpegDecodeItem* items, const int16_t* coef, uint8_t* frames, int mcu_order) {
+    const JpegDecodeItem& it = items[blockIdx.y];
+    if (it.status != 0) return;
+    const int band = (int)blockIdx.x / it.tiles_x, span = (int)blockIdx.x - band * it.tiles_x;
+    const int m0 = band * it.tile_mcy, m1 = min(m0 + it.tile_mcy, it.roi_mcy);
+    const int c0 = span * it.tile_mcx, c1 = min(c0 + it.tile_mcx, it.roi_mcx);
+    if (m0 >= m1 || c0 >= c1) return;
+    __shared__ __align__(16) uint16_t s_qt[3][64];
+    __shared__ TileCtx s_t;
+    extern __shared__ __align__(16) uint8_t s_tile[];
+    for (int i = threadIdx.x; i < 3 * 64; i += blockDim.x) s_qt[i >> 6][i & 63] = it.qt[i >> 6][i & 63];
+    int maxh = 1, maxv = 1;
+    for (int c = 0; c < it.ncomp; c++) {
+        maxh = max(maxh, it.h[c]);
+        maxv = max(maxv, it.v[c]);
+    }
+    if (threadIdx.x == 0) {
+        const TileLayout L = tile_layout(it, c1 - c0);
+        int nb = 0;
+        for (int c = 0; c < it.ncomp; c++) {
+            const int hr = maxh / it.h[c], vr = maxv / it.v[c];
+            const bool halo = fancy_cols(hr, vr);
+            s_t.off[c] = (int)L.off[c];
+            s_t.stride[c] = (int)L.stride[c];
+            s_t.h[c] = it.h[c];
+            s_t.v[c] = it.v[c];
+            s_t.ring[c] = fancy_rows(hr, vr);
+            s_t.row0[c] = it.roi_my0 * 8 * it.v[c];
+            s_t.xb0[c] = (c0 - 1) * it.h[c];
+            s_t.col0[c] = (it.roi_mx0 * it.h[c] + s_t.xb0[c]) * 8;
+            s_t.ca[c] = halo && c0 > 0 ? c0 - 1 : c0;
+            s_t.nc[c] = (halo && c1 < it.roi_mcx ? c1 + 1 : c1) - s_t.ca[c];
+            s_t.kfirst[c] = nb;
+            nb += it.h[c] * it.v[c];
+        }
+        s_t.nb = nb;
+    }
+    __syncthreads();
+    const TileCtx& t = s_t;
+    const bool fast = it.ncomp == 3 && it.h[0] == 2 && it.v[0] == 2 && it.h[1] == 1 && it.v[1] == 1 &&
+                      it.h[2] == 1 && it.v[2] == 1 && (it.width & 15) == 0 && (it.win_x0 & 15) == 0 &&
+                      (it.win_w & 15) == 0 && (it.win_stride & 15) == 0 && (it.frame_off & 15) == 0;
+    // the ring's rows above the band and the band's first row
+    if (m0 > 0) idct_phase(it, t, coef, mcu_order, s_qt, s_tile, -1, m0 - 1);
+    idct_phase(it, t, coef, mcu_order, s_qt, s_tile, -1, m0);
+    for (int m = m0; m < m1; m++) {
+        idct_phase(it, t, coef, mcu_order, s_qt, s_tile, m, m + 1 < it.roi_mcy ? m + 1 : -1);
+        __syncthreads();
+        color_phase(it, t, s_tile, frames, m, c0, c1, maxh, maxv, fast);
+        __syncthreads();
+    }
 }
 
 // ------------------------------------------------------------------ launcher
@@ -841,17 +964,10 @@ int jpeg_decode_launch(const JpegDecodeBatch& b, cudaStream_t st, cudaEvent_t ev
         LP_CUDA_OK(cudaGetLastError());
     }
     if (ev_after_huff) LP_CUDA_OK(cudaEventRecord(ev_after_huff, st));
-    {
-        dim3 grid(ceil_div(b.max_blocks_per_image, 128), b.n);
+    if (b.max_tiles_per_image > 0) {
+        const dim3 grid((unsigned)b.max_tiles_per_image, b.n);
         const int mcu_order = !b.scans && b.use_parallel_huffman;
-        jpeg_idct_kernel<<<grid, 128, 0, st>>>(b.items, b.coef, b.planes, mcu_order);
-        g_launches++;
-        LP_CUDA_OK(cudaGetLastError());
-    }
-    {
-        const long segs = (long)ceil_div(b.max_width, 16) * b.max_height;
-        dim3 grid((unsigned)((segs + 127) / 128), b.n);
-        jpeg_upsample_color_kernel<<<grid, 128, 0, st>>>(b.items, b.planes, b.frames);
+        jpeg_idct_color_kernel<<<grid, kIdctColorThreads, kTileSmemBytes, st>>>(b.items, b.coef, b.frames, mcu_order);
         g_launches++;
         LP_CUDA_OK(cudaGetLastError());
     }

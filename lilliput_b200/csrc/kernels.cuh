@@ -66,7 +66,6 @@ struct JpegDecodeItem {
     uint32_t scan_len;    // bytes
     uint32_t table_set;   // index into the Huffman table-set array
     uint64_t coef_off;    // int16 offset of this image's coefficient blocks
-    uint64_t plane_off;   // byte offset of this image's component planes
     uint64_t frame_off;   // byte offset of this image's packed output frame
     int32_t width, height, ncomp;
     int32_t mcus_x, mcus_y, restart_interval;
@@ -74,7 +73,9 @@ struct JpegDecodeItem {
     int32_t bw[3], bh[3]; // blocks per component plane (padded to the MCU grid)
     int32_t dw[3], dh[3]; // true downsampled component size in samples
     uint32_t block_off[3];  // first block of component c inside the image's coef area
-    uint32_t plane_rel[3];  // byte offset of component c's plane inside the image's plane area
+    // tiles of jpeg_idct_color_kernel (one CTA each): tiles_x spans of tile_mcx ROI MCU columns, bands of tile_mcy
+    // ROI MCU rows
+    int32_t tile_mcx, tile_mcy, tiles_x;
     uint16_t qt[3][64];     // per-component quantisation table, natural order
     int32_t td[3], ta[3];
     int32_t status;         // written by the decode kernel: 0 ok, <0 corrupt
@@ -86,7 +87,7 @@ struct JpegDecodeItem {
     uint32_t clean_len;     // written by jpeg_unstuff_kernel
     uint32_t pad_;
     // Region of interest.  Only MCUs [roi_mx0, roi_mx0+roi_mcx) x [roi_my0, roi_my0+roi_mcy) get
-    // coefficients / planes (bw, bh, block_off, plane_rel describe THAT grid); the packed frame holds
+    // coefficients (bw, bh, block_off describe THAT grid); the packed frame holds
     // the pixel window [win_x0, win_x0+win_w) x [win_y0, win_y0+win_h) with rows win_stride apart.
     // A full decode has roi = every MCU and win = the whole image.
     int32_t roi_mx0, roi_my0, roi_mcx, roi_mcy;
@@ -97,9 +98,10 @@ struct JpegDecodeItem {
 
 // Fills the ROI / window / layout fields of `it` (whose width, height, ncomp, h, v, mcus_* are set)
 // for the pixel window [x0,x1) x [y0,y1).  align16 rounds the window's x range outwards to 16 px so
-// the vectorised colour kernel can use 16-byte stores.  Returns blocks in the ROI.
+// the vectorised colour step can use 16-byte stores.  Returns blocks in the ROI; *tiles (if given) = the CTAs
+// jpeg_idct_color_kernel runs for the image.
 uint32_t jpeg_item_set_window(JpegDecodeItem* it, int x0, int y0, int x1, int y1, bool align16,
-                              uint32_t* plane_bytes);
+                              uint32_t* tiles);
 
 // Huffman decode tables for one image (or many images sharing them), device format.
 constexpr int kHuffAcLookBits = 12;    // AC lookahead of the parallel decoder (jpeg_huff_parallel.cu)
@@ -128,12 +130,10 @@ struct JpegDecodeBatch {
     const JpegHuffSet* tables;  // device
     const uint8_t* scan;        // device, concatenated entropy-coded segments
     int16_t* coef;              // device, zeroed by the launcher
-    uint8_t* planes;            // device
     uint8_t* frames;            // device, packed BGR / gray frames
     int n;
     size_t coef_elems_total;    // for the memset
-    int max_blocks_per_image;
-    int max_width, max_height;
+    int max_tiles_per_image;    // largest *tiles of jpeg_item_set_window over the batch
     // parallel Huffman scratch (all device); used when use_parallel_huffman is set
     bool use_parallel_huffman = false;
     uint8_t* clean = nullptr;
@@ -169,7 +169,7 @@ int jpeg_huff_parallel_launch(const JpegHuffParallelArgs& a, cudaStream_t st);
 int jpeg_huff_parallel_slots();
 // Diagnostics: clock64 cycles per phase of the sync kernels summed over CTAs (see jpeg_huff_parallel.cu)
 int jpeg_huff_phase_clocks(unsigned long long out[8], int reset);
-// Launches: memset(coef) -> huffman decode -> idct -> upsample+colour.
+// Launches: memset(coef) -> huffman decode -> fused idct + upsample + colour.
 int jpeg_decode_launch(const JpegDecodeBatch& b, cudaStream_t st, cudaEvent_t ev_after_huff);
 
 // ---- png_parse.cpp (host) / png_decode.cu ------------------------------------------------------
