@@ -71,6 +71,11 @@ def main():
         lambda lib: lib.webp_frames(webp_lossless))
     add("webp_lossy_encode_512", "webp_encoder_write + flush, 512x512 BGR q80",
         lambda lib: lib.encode(".webp", bgr1080[:512, :512].copy(), {abi.WebpQuality: 80}))
+    # a large frame whose alpha plane codes to many bits: the ALPH packer's worst case
+    bgra4k_noisy = rgba4k.copy()
+    bgra4k_noisy[:, :, 3] = np.random.Generator(np.random.PCG64(6)).integers(0, 256, (2160, 3840), dtype=np.uint8)
+    add("webp_lossy_encode_4k_bgra", "webp_encoder_write + flush, 3840x2160 BGRA with a uniformly random alpha plane, q80",
+        lambda lib: lib.encode(".webp", bgra4k_noisy, {abi.WebpQuality: 80}))
     add("gif_to_webp_config4", "lp_transform: 8-frame 1280x720 GIF -> Fit 256x256 -> animated WebP q80 (BASELINE config 4, 8 of 128 frames)",
         lambda lib: lib.transform(gif, abi.ImageOptions(FileType=".webp", Width=256, Height=256, ResizeMethod=abi.ImageOpsFit,
                                                         EncodeOptions={abi.WebpQuality: 80}, EncodeTimeout_ns=T)), reps=2)

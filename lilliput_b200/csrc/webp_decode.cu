@@ -295,28 +295,25 @@ __global__ void __launch_bounds__(kVp8WarpsPerBlock * 32) vp8_decode_kernel(cons
         for (int mb_x = 0; mb_x < mb_w; mb_x++) filter_macroblock_warp(h, w, mb_x, mb_y, lane);
 }
 
-struct Vp8Output {
-    const uint8_t *y, *u, *v;
-    const uint8_t* alpha;  // width x height plane or null
-    int ys, cs, width, height;
-    uint8_t* dst;
-    size_t dst_step;
-    int channels;  // 3 or 4
-};
-
-__global__ void vp8_output_kernel(Vp8Output o) {
+// Upsampling + colour conversion of decoded frames of one geometry, blockIdx.z = frame: work areas `work_stride` apart,
+// frames `dst_stride` apart in dst, rows `dst_step` apart.  channels 3 or 4; the fourth byte comes from `alpha` (a
+// width x height plane, one-frame launches only) or is 255.
+__global__ void vp8_output_kernel(uint8_t* work, size_t work_stride, int mb_w, int mb_h, int width, int height, uint8_t* dst,
+                                  size_t dst_stride, size_t dst_step, int channels, const uint8_t* alpha) {
     const int x = blockIdx.x * blockDim.x + threadIdx.x;
     const int y = blockIdx.y;
-    if (x >= o.width) return;
-    const int u = vp8::upsample_at(o.u, o.cs, o.width, o.height, x, y);
-    const int v = vp8::upsample_at(o.v, o.cs, o.width, o.height, x, y);
+    if (x >= width) return;
+    vp8::Work w;
+    vp8::work_carve(work + (size_t)blockIdx.z * work_stride, mb_w, mb_h, w);
+    const int u = vp8::upsample_at(w.u, mb_w * 8, width, height, x, y);
+    const int v = vp8::upsample_at(w.v, mb_w * 8, width, height, x, y);
     uint8_t bgr[3];
-    vp8::yuv_to_bgr(o.y[(size_t)y * o.ys + x], u, v, bgr);
-    uint8_t* d = o.dst + (size_t)y * o.dst_step + (size_t)x * o.channels;
+    vp8::yuv_to_bgr(w.y[(size_t)y * (mb_w * 16) + x], u, v, bgr);
+    uint8_t* d = dst + (size_t)blockIdx.z * dst_stride + (size_t)y * dst_step + (size_t)x * channels;
     d[0] = bgr[0];
     d[1] = bgr[1];
     d[2] = bgr[2];
-    if (o.channels == 4) d[3] = o.alpha ? o.alpha[(size_t)y * o.width + x] : 255;
+    if (channels == 4) d[3] = alpha ? alpha[(size_t)y * width + x] : 255;
 }
 
 // VP8L (lossless) frames and ALPH planes: an LZ77 + prefix-coded stream is one serial chain, so
@@ -566,26 +563,6 @@ bool webp_still_info(const uint8_t* data, size_t len, WebpStillInfo* out) {
     return true;
 }
 
-__global__ void vp8_output_batch_kernel(const uint8_t* work, size_t work_stride, int mb_w, int mb_h, int width, int height,
-                                        uint8_t* frames, size_t frame_stride) {
-    const int x = blockIdx.x * blockDim.x + threadIdx.x;
-    const int y = blockIdx.y;
-    if (x >= width) return;
-    const uint8_t* base = work + (size_t)blockIdx.z * work_stride;
-    const size_t ypl = (size_t)mb_w * 16 * mb_h * 16;
-    const uint8_t* yp = base;
-    const uint8_t* up = base + ypl;
-    const uint8_t* vp = up + ypl / 4;
-    const int u = vp8::upsample_at(up, mb_w * 8, width, height, x, y);
-    const int v = vp8::upsample_at(vp, mb_w * 8, width, height, x, y);
-    uint8_t bgr[3];
-    vp8::yuv_to_bgr(yp[(size_t)y * (mb_w * 16) + x], u, v, bgr);
-    uint8_t* d = frames + (size_t)blockIdx.z * frame_stride + ((size_t)y * width + x) * 3;
-    d[0] = bgr[0];
-    d[1] = bgr[1];
-    d[2] = bgr[2];
-}
-
 // n VP8 key frames (any sizes, equal sizes adjacent): one warp per frame (vp8_decode_kernel) in ONE launch,
 // then every pixel of every frame through the fancy upsampler + colour conversion, one launch per run of
 // equal geometry.  Packed BGR frames at d_frames + frame_off[i].
@@ -621,8 +598,8 @@ int webp_vp8_decode_batch(const uint8_t* d_in, const uint64_t* in_off, const uin
                 i1++;
             const int mb_w = (width[i0] + 15) >> 4, mb_h = (height[i0] + 15) >> 4;
             dim3 grid(ceil_div(width[i0], 128), height[i0], i1 - i0);
-            vp8_output_batch_kernel<<<grid, 128, 0, st>>>(d_work + work_off[i0], vp8::work_bytes(mb_w, mb_h), mb_w, mb_h, width[i0],
-                                                          height[i0], d_frames + frame_off[i0], fstride);
+            vp8_output_kernel<<<grid, 128, 0, st>>>(d_work + work_off[i0], vp8::work_bytes(mb_w, mb_h), mb_w, mb_h, width[i0],
+                                                    height[i0], d_frames + frame_off[i0], fstride, (size_t)width[i0] * 3, 3, nullptr);
             g_launches++;
             i0 = i1;
         }
@@ -792,11 +769,9 @@ bool webp_decoder_decode(const webp_decoder d, opencv_mat mat) {
         cudaMemcpyAsync(d->d_item, &item, sizeof(item), cudaMemcpyHostToDevice, st);
         vp8_decode_kernel<<<1, kVp8WarpsPerBlock * 32, 0, st>>>(d->d_item, 1);
         g_launches++;
-        vp8::Work w;
-        vp8::work_carve(d->d_work, mb_w, mb_h, w);
-        Vp8Output o{w.y, w.u, w.v, need_alph ? d->d_alpha : nullptr, mb_w * 16, mb_w * 8, f.width, f.height, frame_dev, frame_step, channels};
         dim3 grid(ceil_div(f.width, 128), f.height);
-        vp8_output_kernel<<<grid, 128, 0, st>>>(o);
+        vp8_output_kernel<<<grid, 128, 0, st>>>(d->d_work, 0, mb_w, mb_h, f.width, f.height, frame_dev, 0, frame_step, channels,
+                                                need_alph ? d->d_alpha : nullptr);
         g_launches++;
     }
     int status = 0;

@@ -11,8 +11,10 @@
 //     reconstruction: the work inside a macroblock spread over the lanes) and codes the first partition
 //     and up to eight token partitions on a lane each.  A valid VP8 stream at libwebp's quality ->
 //     quantiser mapping, PSNR and size; NOT libwebp's own choices, so the bytes differ from the
-//     reference's by design (DESIGN.md s.1 row R8 says what is and is not claimed).
-//   alpha of a lossy frame: an ALPH chunk holding a VP8L-coded plane (same lossless coder).
+//     reference's by design (DESIGN.md s.1 row R8 says what is and is not claimed).  One code path,
+//     webp_encode_lossy_batch, for N frames of one geometry: webp_encoder_write calls it with N = 1.
+//   alpha of a lossy frame: an ALPH chunk holding a VP8L-coded plane (vp8l_enc_core.h; histograms on
+//     the device, prefix codes on the host, one CTA per plane packs the pixels).
 //   animation: every frame a full-canvas ANMF (no blending, no disposal), durations = the delays
 //     handed to webp_encoder_write.  (The reference's WebPAnimEncoder also searches sub-rectangles
 //     and key-frame placement; that is a size optimisation, not a semantic one.)
@@ -85,12 +87,7 @@ __global__ void vp8l_pack_kernel(const uint32_t* resid, size_t n, const vp8lenc:
     if ((uint32_t)hi) atomicOr(&out[w + 2], (uint32_t)hi);
 }
 
-__global__ void extract_alpha_kernel(const uint8_t* frame, size_t step, int width, int height, uint8_t* plane) {
-    const int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y;
-    if (x < width) plane[(size_t)y * width + x] = frame[(size_t)y * step + (size_t)x * 4 + 3];
-}
-
-// frame (channels 3/4) -> "VP8L" payload; plane (channels 1) -> "ALPH" payload.
+// BGR(A) frame (channels 3/4) -> "VP8L" payload.
 static int vp8l_encode_dev(const uint8_t* d_frame, size_t step, int width, int height, int channels,
                            std::vector<uint8_t>* out, cudaStream_t st) {
     const size_t npix = (size_t)width * height;
@@ -122,8 +119,7 @@ static int vp8l_encode_dev(const uint8_t* d_frame, size_t step, int width, int h
         }
         vp8lenc::BitWriter bw;
         vp8lenc::CodeTable table;
-        if (channels == 1) bw.put(1, 8);  // ALPH header byte: VP8L-compressed, no filter, no pre-processing
-        vp8lenc::write_stream_head(bw, width, height, channels == 4, channels != 1, channels != 1, hist, &table);
+        vp8lenc::write_stream_head(bw, width, height, channels == 4, true, true, hist, &table);
         const unsigned long long base_bit = bw.nbits;
         cudaMemcpyAsync(d_table, &table, sizeof(table), cudaMemcpyHostToDevice, st);
         const int blocks = (int)ceil_div(npix, (size_t)256);
@@ -164,25 +160,6 @@ static int vp8l_encode_dev(const uint8_t* d_frame, size_t step, int width, int h
 }
 
 // ------------------------------------------------------------------ lossy kernels
-
-// BGR(A) -> padded Y / U / V planes (edge replication up to the macroblock grid).
-__global__ void vp8_planes_kernel(const uint8_t* frame, size_t step, int channels, int width, int height, int ys, int yh,
-                                  uint8_t* sy, uint8_t* su, uint8_t* sv) {
-    const int cx = blockIdx.x * blockDim.x + threadIdx.x, cy = blockIdx.y;  // one chroma sample = 2x2 luma
-    if (cx >= ys / 2) return;
-    int r = 0, g = 0, b = 0;
-    for (int dy = 0; dy < 2; dy++)
-        for (int dx = 0; dx < 2; dx++) {
-            const int x = min(2 * cx + dx, width - 1), y = min(2 * cy + dy, height - 1);
-            const uint8_t* p = frame + (size_t)y * step + (size_t)x * channels;
-            sy[(size_t)(2 * cy + dy) * ys + 2 * cx + dx] = (uint8_t)vp8enc::rgb_to_y(p[2], p[1], p[0]);
-            b += p[0];
-            g += p[1];
-            r += p[2];
-        }
-    su[(size_t)cy * (ys / 2) + cx] = (uint8_t)vp8enc::rgb_to_u(r, g, b);
-    sv[(size_t)cy * (ys / 2) + cx] = (uint8_t)vp8enc::rgb_to_v(r, g, b);
-}
 
 // ---- macroblock analysis, one WARP per frame --------------------------------------------------
 // vp8enc::analyse_and_reconstruct (vp8_enc_core.h) walks the macroblocks on one lane; that chain (4 + 4 mode trials
@@ -623,89 +600,12 @@ static int vp8_try_i4() {
     return v;
 }
 
-struct Vp8EncJob {
-    vp8enc::Params P;
-    vp8enc::Buffers B;
-    uint8_t *part0, *tokens, *aux, *out;
-    size_t part0_cap, tokens_cap, out_cap;
-    size_t* out_len;
-};
+// ------------------------------------------------------------------ lossy encode
+// N frames of one geometry per launch: the batch ABI (xbatch.cu) passes many, webp_encoder_write one.  One frame per
+// warp (the macroblock walk and the boolean coder are a serial dependency chain per frame, so the parallelism is
+// across frames), alpha planes through one CTA per frame.
 
-__global__ void __launch_bounds__(32) vp8_encode_kernel(Vp8EncJob j) {
-    __shared__ Vp8WarpBuf wb;
-    if (j.P.filter_level < 0) j.P.filter_level = vp8enc::filter_level_for_q(j.P.q);
-    vp8_analyse_warp(j.P, j.B, wb);
-    const size_t n = vp8_write_bitstream_warp(j.P, j.B, j.part0, j.part0_cap, j.tokens, j.tokens_cap, j.aux, j.out, j.out_cap);
-    if (threadIdx.x == 0) *j.out_len = n;
-}
-
-static int vp8_encode_dev(const uint8_t* d_frame, size_t step, int width, int height, int channels, int quality,
-                          std::vector<uint8_t>* out, cudaStream_t st) {
-    Vp8EncJob j;
-    j.P.width = width;
-    j.P.height = height;
-    j.P.mb_w = (width + 15) >> 4;
-    j.P.mb_h = (height + 15) >> 4;
-    j.P.q = vp8enc::quality_to_q(quality);
-    j.P.filter_level = -1;  // chosen on the device, where the quantiser tables live
-    j.P.try_i4 = vp8_try_i4();
-    const int ys = j.P.mb_w * 16, yh = j.P.mb_h * 16;
-    const size_t ypl = (size_t)ys * yh, nmb = (size_t)j.P.mb_w * j.P.mb_h;
-    const size_t planes_b = round_up(ypl * 3 / 2, (size_t)256);
-    const size_t levels_b = round_up(nmb * 25 * 16 * 2, (size_t)256), modes_b = round_up(nmb * vp8enc::kModeStride, (size_t)256);
-    j.part0_cap = round_up(nmb * 2 + 4096, (size_t)256);
-    j.tokens_cap = round_up(nmb * 2048 + 4096, (size_t)256);
-    j.out_cap = 16 + j.part0_cap + j.tokens_cap;
-    const size_t aux_b = vp8enc::kAuxBytes;  // statistics + probabilities of the bitstream pass (vp8_enc_core.h)
-    uint8_t* scratch = nullptr;
-    LP_CUDA_OK(cudaMallocAsync(&scratch, 256 + 2 * planes_b + levels_b + modes_b + j.part0_cap + j.tokens_cap + aux_b + j.out_cap, st));
-    uint8_t* p = scratch;
-    j.out_len = reinterpret_cast<size_t*>(p);
-    p += 256;
-    uint8_t* src = p;
-    p += planes_b;
-    uint8_t* rec = p;
-    p += planes_b;
-    j.B.sy = src;
-    j.B.su = src + ypl;
-    j.B.sv = src + ypl + ypl / 4;
-    j.B.ry = rec;
-    j.B.ru = rec + ypl;
-    j.B.rv = rec + ypl + ypl / 4;
-    j.B.levels = reinterpret_cast<int16_t*>(p);
-    p += levels_b;
-    j.B.modes = p;
-    p += modes_b;
-    j.part0 = p;
-    p += j.part0_cap;
-    j.tokens = p;
-    p += j.tokens_cap;
-    j.aux = p;
-    p += aux_b;
-    j.out = p;
-    dim3 grid(ceil_div(ys / 2, 128), yh / 2);
-    vp8_planes_kernel<<<grid, 128, 0, st>>>(d_frame, step, channels, width, height, ys, yh, src, src + ypl, src + ypl + ypl / 4);
-    vp8_encode_kernel<<<1, 32, 0, st>>>(j);
-    g_launches += 2;
-    size_t n = 0;
-    int rc = LP_OK;
-    if (cudaMemcpyAsync(&n, j.out_len, sizeof(n), cudaMemcpyDeviceToHost, st) != cudaSuccess ||
-        cudaStreamSynchronize(st) != cudaSuccess)
-        rc = LP_ERR_CUDA;
-    if (!rc && (n == 0 || n > j.out_cap)) rc = LP_ERR_INVALID_IMAGE;  // (n > out_cap cannot come from the kernel)
-    if (!rc) {
-        out->resize(n);
-        if (cudaMemcpy(out->data(), j.out, n, cudaMemcpyDeviceToHost) != cudaSuccess) rc = LP_ERR_CUDA;
-    }
-    cudaFreeAsync(scratch, st);
-    return rc;
-}
-
-// ------------------------------------------------------------------ batched lossy encode
-// N frames of one geometry per launch (the batch ABI, xbatch.cu): the per-frame work is the same code as
-// above, one frame per warp (lane 0 walks the macroblocks and the boolean coder -- a serial dependency
-// chain per frame, so the parallelism is across frames), alpha planes through one CTA per frame.
-
+// BGR(A) -> padded Y / U / V planes (edge replication up to the macroblock grid); one chroma sample = 2x2 luma.
 __global__ void vp8_planes_batch_kernel(const uint8_t* frames, size_t img_stride, size_t step, int channels, int width,
                                         int height, int ys, int yh, uint8_t* planes, size_t planes_stride) {
     const int cx = blockIdx.x * blockDim.x + threadIdx.x, cy = blockIdx.y;
@@ -1167,33 +1067,19 @@ size_t webp_encoder_write(webp_encoder e, const opencv_mat src, const int* opt, 
     const int channels = type == CV_8UC4 ? 4 : 3;
     cudaStream_t st = thread_stream();
     EncodedFrame f;
-    f.width = cols;
-    f.height = rows;
-    f.lossless = lossless;
-    f.has_alpha = channels == 4;
-    f.duration = delay;
-    int rc;
     if (lossless) {
-        rc = vp8l_encode_dev(dev, step, cols, rows, channels, &f.image, st);
+        f.width = cols;
+        f.height = rows;
+        f.has_alpha = channels == 4;
+        if (vp8l_encode_dev(dev, step, cols, rows, channels, &f.image, st)) return 0;
     } else {
-        rc = vp8_encode_dev(dev, step, cols, rows, channels, (int)quality, &f.image, st);
-        if (!rc && channels == 4) {
-            // libwebp writes no ALPH chunk for an opaque picture (WebPEncode: WebPPictureHasTransparency)
-            uint8_t* plane = nullptr;
-            if (cudaMallocAsync(&plane, (size_t)cols * rows + 512, st) != cudaSuccess) return 0;
-            uint32_t* d_flag = reinterpret_cast<uint32_t*>(plane + round_up((size_t)cols * rows, (size_t)256));
-            cudaMemsetAsync(d_flag, 0, 4, st);
-            dim3 grid(ceil_div(cols, 256), rows, 1);
-            extract_alpha_batch_kernel<<<grid, 256, 0, st>>>(dev, 0, step, cols, rows, plane, d_flag);
-            g_launches++;
-            uint32_t flag = 0;
-            if (cudaMemcpyAsync(&flag, d_flag, 4, cudaMemcpyDeviceToHost, st) != cudaSuccess || cudaStreamSynchronize(st) != cudaSuccess) rc = LP_ERR_CUDA;
-            f.has_alpha = flag != 0;
-            if (!rc && flag) rc = vp8l_encode_dev(plane, (size_t)cols, cols, rows, 1, &f.alph, st);
-            cudaFreeAsync(plane, st);
-        }
+        std::vector<WebpEncodedFrame> one;
+        if (webp_encode_lossy_batch(dev, 0, step, cols, rows, channels, 1, (int)quality, &one, st) || one[0].image.empty())
+            return 0;
+        f = std::move(one[0]);
     }
-    if (rc) return 0;
+    f.lossless = lossless;
+    f.duration = delay;
     if (e->frames.empty()) e->first_frame_delay = delay;
     const size_t size = f.image.size() + f.alph.size();
     e->frames.push_back(std::move(f));
