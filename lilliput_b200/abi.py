@@ -339,6 +339,13 @@ class Batch:
                                          C.c_void_p, C.c_void_p]
         l.lp_batch_last_launches.restype = C.c_int
         l.lp_batch_last_launches.argtypes = [C.c_void_p]
+        l.lp_batch_chunk.restype = C.c_int
+        l.lp_batch_chunk.argtypes = [C.c_void_p]
+        for name in ("lp_batch_decoded_dev", "lp_batch_resized_dev"):
+            getattr(l, name).restype = C.c_void_p
+            getattr(l, name).argtypes = [C.c_void_p, C.POINTER(C.c_size_t)]
+        l.lp_memcpy_d2h.restype = C.c_int
+        l.lp_memcpy_d2h.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t]
         cfg = _BatchConfig(device, max_images, src_w, src_h, dst_w, dst_h, resize_method, quality,
                            max_in_bytes, out_cap, chunk)
         self.h = l.lp_batch_create(C.byref(cfg))
@@ -410,6 +417,32 @@ class Batch:
 
     def last_launches(self):
         return self.lib.l.lp_batch_last_launches(self.h)
+
+    def _copy_back(self, getter, n):
+        stride = C.c_size_t(0)
+        ptr = getter(self.h, C.byref(stride))
+        buf = np.empty((n, stride.value), dtype=np.uint8)
+        rc = self.lib.l.lp_memcpy_d2h(buf.ctypes.data, ptr, buf.nbytes)
+        if rc:
+            raise LilliputError(rc)
+        return buf
+
+    def decoded_windows(self, n: int, win_h: int) -> np.ndarray:
+        """The decoded pixel windows of the last `run()`: (n, win_h, row stride in bytes), u8 BGR, rows padded as
+        the decoder wrote them.  The frame buffer holds one chunk, so the staged batch must fit in one."""
+        if n > self.lib.l.lp_batch_chunk(self.h):
+            raise ValueError("the decoded frames of a multi-chunk batch are not kept")
+        buf = self._copy_back(self.lib.l.lp_batch_decoded_dev, n)
+        if buf.shape[1] % win_h:
+            raise ValueError(f"frame stride {buf.shape[1]} is not a whole number of {win_h} rows")
+        return buf.reshape(n, win_h, buf.shape[1] // win_h)
+
+    def resized_frames(self, n: int, w: int, h: int) -> np.ndarray:
+        """The resized frames of the last `run()`: (n, h, w, 3) u8 BGR."""
+        buf = self._copy_back(self.lib.l.lp_batch_resized_dev, n)
+        if buf.shape[1] != w * h * 3:
+            raise ValueError(f"resized frames are {buf.shape[1]} bytes, not {w}x{h}x3")
+        return buf.reshape(n, h, w, 3)
 
 
 # ----------------------------------------------------------------------------------------------

@@ -742,13 +742,14 @@ __device__ __forceinline__ void idct_phase(const JpegDecodeItem& it, const TileC
     }
 }
 
-// Value of component c at full-resolution pixel (x, y): libjpeg-turbo jdsample.c.
+// Value of component c at full-resolution pixel (x, y): libjpeg-turbo jdsample.c.  jinit_upsampler picks the
+// h2v1 / h2v2 triangle filters only for components more than two samples wide; narrower ones are replicated.
 __device__ __forceinline__ int upsampled(const JpegDecodeItem& it, const TileCtx& t, const uint8_t* tile, int c,
                                          int maxh, int maxv, int x, int y) {
     const int hr = maxh / t.h[c], vr = maxv / t.v[c];
     const int cw = it.dw[c], ch = it.dh[c];
     if (hr == 1 && vr == 1) return tile[tile_row(t, c, y) + x];
-    if (hr == 2 && vr == 2) {
+    if (hr == 2 && vr == 2 && cw > 2) {
         const int cy = y >> 1, i = x >> 1;
         const int fy = min(max((y & 1) ? cy + 1 : cy - 1, 0), ch - 1);
         const uint8_t* s0 = tile + tile_row(t, c, cy);
@@ -761,7 +762,7 @@ __device__ __forceinline__ int upsampled(const JpegDecodeItem& it, const TileCtx
         if (i == 0) return (cs * 4 + 8) >> 4;
         return (cs * 3 + 3 * s0[i - 1] + s1[i - 1] + 8) >> 4;
     }
-    if (hr == 2 && vr == 1) {
+    if (hr == 2 && vr == 1 && cw > 2) {
         const uint8_t* s = tile + tile_row(t, c, y);
         const int i = x >> 1;
         if (x & 1) return (i == cw - 1) ? s[i] : (3 * s[i] + s[i + 1] + 2) >> 2;
@@ -772,7 +773,7 @@ __device__ __forceinline__ int upsampled(const JpegDecodeItem& it, const TileCtx
         const int fy = min(max((y & 1) ? cy + 1 : cy - 1, 0), ch - 1);
         return (3 * tile[tile_row(t, c, cy) + x] + tile[tile_row(t, c, fy) + x] + ((y & 1) ? 2 : 1)) >> 2;
     }
-    return tile[tile_row(t, c, y / vr) + x / hr];  // int_upsample (replication)
+    return tile[tile_row(t, c, y / vr) + x / hr];  // int_upsample / h2v1_upsample / h2v2_upsample (replication)
 }
 
 // 4:2:0, 16-byte aligned: 16 consecutive pixels of row y from x0 (one 16-byte Y load, four 8-byte chroma loads,

@@ -334,7 +334,9 @@ static int exif_orientation(const uint8_t* p, size_t n) {
 }
 
 /* jdsample.c: fancy (triangle) upsampling.  `get(r)` rows are clamped to the
- * component's true downsampled height; columns to its true downsampled width. */
+ * component's true downsampled height; columns to its true downsampled width.
+ * jinit_upsampler picks the h2v1 / h2v2 triangle filters only for components more
+ * than two samples wide; narrower ones are replicated (h2v1_upsample / h2v2_upsample). */
 static void upsample_rows(const Comp* c, int maxh, int maxv, int y, int out_w, uint8_t* out) {
     int stride = c->bw * 8;
     int hr = maxh / c->h, vr = maxv / c->v;
@@ -343,13 +345,12 @@ static void upsample_rows(const Comp* c, int maxh, int maxv, int y, int out_w, u
         memcpy(out, c->plane + (size_t)y * stride, out_w);
         return;
     }
-    if (hr == 2 && vr == 1) { /* h2v1_fancy_upsample */
+    if (hr == 2 && vr == 1 && cw > 2) { /* h2v1_fancy_upsample */
         const uint8_t* s = c->plane + (size_t)y * stride;
         for (int i = 0; i < cw; i++) {
             int l = s[i > 0 ? i - 1 : 0], r = s[i + 1 < cw ? i + 1 : cw - 1], v = s[i] * 3;
             int a = (i == 0) ? s[0] : (v + l + 1) >> 2;
             int b = (i == cw - 1) ? s[i] : (v + r + 2) >> 2;
-            if (cw == 1) { a = b = s[0]; }
             if (2 * i < out_w) out[2 * i] = (uint8_t)a;
             if (2 * i + 1 < out_w) out[2 * i + 1] = (uint8_t)b;
         }
@@ -364,7 +365,7 @@ static void upsample_rows(const Comp* c, int maxh, int maxv, int y, int out_w, u
         for (int i = 0; i < out_w; i++) out[i] = (uint8_t)((s0[i] * 3 + s1[i] + bias) >> 2);
         return;
     }
-    if (hr == 2 && vr == 2) { /* h2v2_fancy_upsample */
+    if (hr == 2 && vr == 2 && cw > 2) { /* h2v2_fancy_upsample */
         int cy = y >> 1, far = (y & 1) ? cy + 1 : cy - 1;
         if (far < 0) far = 0;
         if (far > c->dh - 1) far = c->dh - 1;
@@ -381,7 +382,7 @@ static void upsample_rows(const Comp* c, int maxh, int maxv, int y, int out_w, u
         }
         return;
     }
-    /* int_upsample: pixel replication for other integral ratios */
+    /* int_upsample / h2v1_upsample / h2v2_upsample: pixel replication */
     const uint8_t* s = c->plane + (size_t)(y / vr) * stride;
     for (int i = 0; i < out_w; i++) out[i] = s[i / hr];
 }

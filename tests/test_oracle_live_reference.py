@@ -91,6 +91,17 @@ def _jpeg_files(rng):
         ok, enc = cv2.imencode(".jpg", img, opts)
         assert ok
         out.append((f"{w}x{h} gray={gray} opts={opts}", enc.tobytes()))
+    # frames 4 px wide or less, where libjpeg-turbo replicates 4:2:0 / 4:2:2 chroma instead of filtering it; their own
+    # generator, so the draws above stay as they were
+    narrow = np.random.default_rng(91)
+    for w in (1, 2, 3, 4):
+        for sf in (0x221111, 0x211111):
+            h = int(narrow.integers(1, 40))
+            img = _rand_img(narrow, h, w, 3)
+            opts = [cv2.IMWRITE_JPEG_QUALITY, int(narrow.integers(1, 101)), cv2.IMWRITE_JPEG_SAMPLING_FACTOR, sf]
+            ok, enc = cv2.imencode(".jpg", img, opts)
+            assert ok
+            out.append((f"{w}x{h} opts={opts}", enc.tobytes()))
     return out
 
 
