@@ -290,6 +290,14 @@ size_t gif_plan_device_bytes(const GifAnimPlan* p);
 int gif_decode_batch(GifAnimPlan* const* plans, const uint8_t* const* files, const size_t* file_len, int n,
                      uint8_t* d_scratch, size_t scratch_bytes, uint8_t* d_canvases, size_t canvas_stride,
                      const int* first_frame, int* h_status, cudaStream_t st);
+// device scratch gif_encode_batch needs for one animation whose frames are resized to ow x oh
+size_t gif_plan_encode_bytes(const GifAnimPlan* p, int ow, int oh);
+// GIF files of `n` animations whose frames, resized to ow x oh BGRA, sit at d_frames + (first_frame[a] + f) * frame_stride:
+// palette mapping + LZW of every frame (device), container assembly into out[a] (host), status and out_len per
+// animation as lp_transform reports them.  h_stage: pinned staging for the code streams.
+int gif_encode_batch(GifAnimPlan* const* plans, int n, const uint8_t* d_frames, size_t frame_stride, int ow, int oh,
+                     const int* first_frame, uint8_t* d_scratch, size_t scratch_bytes, uint8_t* h_stage, size_t stage_bytes,
+                     uint8_t* const* out, size_t out_cap, size_t* out_len, int* status, size_t* d2h, cudaStream_t st);
 
 // ---- pixel_ops.cu --------------------------------------------------------------------------
 int orient_launch(const uint8_t* src, int w, int h, int channels, int orientation, uint8_t* dst,

@@ -12,9 +12,10 @@
 //        WebP  -> VP8 key frames, one frame per warp (webp_decode.cu), resize
 //        GIF   -> every frame of every animation: LZW (one warp per frame), per-pixel compositor over the
 //                 frame sequence (gif_decode.cu), resize of every composited canvas
-//      and the sinks: JPEG (jpeg_encode.cu), lossy WebP still / animation (webp_encode.cu);
+//      and the sinks: JPEG (jpeg_encode.cu), lossy WebP still / animation (webp_encode.cu), GIF from GIF sources
+//      (palette mapping + LZW of every frame of the task, gif_decode.cu; the container assembled on the host);
 //   3. anything the grid path does not cover (progressive JPEG sources, EXIF-rotated sources, ICC profiles to carry,
-//      lossless WebP output, PNG / GIF output ...) and any item whose grid stage fails goes through
+//      lossless WebP output, PNG output, GIF output from other formats ...) and any item whose grid stage fails goes through
 //      lp_transform on a worker thread -- still this library's device kernels, one image per call -- so the
 //      status and bytes of EVERY item are what lp_transform would have returned.
 // Two worker lanes, each with half of the device arena and its own stream, process chunks of groups
@@ -47,7 +48,7 @@ lp_batch* batch_create_in(const lp_batch_config* cfg, uint8_t* dev_arena, size_t
 namespace {
 
 enum Kind { K_FALLBACK = 0, K_JPEG = 1, K_PNG = 2, K_WEBP = 3, K_GIF = 4 };
-enum Sink { S_NONE = 0, S_JPEG = 1, S_WEBP = 2 };
+enum Sink { S_NONE = 0, S_JPEG = 1, S_WEBP = 2, S_GIF = 3 };
 
 struct XItem {
     Kind kind = K_FALLBACK;
@@ -180,6 +181,7 @@ static void parse_item(lp_xbatch* X, int i) {
         return;
     }
     if (!memcmp(d, png_sig, 8)) {
+        if (X->sink == S_GIF) return;  // GIF output needs a GIF source: per image (ErrGifEncoderNeedsDecoder)
         std::unique_ptr<PngHeader> h(new PngHeader);
         if (png_parse(d, n, h.get()) != LP_OK) return;
         if (h->orientation != 1 || h->idat.empty() || h->idat_total < 2) return;
@@ -205,6 +207,7 @@ static void parse_item(lp_xbatch* X, int i) {
         return;
     }
     if (!memcmp(d, "RIFF", 4) && !memcmp(d + 8, "WEBP", 4)) {
+        if (X->sink == S_GIF) return;
         WebpStillInfo w;
         if (!webp_still_info(d, n, &w) || !w.simple_lossy) return;
         if (w.width > max_side || w.height > max_side) return;
@@ -217,9 +220,11 @@ static void parse_item(lp_xbatch* X, int i) {
         return;
     }
     if (!memcmp(d, "GIF8", 4)) {
-        if (X->sink != S_WEBP || X->opt.disable_animated_output || X->opt.max_encode_frames != 0 ||
+        if ((X->sink != S_WEBP && X->sink != S_GIF) || X->opt.disable_animated_output || X->opt.max_encode_frames != 0 ||
             X->opt.max_encode_duration_ns != 0)
             return;
+        // a GIF written with no time to encode fails with ErrEncodeTimeout after its first frame (Transform's deadline)
+        if (X->sink == S_GIF && X->opt.encode_timeout_ns <= 0) return;
         GifAnimPlan* p = gif_plan_parse(d, n, 4096);
         if (!p) return;
         int w = 0, h = 0, nf = 0;
@@ -227,7 +232,8 @@ static void parse_item(lp_xbatch* X, int i) {
         it.w = w;
         it.h = h;
         it.ch = 4;
-        if (nf < 2 || w > max_side || h > max_side || !plan_geometry(X->opt, &it)) {  // stills and odd files: per image
+        // stills to WebP and odd files: per image (the GIF writer is the same for one frame)
+        if ((nf < 2 && X->sink == S_WEBP) || w > max_side || h > max_side || !plan_geometry(X->opt, &it)) {
             gif_plan_free(p);
             return;
         }
@@ -619,7 +625,40 @@ static void run_webp(lp_xbatch* X, Lane& L, const std::vector<int>& idx) {
     for (int i : failed) push_fallback(X, i);
 }
 
-// ------------------------------------------------------------------ GIF groups (animations -> animated WebP)
+// ------------------------------------------------------------------ GIF groups (animations -> animated WebP or GIF)
+
+// GIF sink: palette mapping + LZW of every resized frame of the task in one set of launches, the code streams packed
+// and copied home at once, each file assembled on the host from the plan's container metadata
+static void gif_sink(lp_xbatch* X, Lane& L, Bump& bump, const std::vector<int>& idx, const std::vector<int>& first,
+                     const std::vector<GifAnimPlan*>& plans, const std::vector<int>& st, const uint8_t* d_resized,
+                     size_t out_stride) {
+    const int na = (int)idx.size();
+    const XItem& g = X->items[idx[0]];
+    size_t bytes = 0;
+    for (GifAnimPlan* p : plans) bytes += gif_plan_encode_bytes(p, g.ow, g.oh);
+    uint8_t* d_scratch = bump.take<uint8_t>(bytes);
+    std::vector<uint8_t*> out((size_t)na);
+    std::vector<size_t> olen((size_t)na, 0);
+    std::vector<int> ost((size_t)na, LP_OK);
+    for (int a = 0; a < na; a++) out[a] = X->out[idx[a]];
+    cudaEventRecord(L.ev[2], L.st);
+    int rc = d_scratch ? gif_encode_batch(plans.data(), na, d_resized, out_stride, g.ow, g.oh, first.data(), d_scratch, bytes,
+                                          L.host, L.host_bytes, out.data(), X->out_cap, olen.data(), ost.data(), &L.d2h, L.st)
+                       : LP_ERR_BUF_TOO_SMALL;
+    cudaEventRecord(L.ev[3], L.st);
+    cudaEventSynchronize(L.ev[3]);
+    lane_time(L, 2, 3, &L.ms_encode);
+    for (int a = 0; a < na; a++) {
+        const int i = idx[a];
+        if (rc || st[a] != 0) {  // a corrupt code stream: the per-image path reports the precise error
+            push_fallback(X, i);
+            continue;
+        }
+        X->status[i] = ost[a];
+        X->out_len[i] = olen[a];
+    }
+    if (rc) cudaGetLastError();
+}
 
 static void run_gif(lp_xbatch* X, Lane& L, const std::vector<int>& idx) {
     const int na = (int)idx.size();
@@ -667,6 +706,10 @@ static void run_gif(lp_xbatch* X, Lane& L, const std::vector<int>& idx) {
     }
     lane_time(L, 0, 1, &L.ms_decode);
     lane_time(L, 1, 2, &L.ms_resize);
+    if (X->sink == S_GIF) {
+        gif_sink(X, L, bump, idx, first, plans, st, d_resized, out_stride);
+        return;
+    }
     cudaEventRecord(L.ev[2], L.st);
     std::vector<WebpEncodedFrame> frames;
     int rc = webp_encode_lossy_batch(d_resized, out_stride, (size_t)g.ow * 4, g.ow, g.oh, 4, nf, X->quality, &frames, L.st);
@@ -866,7 +909,8 @@ static size_t item_device_bytes(const lp_xbatch* X, const XItem& it, int i) {
         case K_WEBP:
             return X->in_len[i] + (size_t)it.w * it.h * 3 + outb + 4096;
         case K_GIF:
-            return gif_plan_device_bytes(it.gif) + (size_t)it.gif_frames * ((size_t)it.w * it.h * 4 + outb) + 8192;
+            return gif_plan_device_bytes(it.gif) + (size_t)it.gif_frames * ((size_t)it.w * it.h * 4 + outb) + 8192 +
+                   (X->sink == S_GIF ? gif_plan_encode_bytes(it.gif, it.ow, it.oh) : 0);
         default:
             return 0;
     }
@@ -913,6 +957,8 @@ extern "C" int lp_xbatch_transform(lp_xbatch* X, const uint8_t* const* in, const
         const int q = option_value(*opt, CV_IMWRITE_WEBP_QUALITY, 100);
         X->quality = q < 1 ? 1 : q;
         X->sink = q > 100 ? S_NONE : S_WEBP;  // lossless output: per image
+    } else if (ext == ".gif") {
+        X->sink = S_GIF;
     }
     parallel_for(n, X->threads, [&](int i) { parse_item(X, i); });
     const auto t1 = std::chrono::steady_clock::now();
