@@ -828,6 +828,31 @@ LP_VP8_HD size_t partition_scratch_cap(const Params& P, int part, int nparts) {
     return (size_t)partition_rows(P, part, nparts) * (size_t)P.mb_w * 2048 + 64;
 }
 
+// ---- scratch sizing: ONE rule for the device launcher (webp_encode.cu) and the host build (oracle_webp.cpp), so that
+// the CPU tests run the encoder under exactly the device's limits.
+// Token partitions: the layout above, 2 KiB per macroblock (the worst partition measured uses well under half of it).
+LP_VP8_HD size_t token_scratch_bytes(const Params& P) { return (size_t)P.mb_w * P.mb_h * 2048 + 4096; }
+// First partition: a worst-case bound, so that it never overflows below the format's limit.  A boolean moves at most
+// log2(range / new range) < 8 bits out of the coder, the coder adds 4 bytes on flush.  Summed over the costliest path
+// through the fixed probabilities (oracle_webp.cpp: vp8_cpu_part0_worst_bits computes it, the tests compare) the frame
+// header takes at most 16723 bits and a macroblock at most 228 -- skip flag, sixteen sub-block modes in adversarial
+// contexts, chroma mode (8 bits per boolean would say 1216).  The header term holds for the fields write_part0 codes
+// today -- no segmentation, no loop-filter deltas, no quantiser deltas; a header that codes more needs a new bound (the
+// test comparing it with vp8_cpu_part0_worst_bits fails first).  The partition's size is a 19-bit field of the frame
+// tag: a first partition that outgrows kPart0Max bytes makes no valid stream whatever the scratch.
+constexpr uint32_t kPart0HeaderBits = 16768, kPart0MbBits = 232;
+constexpr size_t kPart0Max = (1u << 19) - 1;
+LP_VP8_HD size_t part0_scratch_bytes(const Params& P) {
+    const size_t bound = ((size_t)kPart0HeaderBits + (size_t)P.mb_w * P.mb_h * kPart0MbBits + 7) / 8 + 4 + 64;
+    return bound < kPart0Max ? bound : kPart0Max;
+}
+// write_bitstream's result when the first partition did not fit part0_scratch_bytes, i.e. would exceed the format's
+// limit: large frames of fine detail coded with 4x4 prediction (4096 x 4096 noise: ~9 bytes per macroblock, 64 K
+// macroblocks).  The encoder's callers then code the frame once more with 16x16 prediction only (Params::try_i4 = 0,
+// < 1 byte of modes per macroblock, the idea of libwebp's partition_limit); a frame that does not fit even so (noise
+// near 16383 x 16383) stays refused.
+constexpr size_t kPart0TooLarge = ~(size_t)0;
+
 // aux accessors
 LP_VP8_INL uint32_t* aux_stats(uint8_t* aux) { return reinterpret_cast<uint32_t*>(aux + kAuxStatsOff); }
 LP_VP8_INL uint32_t* aux_counts(uint8_t* aux) { return reinterpret_cast<uint32_t*>(aux + kAuxCountsOff); }
@@ -1035,7 +1060,7 @@ LP_VP8_FN size_t write_frame_header(const Params& P, size_t part0_len, const siz
 }
 
 // part0 / tokens / aux (kAuxBytes, 4-byte aligned) are scratch areas; `out` receives the "VP8 " chunk payload.  Returns
-// the payload size, 0 when it does not fit.
+// the payload size, kPart0TooLarge when the first partition outgrew part0_cap, 0 when anything else does not fit.
 LP_VP8_FN size_t write_bitstream(const Params& P, const Buffers& B, uint8_t* part0, size_t part0_cap, uint8_t* tokens,
                                  size_t tokens_cap, uint8_t* aux, uint8_t* out, size_t out_cap) {
     const int nparts = 1 << log2_partitions(P);
@@ -1045,6 +1070,7 @@ LP_VP8_FN size_t write_bitstream(const Params& P, const Buffers& B, uint8_t* par
         if (stats_partition(q, nparts)) walk_partition<false>(P, B, q, nparts, aux, nullptr, 0);
     finish_statistics(aux, 0, 1);
     const size_t part0_len = write_part0(P, B, aux, part0, part0_cap);
+    if (!part0_len) return kPart0TooLarge;
     size_t sizes[8];
     for (int q = 0; q < nparts; q++)
         sizes[q] = walk_partition<true>(P, B, q, nparts, aux, tokens + partition_scratch_off(P, q, nparts), partition_scratch_cap(P, q, nparts));

@@ -573,6 +573,7 @@ __device__ size_t vp8_write_bitstream_warp(const vp8enc::Params& P, const vp8enc
         mine = vp8enc::write_part0(P, B, aux, part0, part0_cap);
     __syncwarp();
     const size_t part0_len = (size_t)__shfl_sync(FULL, mine, nparts);
+    if (!part0_len) return vp8enc::kPart0TooLarge;
     size_t sizes[8];
 #pragma unroll
     for (int q = 0; q < 8; q++) sizes[q] = (size_t)__shfl_sync(FULL, mine, q);
@@ -637,7 +638,7 @@ struct Vp8EncBatch {
     size_t part0_cap, tokens_cap;
     uint8_t* out;           // n * out_cap
     size_t out_cap;
-    uint32_t* out_len;      // n (0 = did not fit)
+    uint32_t* out_len;      // n (0 = did not fit, (uint32_t)kPart0TooLarge = first partition beyond the format's limit)
     int n;
 };
 
@@ -755,9 +756,12 @@ __global__ void __launch_bounds__(kPackThreads)
     if (threadIdx.x == 0) total_bits[f] = base;
 }
 
-int webp_encode_lossy_batch(const uint8_t* d_frames, size_t img_stride, size_t row_step, int width, int height,
-                            int channels, int n, int quality, std::vector<WebpEncodedFrame>* out, cudaStream_t st) {
+// `too_large[i]` = 1 when frame i failed only because its first partition outgrew the format's limit
+static int lossy_batch(const uint8_t* d_frames, size_t img_stride, size_t row_step, int width, int height, int channels,
+                       int n, int quality, int try_i4, std::vector<WebpEncodedFrame>* out, std::vector<uint8_t>* too_large,
+                       cudaStream_t st) {
     out->assign((size_t)n, WebpEncodedFrame());
+    too_large->assign((size_t)n, 0);
     if (n <= 0) return LP_OK;
     if (width > 16383 || height > 16383 || (channels != 3 && channels != 4)) return LP_ERR_INVALID_IMAGE;
     Vp8EncBatch b;
@@ -767,22 +771,22 @@ int webp_encode_lossy_batch(const uint8_t* d_frames, size_t img_stride, size_t r
     b.P.mb_h = (height + 15) >> 4;
     b.P.q = vp8enc::quality_to_q(quality);
     b.P.filter_level = -1;
-    b.P.try_i4 = vp8_try_i4();
+    b.P.try_i4 = try_i4;
     b.n = n;
     const int ys = b.P.mb_w * 16, yh = b.P.mb_h * 16;
     const size_t ypl = (size_t)ys * yh, nmb = (size_t)b.P.mb_w * b.P.mb_h;
     const size_t planes_b = round_up(ypl * 3 / 2, (size_t)256);
     const size_t levels_b = round_up(nmb * 25 * 16 * 2, (size_t)256), modes_b = round_up(nmb * vp8enc::kModeStride, (size_t)256);
-    b.part0_cap = round_up(nmb * 2 + 4096, (size_t)256);
-    b.tokens_cap = round_up(nmb * 2048 + 4096, (size_t)256);
+    b.part0_cap = vp8enc::part0_scratch_bytes(b.P);  // the sizes the host build of the core encodes with, too
+    b.tokens_cap = vp8enc::token_scratch_bytes(b.P);
     const size_t aux_b = vp8enc::kAuxBytes;  // statistics + probabilities of the bitstream pass (vp8_enc_core.h)
     b.off_src = 0;
     b.off_rec = planes_b;
     b.off_levels = 2 * planes_b;
     b.off_modes = b.off_levels + levels_b;
     b.off_part0 = b.off_modes + modes_b;
-    b.off_tokens = b.off_part0 + b.part0_cap;
-    b.off_aux = b.off_tokens + b.tokens_cap;
+    b.off_tokens = b.off_part0 + round_up(b.part0_cap, (size_t)256);
+    b.off_aux = b.off_tokens + round_up(b.tokens_cap, (size_t)256);
     b.stride = b.off_aux + aux_b;
     // the stream is the two partitions back to back: a slot that holds what they can hold never overflows;
     // real frames use a few per cent of it, so the slots are compacted on the device before they cross PCIe
@@ -915,6 +919,7 @@ int webp_encode_lossy_batch(const uint8_t* d_frames, size_t img_stride, size_t r
             f.height = height;
             f.lossless = false;
             f.has_alpha = alpha && transp[i];
+            (*too_large)[i] = lens[i] == (uint32_t)vp8enc::kPart0TooLarge;
             if (lens[i] == 0 || lens[i] > b.out_cap) { f.image.clear(); continue; }  // caller reports the item
             f.image.assign(home.data() + off[i], home.data() + off[i] + lens[i]);
             if (f.has_alpha) {
@@ -924,6 +929,23 @@ int webp_encode_lossy_batch(const uint8_t* d_frames, size_t img_stride, size_t r
         }
     } while (0);
     cudaFreeAsync(scratch, st);
+    return rc;
+}
+
+int webp_encode_lossy_batch(const uint8_t* d_frames, size_t img_stride, size_t row_step, int width, int height,
+                            int channels, int n, int quality, std::vector<WebpEncodedFrame>* out, cudaStream_t st) {
+    const int try_i4 = vp8_try_i4();
+    std::vector<uint8_t> too_large;
+    int rc = lossy_batch(d_frames, img_stride, row_step, width, height, channels, n, quality, try_i4, out, &too_large, st);
+    // a frame whose first partition outgrew the format's limit (vp8enc::kPart0TooLarge): once more, alone, with 16x16
+    // prediction only.  Rare (large frames of fine detail), so one launch per such frame.
+    for (int i = 0; rc == LP_OK && try_i4 && i < n; i++) {
+        if (!too_large[i]) continue;
+        std::vector<WebpEncodedFrame> one;
+        std::vector<uint8_t> again;
+        rc = lossy_batch(d_frames + (size_t)i * img_stride, 0, row_step, width, height, channels, 1, quality, 0, &one, &again, st);
+        if (rc == LP_OK) (*out)[i] = std::move(one[0]);
+    }
     return rc;
 }
 

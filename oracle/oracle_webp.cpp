@@ -10,6 +10,8 @@
 // by the reference), and in the build container a 1 496-configuration libwebp encoder sweep.
 // libwebp 1.5.0 is the algorithm's home (deps/build-deps-linux.sh:235; call sites ref webp.cpp:65-112,
 // 309-350); the bitstream formats are RFC 6386 (VP8) and the WebP lossless specification (VP8L).
+#include <algorithm>
+#include <cmath>
 #include <cstdlib>
 #include <cstring>
 #include <vector>
@@ -149,19 +151,100 @@ static long vp8_cpu_encode_impl(const uint8_t* frame, size_t step, int w, int h,
     std::vector<uint8_t> modes((size_t)P.mb_w * P.mb_h * vp8enc::kModeStride);
     vp8enc::Buffers B{sy.data(), su.data(), sv.data(), ry.data(), ru.data(), rv.data(), levels.data(), modes.data()};
     vp8enc::analyse_and_reconstruct(P, B);
-    const size_t scratch = (size_t)P.mb_w * P.mb_h * 2048 + 4096;  // the layout vp8enc::partition_scratch_off assumes
-    std::vector<uint8_t> part0(scratch), tokens(scratch), aux(vp8enc::kAuxBytes);
-    return (long)vp8enc::write_bitstream(P, B, part0.data(), part0.size(), tokens.data(), tokens.size(), aux.data(), out, cap);
+    // the device's scratch sizes (webp_encode_lossy_batch)
+    std::vector<uint8_t> part0(vp8enc::part0_scratch_bytes(P)), tokens(vp8enc::token_scratch_bytes(P)), aux(vp8enc::kAuxBytes);
+    const size_t n = vp8enc::write_bitstream(P, B, part0.data(), part0.size(), tokens.data(), tokens.size(), aux.data(), out, cap);
+    return n == vp8enc::kPart0TooLarge ? -1 : (long)n;
 }
-// the encoder as the device runs it (vp8enc::kTryI4: whether macroblocks weigh 4x4 against 16x16 prediction)
+// the encoder as the device runs it (vp8enc::kTryI4: whether macroblocks weigh 4x4 against 16x16 prediction; a frame
+// whose first partition outgrows the format's limit coded again with 16x16 prediction only).  Returns 0 = failed.
 extern "C" long vp8_cpu_encode(const uint8_t* frame, size_t step, int w, int h, int channels, int quality,
                                int filter_level, uint8_t* out, size_t cap) {
-    return vp8_cpu_encode_impl(frame, step, w, h, channels, quality, filter_level, vp8enc::kTryI4, out, cap);
+    long n = vp8_cpu_encode_impl(frame, step, w, h, channels, quality, filter_level, vp8enc::kTryI4, out, cap);
+    if (n < 0 && vp8enc::kTryI4) n = vp8_cpu_encode_impl(frame, step, w, h, channels, quality, filter_level, 0, out, cap);
+    return n < 0 ? 0 : n;
 }
-// ... and with the choice forced on or off (measurements, tests of both paths)
+// ... and with the choice forced on or off, no retry (measurements, tests of both paths).  Returns 0 = failed, -1 = the
+// first partition outgrew the format's limit.
 extern "C" long vp8_cpu_encode_i4(const uint8_t* frame, size_t step, int w, int h, int channels, int quality,
                                   int filter_level, int try_i4, uint8_t* out, size_t cap) {
     return vp8_cpu_encode_impl(frame, step, w, h, channels, quality, filter_level, try_i4, out, cap);
+}
+// the scratch the encoder gets for a w x h frame: [0] first partition, [1] token partitions
+extern "C" void vp8_cpu_scratch_bytes(int w, int h, size_t* sizes) {
+    vp8enc::Params P{};
+    P.width = w;
+    P.height = h;
+    P.mb_w = (w + 15) >> 4;
+    P.mb_h = (h + 15) >> 4;
+    sizes[0] = vp8enc::part0_scratch_bytes(P);
+    sizes[1] = vp8enc::token_scratch_bytes(P);
+}
+
+// The exact worst case of the first partition, from the format's fixed probabilities: what the sizing constants of
+// vp8_enc_core.h (kPart0HeaderBits, kPart0MbBits) must cover.  A boolean coded with probability `p` shifts the coder
+// log2(range / new range) bits out, and over a partition these sum (telescoping) to at least the bits written, so a
+// boolean's worst is that ratio's maximum over the ranges the coder can hold (128..255).  `header` gets the worst frame
+// header, `per_mb` the worst macroblock: skip flag at any probability, the costliest luma coding (sixteen sub-block modes,
+// every context chosen adversarially through the neighbours, by a walk over the four modes above the next block) and
+// the costliest chroma mode.
+static double bool_bits(int bit, int p) {
+    double worst = 0;
+    for (uint32_t r = 128; r < 256; r++) {
+        const uint32_t split = 1 + (((r - 1) * (uint32_t)p) >> 8);
+        const double b = std::log2((double)r / (double)(bit ? r - split : split));
+        worst = b > worst ? b : worst;
+    }
+    return worst;
+}
+static double bool_bits_any(int p) { return std::fmax(bool_bits(0, p), bool_bits(1, p)); }
+static double i4_mode_bits(int mode, const uint8_t* prob) {
+    const uint32_t nodes = vp8enc::kVp8BModePathNodes[mode], bits = vp8enc::kVp8BModePathBits[mode];
+    double b = 0;
+    for (int k = 0; k < (int)(bits >> 8); k++) b += bool_bits((int)((bits >> k) & 1u), prob[(nodes >> (4 * k)) & 15u]);
+    return b;
+}
+extern "C" void vp8_cpu_part0_worst_bits(double* header, double* per_mb) {
+    const double b128 = bool_bits_any(128);
+    double h = 29 * b128 + std::fmax(bool_bits(0, 128), bool_bits(1, 128) + 8 * b128);  // fixed fields, skip probability
+    const uint8_t* upd = &kVp8CoeffUpdateProba[0][0][0][0];
+    for (int i = 0; i < vp8enc::kNumProbas; i++) h += std::fmax(bool_bits(0, upd[i]), bool_bits(1, upd[i]) + 8 * b128);
+    *header = h;
+    double skip = 0;
+    for (int p = 1; p < 256; p++) skip = std::fmax(skip, bool_bits_any(p));
+    static double cost[10][10][10];  // [above][left][mode]
+    for (int t = 0; t < 10; t++)
+        for (int l = 0; l < 10; l++)
+            for (int m = 0; m < 10; m++) cost[t][l][m] = i4_mode_bits(m, kVp8BModesProba[t][l]);
+    // sub-blocks in raster order; the state is the mode last placed in each column (10^4 states).  Modes above the top
+    // row and left of the left column belong to the neighbours: any of the ten.
+    std::vector<double> best(10000, -1.0), next(10000);
+    best[0] = 0;
+    for (int n = 0; n < 16; n++) {
+        const int bx = n & 3, by = n >> 2;
+        std::fill(next.begin(), next.end(), -1.0);
+        for (int s = 0; s < 10000; s++) {
+            if (best[s] < 0) continue;
+            int col[4] = {s % 10, s / 10 % 10, s / 100 % 10, s / 1000};
+            for (int m = 0; m < 10; m++) {
+                double c = 0;
+                for (int t = 0; t < 10; t++)
+                    for (int l = 0; l < 10; l++)
+                        if ((by == 0 || t == col[bx]) && (bx == 0 || l == col[bx - 1])) c = std::fmax(c, cost[t][l][m]);
+                int nc[4] = {col[0], col[1], col[2], col[3]};
+                nc[bx] = m;
+                const int ns = nc[0] + 10 * nc[1] + 100 * nc[2] + 1000 * nc[3];
+                next[ns] = std::fmax(next[ns], best[s] + c);
+            }
+        }
+        best.swap(next);
+    }
+    double i4 = 0;
+    for (double b : best) i4 = std::fmax(i4, b);
+    i4 += bool_bits(0, 145);
+    const double i16 = bool_bits(1, 145) + std::fmax(bool_bits(1, 156) + b128, bool_bits(0, 156) + bool_bits_any(163));
+    const double uv = std::fmax(bool_bits(0, 142), bool_bits(1, 142) + std::fmax(bool_bits(0, 114), bool_bits(1, 114) + bool_bits_any(183)));
+    *per_mb = skip + std::fmax(i4, i16) + uv;
 }
 
 // Self-check of the data forms of the 4x4 predictors and of the sub-block mode costs (vp8_enc_core.h) against the code

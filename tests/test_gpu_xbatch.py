@@ -15,7 +15,7 @@ import pytest
 from lilliput_b200 import abi
 from lilliput_b200.synth import synth_image
 from tests.png_writer import write_png
-from tests.webp_util import psnr
+from tests.webp_util import frames_of, libwebp_decode, optional_reference, pillow_animation, psnr, riff
 
 pytestmark = pytest.mark.gpu
 T = 10**12
@@ -90,7 +90,7 @@ def test_mixed_batch_resize_method_and_quality(cuda_lib, xb, oracle):
     check_against_per_image(cuda_lib, xb, files, opt)
 
 
-def test_png_to_webp_config3_miniature(cuda_lib, ref_lib, xb, oracle):
+def test_png_to_webp_config3_miniature(cuda_lib, xb, oracle):
     files = [rgb_png(synth_image(500 + k, 384, 216, 4, noise=8.0)) for k in range(5)]
     files.append(rgb_png(synth_image(510, 384, 216, 3)))            # opaque RGB: no ALPH, simple file
     opaque = synth_image(511, 384, 216, 4)
@@ -100,14 +100,19 @@ def test_png_to_webp_config3_miniature(cuda_lib, ref_lib, xb, oracle):
                            EncodeOptions={abi.WebpQuality: 85}, EncodeTimeout_ns=T)
     outs, status = check_against_per_image(cuda_lib, xb, files, opt)
     assert status == [0] * len(files) and xb.stats()["grid_items"] == len(files)
-    # against the reference: its libwebp decodes our stream; alpha exact, colour close to the fitted source
+    # against libwebp (and the reference's shims where built): it decodes our stream; alpha exact, colour close to the
+    # fitted source
+    ref_lib = optional_reference()
     for k in (0, 5, 6):
         src = oracle.png_decode(files[k])
         src = src[0] if isinstance(src, tuple) else src
         fit = oracle.fit(src, 128, 128)
-        info, frames, _, rc = ref_lib.webp_frames(outs[k])
-        assert rc == 0
-        got = frames[0]
+        got = libwebp_decode(outs[k])
+        _, mine, _, rc = cuda_lib.webp_frames(outs[k])
+        assert rc == 0 and np.array_equal(mine[0], got)
+        if ref_lib:
+            info, frames, _, rc = ref_lib.webp_frames(outs[k])
+            assert rc == 0 and np.array_equal(frames[0], got)
         if k == 0:
             assert got.shape[2] == 4 and np.array_equal(got[:, :, 3], fit[:, :, 3])
         else:
@@ -115,7 +120,7 @@ def test_png_to_webp_config3_miniature(cuda_lib, ref_lib, xb, oracle):
         assert psnr(got[:, :, :3], fit[:, :, :3]) > 28.0
 
 
-def test_png_to_webp_config3_full_size(cuda_lib, ref_lib, xb, oracle):
+def test_png_to_webp_config3_full_size(cuda_lib, xb, oracle):
     """One BASELINE config 3 image at full size: 3840x2160 RGBA PNG (zlib level 6, Paeth) -> Fit 512x512 -> WebP
     q85 + alpha, through the batch call; == lp_transform, and the reference's decoder reads it back."""
     import struct
@@ -138,9 +143,13 @@ def test_png_to_webp_config3_full_size(cuda_lib, ref_lib, xb, oracle):
     outs, status = check_against_per_image(cuda_lib, xb, [png, png], opt)
     assert status == [0, 0] and xb.stats()["grid_items"] == 2
     fit = oracle.fit(img, 512, 512)
-    info, frames, _, rc = ref_lib.webp_frames(outs[0])
-    assert rc == 0 and np.array_equal(frames[0][:, :, 3], fit[:, :, 3])
-    assert psnr(frames[0][:, :, :3], fit[:, :, :3]) > 30.0
+    got = libwebp_decode(outs[0])
+    assert np.array_equal(got[:, :, 3], fit[:, :, 3])
+    assert psnr(got[:, :, :3], fit[:, :, :3]) > 30.0
+    ref_lib = optional_reference()
+    if ref_lib:
+        info, frames, _, rc = ref_lib.webp_frames(outs[0])
+        assert rc == 0 and np.array_equal(frames[0], got)
 
 
 def _gif(frames, duration=40, loop=0, **kw):
@@ -151,7 +160,7 @@ def _gif(frames, duration=40, loop=0, **kw):
     return bio.getvalue()
 
 
-def test_gif_to_animated_webp_config4(cuda_lib, ref_lib, xb, golden):
+def test_gif_to_animated_webp_config4(cuda_lib, xb, golden):
     pytest.importorskip("PIL")
     files = [golden[k].tobytes() for k in golden.files if k.startswith("gif_") and golden[k].ndim == 1][:6]
     base = synth_image(700, 1280, 720, 3, noise=0.0)
@@ -162,13 +171,28 @@ def test_gif_to_animated_webp_config4(cuda_lib, ref_lib, xb, golden):
                            EncodeOptions={abi.WebpQuality: 85}, EncodeTimeout_ns=T)
     outs, status = check_against_per_image(cuda_lib, xb, files, opt, cap=1 << 24)
     assert xb.stats()["grid_items"] >= 2
-    # the reference's libwebp reads the animation back: frame count, delays, loop count
+    # libwebp reads the animation back: frame count, delays, loop count; every frame, rewrapped as a still, decodes to
+    # the device's frame
     k = len(files) - 1
-    info, frames, metas, rc = ref_lib.webp_frames(outs[k])
-    assert rc == 0 and info["num_frames"] == 3 and info["loop_count"] == 3
-    assert [m["delay"] for m in metas] == [20, 70, 130]
-    info, frames, metas, rc = ref_lib.webp_frames(outs[k - 1])
-    assert rc == 0 and info["num_frames"] == 6 and frames[0].shape[:2] == (256, 256)
+    assert pillow_animation(outs[k])[:3] == (3, 3, [20, 70, 130])
+    assert pillow_animation(outs[k - 1])[0] == 6 and pillow_animation(outs[k - 1])[3] == (256, 256)
+    for out in outs:
+        _, mine, _, rc = cuda_lib.webp_frames(out)
+        assert rc == 0 and len(mine) == len(frames_of(out))
+        for f, (tag, payload, alph) in zip(mine, frames_of(out)):
+            chunks = [(b"VP8 ", payload)] if alph is None else [
+                (b"VP8X", bytes([0x10, 0, 0, 0]) + (f.shape[1] - 1).to_bytes(3, "little") + (f.shape[0] - 1).to_bytes(3, "little")),
+                (b"ALPH", alph), (tag, payload)]
+            got = libwebp_decode(riff(chunks))
+            assert np.array_equal(f[:, :, :got.shape[2]], got)
+            assert got.shape[2] == 4 or f.shape[2] == 3 or (f[:, :, 3] == 255).all()
+    ref_lib = optional_reference()
+    if ref_lib:
+        info, frames, metas, rc = ref_lib.webp_frames(outs[k])
+        assert rc == 0 and info["num_frames"] == 3 and info["loop_count"] == 3
+        assert [m["delay"] for m in metas] == [20, 70, 130]
+        info, frames, metas, rc = ref_lib.webp_frames(outs[k - 1])
+        assert rc == 0 and info["num_frames"] == 6 and frames[0].shape[:2] == (256, 256)
 
 
 def test_xbatch_empty_and_small_buffers(cuda_lib, xb, oracle):

@@ -115,6 +115,86 @@ def vp8_cpu_encode(lib, img: np.ndarray, quality: int, filter_level: int = -1, t
     return out[:n].tobytes()
 
 
+def optional_reference():
+    """The reference's own shims (oracle/_ref) when they are built, else None: tests check them in addition to
+    libwebp_decode, never instead of it."""
+    from lilliput_b200 import abi
+    return abi.load_reference() if os.path.exists(abi.REF_LIB) else None
+
+
+def libwebp_decode(data: bytes) -> np.ndarray:
+    """A whole WebP file decoded by libwebp (OpenCV's WebP codec): BGR, or BGRA when the file has alpha -- what
+    WebPDecodeBGR(A)Into gives.  An independent decoder of the device's streams."""
+    import cv2
+    img = cv2.imdecode(np.frombuffer(bytes(data), np.uint8), cv2.IMREAD_UNCHANGED)
+    assert img is not None, "libwebp refused the stream"
+    return img
+
+
+def pillow_animation(data: bytes):
+    """(frame count, loop count, [frame durations in ms], (width, height)) of an animated WebP, as Pillow's WebP
+    reader (libwebp's demuxer) sees them."""
+    import io
+
+    from PIL import Image
+    im = Image.open(io.BytesIO(bytes(data)))
+    assert im.format == "WEBP"
+    durations = []
+    for k in range(im.n_frames):
+        im.seek(k)
+        im.load()  # (the reader sets a frame's duration when it decodes it)
+        durations.append(im.info["duration"])
+    return im.n_frames, im.info.get("loop", 0), durations, im.size
+
+
+def vp8_partition_sizes(payload: bytes):
+    """(first partition size, [token partition sizes]) of a "VP8 " key-frame payload, from its frame tag and the
+    partition size table behind the first partition (RFC 6386 9.1 / 9.5)."""
+    tag = payload[0] | (payload[1] << 8) | (payload[2] << 16)
+    p0 = tag >> 5
+    nparts = 1 << _log2_partitions_field(payload, p0)
+    at = 10 + p0
+    sizes = [int.from_bytes(payload[at + 3 * i:at + 3 * i + 3], "little") for i in range(nparts - 1)]
+    rest = len(payload) - at - 3 * (nparts - 1) - sum(sizes)
+    return p0, sizes + [rest]
+
+
+def _log2_partitions_field(payload: bytes, p0: int) -> int:
+    """The 2-bit partition-count field of the frame header, read with a boolean decoder (RFC 6386 7.3 / 9.2-9.5)."""
+    data = payload[10:10 + p0]
+    value, pos, rng, bits = (data[0] << 8) | data[1], 2, 255, 8
+
+    def read_bit():
+        nonlocal value, pos, rng, bits
+        split = 1 + (((rng - 1) * 128) >> 8)
+        big = split << 8
+        if value >= big:
+            bit, rng, value = 1, rng - split, value - big
+        else:
+            bit, rng = 0, split
+        while rng < 128:
+            value <<= 1
+            rng <<= 1
+            bits -= 1
+            if bits == 0:
+                value |= data[pos] if pos < len(data) else 0
+                pos += 1
+                bits = 8
+        return bit
+
+    def read_literal(n):
+        v = 0
+        for _ in range(n):
+            v = (v << 1) | read_bit()
+        return v
+    # colour space, clamping, segmentation (this encoder writes none), filter type, level, sharpness, no deltas
+    read_literal(2)
+    assert read_bit() == 0, "segmentation header not parsed here"
+    read_literal(1 + 6 + 3)
+    assert read_bit() == 0, "loop-filter deltas not parsed here"
+    return read_literal(2)
+
+
 def riff(chunks) -> bytes:
     body = b"WEBP" + b"".join(t + struct.pack("<I", len(p)) + p + (b"\0" if len(p) & 1 else b"") for t, p in chunks)
     return b"RIFF" + struct.pack("<I", len(body)) + body
