@@ -7,7 +7,8 @@
 // restore-previous of the previous frame's clipped rectangle, snapshot, then non-transparent,
 // in-palette pixels drawn with A=255, frames that hang off the canvas clipped.  Output is the
 // full-canvas BGRA frame lilliput's ops.go expects.  Lossless: bit-exact to the reference
-// (tests/test_gpu_gif.py against reference-made golden frames).
+// (tests/test_gpu_gif.py against reference-made golden frames) and to the oracle on hand-built code streams that steer
+// every corner of the LZW kernel and the compositor (tests/test_gpu_gif_streams.py, both callers).
 //
 // One device path serves both callers: the per-image decoder (one frame per call, canvas and snapshot kept in
 // the decoder between calls) and gif_decode_batch (every frame of many animations at once).  One warp per frame

@@ -3,7 +3,7 @@ encoder kernels of csrc/gif_decode.cu) against per-image lp_transform of the sam
 bytes.  grid_items is asserted so that a silent hand-over to the per-image path cannot pass.  The reference's own
 GIF -> GIF bytes (tests/golden/gif_encode_golden.npz) pin the batch too.
 
-The synthetic animations are written byte by byte (literal-code LZW), so each one has exactly the container features
+The synthetic animations are written byte by byte (literal-code LZW, tests/gif_streams.py), so each one has exactly the container features
 it is meant to cover: local colour tables, palette changes, transparency and disposal, partial frames, interlace,
 frames without a graphic control block, comment / application extensions between frames and behind the last one."""
 import hashlib
@@ -14,6 +14,7 @@ import pytest
 
 from lilliput_b200 import abi
 from lilliput_b200.synth import synth_image
+from tests.gif_streams import app, comment, gcb, write_gif
 from tests.golden.make_golden_gif_encode import CASES, TIMEOUT_NS
 from tests.test_gpu_xbatch import check_against_per_image, rgb_png
 
@@ -27,96 +28,6 @@ def xb(cuda_lib):
     x = abi.XBatch(cuda_lib, 0, arena_bytes=8 << 30)
     yield x
     x.close()
-
-
-# ---------------------------------------------------------------- a minimal GIF writer
-
-def _sub_blocks(data: bytes) -> bytes:
-    out = bytearray()
-    for o in range(0, len(data), 255):
-        chunk = data[o:o + 255]
-        out += bytes([len(chunk)]) + chunk
-    return bytes(out) + b"\x00"
-
-
-def _lzw_literals(idx: np.ndarray, bpp: int) -> bytes:
-    """Every pixel as a literal code; a clear code before the table would widen the codes."""
-    clear, eoi, width = 1 << bpp, (1 << bpp) + 1, bpp + 1
-    codes = []
-    flat = idx.reshape(-1).tolist()
-    run = (1 << bpp) - 2
-    for o in range(0, len(flat), run):
-        codes.append(clear)
-        codes += flat[o:o + run]
-    codes.append(eoi)
-    acc = nbits = 0
-    out = bytearray()
-    for c in codes:
-        acc |= c << nbits
-        nbits += width
-        while nbits >= 8:
-            out.append(acc & 255)
-            acc >>= 8
-            nbits -= 8
-    if nbits:
-        out.append(acc & 255)
-    return bytes(out)
-
-
-def _table_bits(pal) -> int:
-    n = len(pal) // 3
-    b = 1
-    while (1 << b) < n:
-        b += 1
-    return b
-
-
-def _gcb(disposal=0, delay=5, transparent=None) -> bytes:
-    return bytes([0x21, 0xF9, 4, (disposal << 2) | (transparent is not None), delay & 255, delay >> 8,
-                  transparent or 0, 0])
-
-
-def _comment(text: bytes) -> bytes:
-    return b"\x21\xFE" + _sub_blocks(text)
-
-
-def _app(ident: bytes, payload: bytes) -> bytes:
-    return b"\x21\xFF\x0b" + ident[:11] + _sub_blocks(payload)
-
-
-NETSCAPE = b"\x21\xFF\x0bNETSCAPE2.0\x03\x01\x00\x00\x00"
-
-
-def write_gif(w, h, frames, gct=None, bg=0, trailer_ext=b"", loop=True) -> bytes:
-    """frames: dicts with idx (rows x cols palette indices), and optionally left, top, local (RGB bytes), interlace,
-    gcb (bytes or None for none), pre (extension bytes in front of the frame)."""
-    out = bytearray(b"GIF89a" + w.to_bytes(2, "little") + h.to_bytes(2, "little"))
-    if gct is not None:
-        out += bytes([0x80 | 0x70 | (_table_bits(gct) - 1), bg, 0]) + gct
-    else:
-        out += bytes([0x70, bg, 0])
-    if loop:
-        out += NETSCAPE
-    for f in frames:
-        idx = np.asarray(f["idx"], np.uint8)
-        fh, fw = idx.shape
-        out += f.get("pre", b"")
-        if f.get("gcb", b"") is not None:
-            out += f.get("gcb") or _gcb()
-        local = f.get("local")
-        flags = (0x80 | (_table_bits(local) - 1) if local is not None else 0) | (0x40 if f.get("interlace") else 0)
-        out += b"\x2C" + f.get("left", 0).to_bytes(2, "little") + f.get("top", 0).to_bytes(2, "little")
-        out += fw.to_bytes(2, "little") + fh.to_bytes(2, "little") + bytes([flags])
-        if local is not None:
-            out += local
-        pal = local if local is not None else gct
-        bpp = max(2, _table_bits(pal))
-        rows = idx
-        if f.get("interlace"):
-            rows = np.concatenate([idx[0::8], idx[4::8], idx[2::4], idx[1::2]])
-        out += bytes([bpp]) + _sub_blocks(_lzw_literals(rows, bpp))
-    out += trailer_ext + b";"
-    return bytes(out)
 
 
 def _pal(seed, n):
@@ -149,30 +60,30 @@ def synthetic_gifs():
     cases["late_buckets"] = write_gif(W, H, [dict(idx=f0), dict(idx=_idx(40, H, W, 64)), dict(idx=(_idx(41, H, W, 64) // 2) * 2)],
                                       gct=g64)
     cases["transparency_disposal"] = write_gif(W, H, [
-        dict(idx=_idx(50, H, W, 16), gcb=_gcb(1, 4, 3)),
-        dict(idx=_idx(51, 30, 40, 16), left=10, top=8, gcb=_gcb(2, 4, 3)),
-        dict(idx=_idx(52, 20, 20, 16), left=40, top=20, gcb=_gcb(3, 4, 5)),
-        dict(idx=_idx(53, H, W, 16), gcb=_gcb(1, 4, 0)),
-        dict(idx=_idx(54, 24, 30, 16), left=5, top=25, gcb=_gcb(0, 4, 7))], gct=g16, bg=3)
+        dict(idx=_idx(50, H, W, 16), gcb=gcb(1, 4, 3)),
+        dict(idx=_idx(51, 30, 40, 16), left=10, top=8, gcb=gcb(2, 4, 3)),
+        dict(idx=_idx(52, 20, 20, 16), left=40, top=20, gcb=gcb(3, 4, 5)),
+        dict(idx=_idx(53, H, W, 16), gcb=gcb(1, 4, 0)),
+        dict(idx=_idx(54, 24, 30, 16), left=5, top=25, gcb=gcb(0, 4, 7))], gct=g16, bg=3)
     # opaque background (first frame without transparency), later frames whose transparent index IS the background
     cases["background_drop"] = write_gif(W, H, [
-        dict(idx=_idx(55, H, W, 16), gcb=_gcb(1, 4)),
-        dict(idx=_idx(56, H, W, 16), gcb=_gcb(1, 4, 6)),
-        dict(idx=_idx(57, 20, 30, 16), left=4, top=4, gcb=_gcb(0, 4, 6))], gct=g16, bg=6)
+        dict(idx=_idx(55, H, W, 16), gcb=gcb(1, 4)),
+        dict(idx=_idx(56, H, W, 16), gcb=gcb(1, 4, 6)),
+        dict(idx=_idx(57, 20, 30, 16), left=4, top=4, gcb=gcb(0, 4, 6))], gct=g16, bg=6)
     cases["partial_offsets"] = write_gif(W, H, [
         dict(idx=_idx(60, H, W, 64)),
         dict(idx=_idx(61, 20, 33, 64), left=7, top=9),                    # no transparent index: one is forced
-        dict(idx=_idx(62, 17, 25, 64), left=40, top=30, gcb=_gcb(1, 3, 12)),
-        dict(idx=_idx(63, 40, 10, 64), left=60, top=10, gcb=_gcb(2, 3))], gct=g64)
+        dict(idx=_idx(62, 17, 25, 64), left=40, top=30, gcb=gcb(1, 3, 12)),
+        dict(idx=_idx(63, 40, 10, 64), left=60, top=10, gcb=gcb(2, 3))], gct=g64)
     cases["interlaced"] = write_gif(W, H, [dict(idx=_idx(70 + k, H, W, 64), interlace=True) for k in range(3)]
                                     + [dict(idx=_idx(73, 19, 23, 64), left=3, top=4, interlace=True)], gct=g64)
     cases["no_gcb"] = write_gif(W, H, [dict(idx=_idx(80 + k, H, W, 16), gcb=None) for k in range(3)], gct=g16)
     cases["extensions"] = write_gif(W, H, [
-        dict(idx=_idx(90, H, W, 16), pre=_comment(b"first frame")),
-        dict(idx=_idx(91, H, W, 16), pre=_app(b"XMP DataXMP", b"<x/>" * 80) + _comment(b"between" * 50)),
-        dict(idx=_idx(92, H, W, 16), pre=_gcb(2, 9, 4) + _comment(b"c"), gcb=_gcb(1, 7))],
-        gct=g16, trailer_ext=_comment(b"after the last frame") + _app(b"TRAILER1.00", b"\x01\x02\x03"))
-    cases["one_frame"] = write_gif(W, H, [dict(idx=_idx(95, H, W, 64), gcb=_gcb(0, 0, 9))], gct=g64, loop=False)
+        dict(idx=_idx(90, H, W, 16), pre=comment(b"first frame")),
+        dict(idx=_idx(91, H, W, 16), pre=app(b"XMP DataXMP", b"<x/>" * 80) + comment(b"between" * 50)),
+        dict(idx=_idx(92, H, W, 16), pre=gcb(2, 9, 4) + comment(b"c"), gcb=gcb(1, 7))],
+        gct=g16, trailer_ext=comment(b"after the last frame") + app(b"TRAILER1.00", b"\x01\x02\x03"))
+    cases["one_frame"] = write_gif(W, H, [dict(idx=_idx(95, H, W, 64), gcb=gcb(0, 0, 9))], gct=g64, loop=False)
     cases["no_global_table"] = write_gif(W, H, [dict(idx=_idx(96 + k, H, W, 8), local=_pal(97, 8)) for k in range(3)])
     return cases
 
