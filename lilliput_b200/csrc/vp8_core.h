@@ -42,6 +42,7 @@ struct BoolDec {
     uint64_t value;
     uint32_t range;  // range - 1, kept in [127, 254]
     int bits;        // number of bits in `value` below the 8-bit compare window
+    int eof;         // a refill found no byte left: the partition is truncated (libwebp's eof_)
 };
 
 LP_VP8_INL int clz32(uint32_t v) {
@@ -58,6 +59,7 @@ LP_VP8_INL void bd_init(BoolDec& b, const uint8_t* p, size_t n) {
     b.value = 0;
     b.range = 254;
     b.bits = -8;
+    b.eof = n == 0;  // libwebp loads on init: an empty partition is already past its end
 }
 
 LP_VP8_INL void bd_fill(BoolDec& b) {
@@ -81,7 +83,9 @@ LP_VP8_INL void bd_fill(BoolDec& b) {
         b.bits += 48;
     } else {
 #endif
-        const uint32_t byte = b.p < b.end ? *b.p++ : 0u;  // zeros past the end, as libwebp feeds
+        uint32_t byte = 0;  // zeros past the end, as libwebp feeds
+        if (b.p < b.end) byte = *b.p++;
+        else b.eof = 1;
         b.value = (b.value << 8) | byte;
         b.bits += 8;
     }
@@ -207,6 +211,7 @@ LP_VP8_FN int parse_frame_header(const uint8_t* data, size_t size, FrameHdr& h, 
         }
         h.part_off[h.num_parts - 1] = (uint32_t)off;
         h.part_len[h.num_parts - 1] = (uint32_t)left;
+        if (!left) return VP8_BAD;  // the last partition must start inside the data (libwebp's ParsePartitions)
     }
     // quantizer indices (s.9.6, s.14.1)
     {
@@ -760,6 +765,15 @@ LP_VP8_FN void reconstruct_mb(const FrameHdr& h, Work& w, int mb_x, int mb_y, co
         }
 }
 
+// After the macroblock loop: whether the first partition or a token partition that some row used
+// ran past its end.  libwebp refuses such a frame ("Premature end-of-file"); the flags are sticky,
+// so one look at the end stands for its check after every row and macroblock.
+LP_VP8_INL bool frame_truncated(const FrameHdr& h, const BoolDec& br, const BoolDec* parts) {
+    bool eof = br.eof;
+    for (int p = 0; p < h.num_parts && p < h.mb_h; p++) eof |= parts[p].eof != 0;
+    return eof;
+}
+
 // Decodes every macroblock of the frame in raster order into the (unfiltered) planes and
 // records the loop-filter parameters.  Serial by construction of the format: mode and token
 // contexts chain left-to-right / top-to-bottom, and so does intra prediction.  (The device
@@ -786,7 +800,7 @@ LP_VP8_FN int decode_macroblocks(const uint8_t* data, const FrameHdr& h, BoolDec
             reconstruct_mb(h, w, mb_x, mb_y, mb, coeffs, yb, ub, vb);
         }
     }
-    return VP8_OK;
+    return frame_truncated(h, br, parts) ? VP8_BAD : VP8_OK;
 }
 
 // ---- loop filter (RFC 6386 s.15) -----------------------------------------------------------

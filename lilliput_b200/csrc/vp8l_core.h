@@ -39,12 +39,13 @@ LP_VP8_INL void* arena_alloc(Arena& a, size_t n) {
 }
 
 // ---- bit reader (spec s.2: least-significant bit first) ------------------------------------
+// Past the end the reader feeds zeros; `pos` counts every byte loaded, those zeros included.
 struct Bits {
     const uint8_t* p;
     size_t n, pos;
     uint64_t val;
     int nbits;
-    int eos;
+    int eos;  // a prefix code matched no symbol
 };
 LP_VP8_INL void bits_init(Bits& b, const uint8_t* p, size_t n) {
     b.p = p;
@@ -70,7 +71,6 @@ LP_VP8_INL void bits_fill(Bits& b) {
         } else {
             for (int k = 0; k < 4; k++)
                 if (b.pos + k < b.n) w |= (uint64_t)b.p[b.pos + k] << (8 * k);
-            if (b.pos >= b.n + 8) b.eos = 1;  // ran well past the end: the stream is truncated
         }
         b.pos += 4;
         b.val |= w << b.nbits;
@@ -83,6 +83,11 @@ LP_VP8_INL uint32_t bits_read(Bits& b, int n) {  // n <= 32
     b.val >>= n;
     b.nbits -= n;
     return n ? v : 0;
+}
+// Whether the stream is unusable: a code matched nothing, or more bits have been used than the payload
+// holds (libwebp's VP8LIsEndOfStream; the stream is truncated).  Sticky: the bits used only grow.
+LP_VP8_INL bool bits_bad(const Bits& b) {
+    return b.eos || (b.pos > b.n && (b.pos - b.n) * 8 > (size_t)b.nbits);
 }
 
 // ---- prefix codes (spec s.6.2) -------------------------------------------------------------
@@ -179,13 +184,12 @@ LP_VP8_FN int code_read_definition(Bits& b, int alphabet, uint8_t* lens, Code& o
     if (bits_read(b, 1)) {  // simple code: 1 or 2 symbols
         const int nsym = (int)bits_read(b, 1) + 1;
         const int first8 = (int)bits_read(b, 1);
+        // a symbol past the alphabet is dropped, as libwebp drops it: the code keeps the other one, or has none
         const int s0 = (int)bits_read(b, first8 ? 8 : 1);
-        if (s0 >= alphabet) return L_BAD;
-        lens[s0] = 1;
+        if (s0 < alphabet) lens[s0] = 1;
         if (nsym == 2) {
             const int s1 = (int)bits_read(b, 8);
-            if (s1 >= alphabet) return L_BAD;
-            lens[s1] = 1;
+            if (s1 < alphabet) lens[s1] = 1;
         }
     } else {
         const uint8_t order[19] = {17, 18, 0, 1, 2, 3, 4, 5, 16, 6, 7, 8, 9, 10, 11, 12, 13, 14, 15};
@@ -258,7 +262,7 @@ LP_VP8_FN int code_read_definition(Bits& b, int alphabet, uint8_t* lens, Code& o
             }
         }
     }
-    if (b.eos) return L_BAD;
+    if (bits_bad(b)) return L_BAD;
     return code_build(out, lens, alphabet, a);
 }
 
@@ -375,7 +379,7 @@ LP_VP8_FN int decode_entropy_image(Bits& b, int xsize, int ysize, Arena& a, cons
             const int dist_symbol = code_read(g.c[4], b);
             const int dist_code = prefix_value(b, dist_symbol);
             const int dist = plane_code_to_distance(dm, xsize, dist_code);
-            if (b.eos || (size_t)dist > src || (size_t)length > npix - src) return L_BAD;
+            if (bits_bad(b) || (size_t)dist > src || (size_t)length > npix - src) return L_BAD;
             for (int i = 0; i < length; i++) {
                 const uint32_t px = data[src - dist];
                 data[src++] = px;
@@ -397,7 +401,7 @@ LP_VP8_FN int decode_entropy_image(Bits& b, int xsize, int ysize, Arena& a, cons
                 row++;
             }
         }
-        if (b.eos) return L_BAD;
+        if (bits_bad(b)) return L_BAD;
     }
     *out = data;
     return L_OK;
@@ -573,7 +577,7 @@ LP_VP8_FN int decode_stream(Bits& b, int width, int height, Arena& a, uint32_t**
             xsize = sub_size(xsize, t.bits);
         }
         ntr++;
-        if (b.eos) return L_BAD;
+        if (bits_bad(b)) return L_BAD;
     }
     uint32_t* px = nullptr;
     int rc = decode_entropy_image<true>(b, xsize, height, a, *dm, &px);
@@ -611,7 +615,7 @@ LP_VP8_FN int decode_vp8l(const uint8_t* p, size_t n, int width, int height, Are
 LP_VP8_FN int decode_alph(const uint8_t* p, size_t n, int width, int height, Arena& a, uint8_t* alpha) {
     if (n < 1) return L_BAD;
     const int method = p[0] & 3, filter = (p[0] >> 2) & 3, pre = (p[0] >> 4) & 3, rsrv = (p[0] >> 6) & 3;
-    if (method > 1 || pre > 1 || rsrv > 1) return L_BAD;
+    if (method > 1 || pre > 1 || rsrv != 0) return L_BAD;
     const size_t npix = (size_t)width * height;
     if (method == 0) {
         if (n - 1 < npix) return L_BAD;

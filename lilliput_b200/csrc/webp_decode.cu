@@ -289,6 +289,7 @@ __global__ void __launch_bounds__(kVp8WarpsPerBlock * 32) vp8_decode_kernel(cons
         }
         if (lane == 0) parts[mb_y & (h.num_parts - 1)] = tbr;
     }
+    if (lane == 0 && vp8::frame_truncated(h, br, parts)) *it.status = vp8::VP8_BAD;
     __syncwarp();
     if (h.filter_type == 0) return;
     for (int mb_y = 0; mb_y < mb_h; mb_y++)
@@ -412,6 +413,15 @@ static bool image_info(const uint8_t* p, size_t n, bool lossless, WebpFrame* f) 
     return ((bits >> 29) & 7) == 0;  // version
 }
 
+// The bytes an image payload of `n` bytes is decoded from, `avail` bytes being left in its container: the
+// chunk and its padding byte when there is one.  libwebp's decoders read on to the end of their input, so a
+// stream cut short can still draw its last bits from the padding byte, and frames are accepted or refused
+// as libwebp accepts or refuses them only if ours do too.  (The header checks use the chunk size.)
+static size_t image_span(size_t n, size_t avail) {
+    const size_t padded = n + (n & 1);
+    return padded < avail ? padded : avail;
+}
+
 // Walks the sub-chunks that make up one image (ALPH? then VP8 / VP8L) in [pos, end).
 static bool parse_image_chunks(const uint8_t* b, size_t pos, size_t end, WebpFrame* f, bool* got_image) {
     *got_image = false;
@@ -430,8 +440,8 @@ static bool parse_image_chunks(const uint8_t* b, size_t pos, size_t end, WebpFra
             if (*got_image) return false;
             f->lossless = tag[3] == 'L';
             f->img_off = pos + 8;
-            f->img_len = n;
-            if (!image_info(b + f->img_off, f->img_len, f->lossless, f)) return false;
+            if (!image_info(b + f->img_off, n, f->lossless, f)) return false;
+            f->img_len = image_span(n, end - f->img_off);
             if (f->has_alph && !f->lossless) f->has_alpha = true;
             *got_image = true;
         }
@@ -503,8 +513,8 @@ static bool webp_parse(const uint8_t* b, size_t size, WebpContainer* c) {
             if (still_done) return false;
             still.lossless = tag[3] == 'L';
             still.img_off = pos + 8;
-            still.img_len = n;
             if (!image_info(d, n, still.lossless, &still)) return false;
+            still.img_len = image_span(n, size - still.img_off);
             if (still.has_alph && !still.lossless) still.has_alpha = true;
             still_open = false;
             still_done = true;
