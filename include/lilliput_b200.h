@@ -160,7 +160,14 @@ void lp_batch_destroy(lp_batch* b);
 
 /* Host -> host: the reference-facing call.  `in[i]` / `out[i]` are HOST buffers
  * (pinned or not); H2D of the compressed bytes and D2H of the encoded bytes are
- * inside the call.  status[i] is an lp_status per image. */
+ * inside the call.  status[i] is an lp_status per image.
+ *
+ * Sources taken: 8-bit Huffman-coded 3-component JPEGs of the configured size whose
+ * EXIF orientation is top-left -- baseline or extended sequential (with or without
+ * restart markers and optimised tables), progressive, or sequential with one scan per
+ * component.  Each item gets the status and bytes lp_transform gives it, except that
+ * gray and EXIF-rotated files, and multi-scan files that overflow the context's scan
+ * or Huffman-table pools (sized by max_images, see batch.cu), get LP_ERR_UNSUPPORTED. */
 int lp_batch_transform(lp_batch* b, const uint8_t* const* in, const size_t* in_len, int n,
                        uint8_t* const* out, size_t* out_len, int* status);
 

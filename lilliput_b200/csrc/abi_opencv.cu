@@ -181,24 +181,13 @@ static int decode_jpeg_into(const Decoder* d, Mat* m) {
     std::vector<JpegHuffSet> sets;
     int nscans = 0, nsets = 0;
     if (h.multiscan) {
-        scans.resize(256);
-        sets.resize(64);
+        scans.resize(kMultiscanMaxScans);
+        sets.resize(kMultiscanMaxSets);
         int rc = jpeg_parse_scans(d->data, d->len, h, scans.data(), (int)scans.size(), &nscans, sets.data(),
                                   (int)sets.size(), &nsets);
         if (rc) return rc;
-        // every scan of a multi-scan file is walked by ONE device thread (jpeg_multiscan_kernel): bound the work a
-        // hostile file (up to 256 scans over a large frame) can queue on the caller's stream.  Real progressive
-        // files have ~10 scans; an 8192 x 8192 4:4:4 frame with 20 scans still passes.
-        size_t visits = 0;
-        for (int k = 0; k < nscans; k++) {
-            size_t per = 0;
-            for (int c = 0; c < scans[k].ns; c++) {
-                const int ci = scans[k].ci[c];
-                per += (size_t)h.mcus_x * h.mcus_y * h.comp[ci].h * h.comp[ci].v;
-            }
-            visits += per;
-        }
-        if (visits > ((size_t)1 << 26)) {
+        const size_t visits = jpeg_multiscan_visits(h, scans.data(), nscans);
+        if (visits > kMultiscanMaxVisits) {
             fprintf(stderr, "[lilliput_b200] multi-scan JPEG: %zu block visits over %d scans exceed the serial decoder's budget\n",
                     visits, nscans);
             return LP_ERR_UNSUPPORTED;
@@ -229,6 +218,11 @@ static int decode_jpeg_into(const Decoder* d, Mat* m) {
     }
     uint32_t tiles = 0;
     const uint32_t blocks = jpeg_item_set_window(&it, 0, 0, h.width, h.height, false, &tiles);  // whole image
+    if (h.multiscan) {  // its scans are [0, nscans) of d_scans; the whole frame is the window, so no masks
+        it.restart_interval = 0;
+        it.table_set = 0;
+        it.nscans = (uint32_t)nscans;
+    }
     it.frame_channels = h.ncomp == 1 ? 1 : 3;
     JpegHuffSet hs;
     jpeg_build_huff_set(h, &hs);
@@ -280,8 +274,8 @@ static int decode_jpeg_into(const Decoder* d, Mat* m) {
     b.nslots = reinterpret_cast<uint32_t*>(d_nslots);
     b.dcdiff = reinterpret_cast<int16_t*>(d_dcdiff);
     if (h.multiscan) {
+        b.n_multiscan = 1;
         b.scans = d_scans;
-        b.nscans = nscans;
     }
     int rc = jpeg_decode_launch(b, st, nullptr);
     JpegDecodeItem back;

@@ -1,5 +1,14 @@
-// batch.cu -- the additive batch entry points (include/lilliput_b200.h): N independent baseline
-// JPEGs -> Fit / area resize -> JPEG, every stage one grid launch over a chunk of the batch.
+// batch.cu -- the additive batch entry points (include/lilliput_b200.h): N independent JPEGs (baseline, restart
+// interval, optimised tables, progressive or one scan per component) -> Fit / area resize -> JPEG, every stage one
+// grid launch over a chunk of the batch.
+//
+// Multi-scan files decode side by side in one extra launch per chunk (jpeg_multiscan_kernel, one thread walking the
+// scans of each file) into the same scan-order coefficient layout as the parallel decoders, so the rest of the chunk
+// is unchanged.  Their scan descriptors and Huffman table sets live in batch-wide pools sized by max_images:
+//   scans      kScansPerImage per image + kMultiscanMaxScans (one file's cap)
+//   table sets one per image (single-scan files) + kSetsPerImage per image + kMultiscanMaxSets (one file's cap)
+// libjpeg-turbo's progressive files have 10 scans and up to 9 distinct optimised table sets, so a batch made only
+// of them fits.  A file that overflows a pool gets LP_ERR_UNSUPPORTED (as the restart-marker scratch does).
 //
 // Per-item semantics are those of ImageOps.Transform (ref ops.go:352-444) for a still JPEG with
 // ImageOpsFit/ImageOpsResize and ".jpeg" output: decode (ref opencv.cpp:166), orientation TL,
@@ -20,9 +29,21 @@
 
 using namespace lp;
 
+static constexpr int kScansPerImage = 16, kSetsPerImage = 10;
+
+namespace lp {
+// Device bytes of the multi-scan pools of a context for max_images = n (what batch_create_in adds for them besides
+// the per-slot masks).
+size_t batch_multiscan_pool_bytes(size_t n) {
+    return ((kSetsPerImage * n + kMultiscanMaxSets) * sizeof(JpegHuffSet) +
+            (kScansPerImage * n + kMultiscanMaxScans) * sizeof(JpegScanDesc));
+}
+}  // namespace lp
+
 struct lp_batch {
     lp_batch_config cfg;
     bool progressive = false;        // JPEG output is progressive (lp_xbatch with JpegProgressive)
+    bool multiscan = true;           // takes multi-scan sources (lp_xbatch groups of single-scan files do not)
     cudaStream_t st = nullptr;       // kernels
     cudaStream_t st_h2d = nullptr;   // input copies (pipelined transform)
     cudaStream_t st_d2h = nullptr;   // output copies (pipelined transform)
@@ -54,6 +75,8 @@ struct lp_batch {
     void* d_states = nullptr;       // parallel Huffman: subsequence exit states
     uint32_t* d_nslots = nullptr;
     int16_t* d_dcdiff = nullptr;    // per chunk slot: DC differences of all blocks
+    uint64_t* d_masks = nullptr;    // per chunk slot: nonzero masks of all blocks (multi-scan items, jpeg_scan_core.h)
+    JpegScanDesc* d_scans = nullptr;  // scan descriptors of the batch's multi-scan files
     uint32_t total_blocks = 0;      // blocks of a whole image (dcdiff slot stride)
     int win_w = 0, win_h = 0;       // decoded pixel window (crop, x range aligned out to 16)
     int win_x0 = 0;
@@ -64,6 +87,8 @@ struct lp_batch {
     std::vector<JpegHuffSet> tables;
     std::unordered_map<std::string, int> table_index;  // every distinct Huffman table set of the batch (hashed)
     size_t tables_uploaded = 0;
+    std::vector<JpegScanDesc> scans;  // multi-scan files: their scans, table_set indexing `tables`
+    size_t scans_uploaded = 0;
     std::vector<int> parse_status;
     std::vector<size_t> file_dev_off;
     size_t dev_off = 0, clean_off = 0, state_off = 0;
@@ -74,6 +99,7 @@ struct lp_batch {
     struct ChunkLayout {
         uint32_t blocks = 0, tiles = 0, total_blocks = 0;
         int ordinal = 0;
+        int n_multiscan = 0;
         std::vector<uint2> rst_work;  // (image in chunk, restart interval) of the chunk's DRI images
         uint2* d_rst_work = nullptr;  // stream-ordered allocation, freed after the chunk's launches
     };
@@ -85,7 +111,8 @@ struct lp_batch {
     std::vector<cudaEvent_t> ev;      // 6 per chunk (stage timing)
     std::vector<cudaEvent_t> ev_h2d;  // per chunk
     std::vector<cudaEvent_t> ev_d2h;  // per chunk
-    int max_tables = 0;  // = max_images: a batch of per-image optimised tables has one set per file
+    int max_tables = 0;  // table-set pool (see the top of the file)
+    size_t max_scans = 0;  // scan-descriptor pool
     bool owns_mem = true;  // false: device / pinned buffers were carved from a caller's arenas (xbatch.cu)
 };
 
@@ -98,6 +125,7 @@ static void batch_free(lp_batch* b) {
     cudaFree(b->d_frames); cudaFree(b->d_resized); cudaFree(b->d_enc_scratch);
     cudaFree(b->d_out); cudaFree(b->d_out_len);
     cudaFree(b->d_clean); cudaFree(b->d_states); cudaFree(b->d_nslots); cudaFree(b->d_dcdiff);
+    cudaFree(b->d_masks); cudaFree(b->d_scans);
     if (b->h_out) cudaFreeHost(b->h_out);
     if (b->h_out_len) cudaFreeHost(b->h_out_len);
     if (b->h_items_back) cudaFreeHost(b->h_items_back);
@@ -114,14 +142,16 @@ static void batch_free(lp_batch* b) {
 
 namespace lp {
 lp_batch* batch_create_in(const lp_batch_config* cfg, uint8_t* dev_arena, size_t dev_bytes, uint8_t* host_arena,
-                          size_t host_bytes, bool progressive_jpeg = false);
+                          size_t host_bytes, bool progressive_jpeg = false, bool multiscan_sources = true);
 }
 extern "C" lp_batch* lp_batch_create(const lp_batch_config* cfg) { return lp::batch_create_in(cfg, nullptr, 0, nullptr, 0); }
 
 // dev_arena / host_arena non-null: every device / pinned buffer is carved from them (nothing is allocated or
 // freed by the context); returns nullptr when they are too small.  progressive_jpeg: write progressive JPEG files.
+// multiscan_sources: take multi-scan files (and allocate their pools and masks); otherwise they get
+// LP_ERR_UNSUPPORTED.
 lp_batch* lp::batch_create_in(const lp_batch_config* cfg, uint8_t* dev_arena, size_t dev_bytes, uint8_t* host_arena,
-                              size_t host_bytes, bool progressive_jpeg) {
+                              size_t host_bytes, bool progressive_jpeg, bool multiscan_sources) {
     if (!cfg || cfg->max_images < 1 || cfg->src_width < 1 || cfg->src_height < 1) return nullptr;
     if (ensure_device()) return nullptr;
     DeviceGuard dev_guard(cfg->device);
@@ -129,6 +159,7 @@ lp_batch* lp::batch_create_in(const lp_batch_config* cfg, uint8_t* dev_arena, si
     lp_batch* b = new lp_batch;
     b->cfg = *cfg;
     b->progressive = progressive_jpeg;
+    b->multiscan = multiscan_sources;
     b->owns_mem = dev_arena == nullptr;
     size_t dev_used = 0, host_used = 0;
     b->W = cfg->src_width;
@@ -189,7 +220,13 @@ lp_batch* lp::batch_create_in(const lp_batch_config* cfg, uint8_t* dev_arena, si
     if (cudaStreamCreateWithFlags(&b->st_d2h, cudaStreamNonBlocking) != cudaSuccess) return fail();
     BALLOC(b->d_scan, cfg->max_in_bytes + 16 * N + 4096);
     BALLOC(b->d_items, N * sizeof(JpegDecodeItem));
-    b->max_tables = (int)N;
+    b->max_tables = (int)N;  // single-scan files: one set each at most
+    if (b->multiscan) {
+        b->max_tables += (int)(kSetsPerImage * N) + kMultiscanMaxSets;
+        b->max_scans = kScansPerImage * N + kMultiscanMaxScans;
+        BALLOC(b->d_scans, b->max_scans * sizeof(JpegScanDesc));
+        BALLOC(b->d_masks, (size_t)b->chunk * max_blocks * sizeof(uint64_t));
+    }
     BALLOC(b->d_tables, (size_t)b->max_tables * sizeof(JpegHuffSet));
     BALLOC(b->d_coef, (size_t)b->chunk * max_blocks * 64 * sizeof(int16_t));
     BALLOC(b->d_frames, (size_t)b->chunk * b->frame_bytes + 256);
@@ -273,6 +310,8 @@ static void batch_begin(lp_batch* b, int n) {
     b->table_index.clear();
     b->last_table_idx = -1;
     b->tables_uploaded = 0;
+    b->scans.clear();
+    b->scans_uploaded = 0;
     b->dev_off = b->clean_off = b->state_off = 0;
     b->parallel_huffman = true;
     for (auto& kv : b->chunk_layout)
@@ -304,22 +343,39 @@ static int batch_layout_chunk(lp_batch* b, const uint8_t* const* in, const size_
 static int batch_parse_chunk(lp_batch* b, const uint8_t* const* in, const size_t* in_len, int i0, int cnt, int ordinal) {
     std::vector<JpegHeader> hdr((size_t)cnt);
     std::vector<uint32_t> blocks_of((size_t)cnt, 0), tiles_of((size_t)cnt, 0), total_of((size_t)cnt, 0);
+    // multi-scan files: their scans (table_set numbering the file's own sets) and the Huffman tables of each set
+    std::vector<std::vector<JpegScanDesc>> ms_scans((size_t)cnt);
+    std::vector<std::vector<JpegHeader>> ms_sets((size_t)cnt);
     auto pass1 = [&](int k0, int k1) {
         for (int k = k0; k < k1; k++) {
             JpegHeader& h = hdr[k - i0];
             int rc = jpeg_parse_header(in[k], in_len[k], &h);
-            if (!rc && !h.supported) rc = LP_ERR_UNSUPPORTED;
+            const bool ms = !rc && !h.supported && h.multiscan && b->multiscan;
+            if (!rc && !h.supported && !ms) rc = LP_ERR_UNSUPPORTED;
             if (!rc && (h.width != b->W || h.height != b->H)) rc = LP_ERR_BAD_ARGUMENT;
             // batch path: TL only (DESIGN.md).  EXIF values outside 2..8 (0, 9, 300 ... the reader passes them through,
             // like the reference's) are no-ops for OrientationTransform, so they are TL as well
             if (!rc && h.orientation >= 2 && h.orientation <= 8) rc = LP_ERR_UNSUPPORTED;
             if (!rc && h.ncomp != 3) rc = LP_ERR_UNSUPPORTED;
+            if (!rc && ms) {
+                // what the per-image decoder refuses when it reads the scans (damage, over the work budget), lp_transform
+                // reports as a failed decode
+                std::vector<JpegScanDesc>& sc = ms_scans[k - i0];
+                std::vector<JpegHeader>& sets = ms_sets[k - i0];
+                sc.resize(kMultiscanMaxScans);
+                sets.resize(kMultiscanMaxSets);
+                int nscans = 0, nsets = 0;
+                rc = jpeg_parse_scans(in[k], in_len[k], h, sc.data(), (int)sc.size(), &nscans, sets.data(), (int)sets.size(), &nsets);
+                if (rc || jpeg_multiscan_visits(h, sc.data(), nscans) > kMultiscanMaxVisits) rc = LP_ERR_DECODING_FAILED;
+                sc.resize(rc ? 0 : (size_t)nscans);
+                sets.resize(rc ? 0 : (size_t)nsets);
+            }
             JpegDecodeItem& it = b->items[k];
             memset(&it, 0, sizeof(it));
             if (!rc) {
-                it.scan_len = (uint32_t)h.scan_length;
+                it.scan_len = (uint32_t)(ms ? in_len[k] : h.scan_length);  // multi-scan: the whole file
                 it.width = h.width; it.height = h.height; it.ncomp = h.ncomp;
-                it.mcus_x = h.mcus_x; it.mcus_y = h.mcus_y; it.restart_interval = h.restart_interval;
+                it.mcus_x = h.mcus_x; it.mcus_y = h.mcus_y; it.restart_interval = ms ? 0 : h.restart_interval;
                 uint32_t total_blocks = 0;
                 for (int c = 0; c < h.ncomp; c++) {
                     it.h[c] = h.comp[c].h; it.v[c] = h.comp[c].v;
@@ -377,6 +433,33 @@ static int batch_parse_chunk(lp_batch* b, const uint8_t* const* in, const size_t
     for (int k = i0; k < i0 + cnt; k++) {
         if (b->parse_status[k]) continue;
         JpegDecodeItem& it = b->items[k];
+        const int slot = k - i0;  // position inside its chunk: the per-chunk scratch is indexed from the chunk's first image
+        if (!ms_scans[slot].empty()) {
+            // multi-scan: its scans go to the pool with their sets' indices in the batch's table-set store; its nonzero
+            // masks take the slot layout of the DC differences
+            const std::vector<JpegScanDesc>& sc = ms_scans[slot];
+            const std::vector<JpegHeader>& sets = ms_sets[slot];
+            std::vector<int> global(sets.size(), -1);
+            bool fits = b->scans.size() + sc.size() <= b->max_scans;
+            for (size_t q = 0; q < sets.size() && fits; q++) fits = (global[q] = table_set_for(b, sets[q])) >= 0;
+            if (!fits) {
+                b->parse_status[k] = LP_ERR_UNSUPPORTED;
+                it.status = -1;
+                continue;
+            }
+            it.table_set = (uint32_t)b->scans.size();
+            it.nscans = (uint32_t)sc.size();
+            for (JpegScanDesc d : sc) {
+                d.table_set = global[d.table_set];
+                b->scans.push_back(d);
+            }
+            it.scan_off = b->file_dev_off[k];
+            it.coef_off = (uint64_t)slot * lay.blocks * 64;
+            it.frame_off = (uint64_t)slot * b->frame_bytes;
+            it.dcdiff_off = (uint64_t)slot * lay.total_blocks;
+            b->chunk_layout[i0].n_multiscan++;
+            continue;
+        }
         const int ts = table_set_for(b, hdr[k - i0]);
         if (ts < 0) {
             b->parse_status[k] = LP_ERR_UNSUPPORTED;
@@ -384,7 +467,6 @@ static int batch_parse_chunk(lp_batch* b, const uint8_t* const* in, const size_t
             continue;
         }
         it.table_set = (uint32_t)ts;
-        const int slot = k - i0;  // position inside its chunk: the per-chunk scratch is indexed from the chunk's first image
         size_t state_need = 2 * huff_nsub(it.scan_len);
         if (it.restart_interval) {
             // RSTn streams: one thread per restart interval (jpeg_rst_*): the marker offsets live where the
@@ -436,6 +518,12 @@ static int batch_upload_items(lp_batch* b, int i0, int cnt, cudaStream_t st) {
                                    cudaMemcpyHostToDevice, st));
         b->tables_uploaded = b->tables.size();
     }
+    if (b->scans.size() > b->scans_uploaded) {
+        LP_CUDA_OK(cudaMemcpyAsync(b->d_scans + b->scans_uploaded, b->scans.data() + b->scans_uploaded,
+                                   (b->scans.size() - b->scans_uploaded) * sizeof(JpegScanDesc), cudaMemcpyHostToDevice,
+                                   st));
+        b->scans_uploaded = b->scans.size();
+    }
     return LP_OK;
 }
 
@@ -472,6 +560,9 @@ static int batch_launch_chunk(lp_batch* b, int i0, int cnt, cudaStream_t st, cud
     d.clean = b->d_clean;
     d.states = b->d_states;
     d.nslots = b->d_nslots;
+    d.n_multiscan = lay.n_multiscan;
+    d.scans = b->d_scans;
+    d.masks = b->d_masks;
     int rc = jpeg_decode_launch(d, st, ev ? ev[1] : nullptr);
     if (rc) return rc;
     if (ev) LP_CUDA_OK(cudaEventRecord(ev[2], st));
@@ -691,7 +782,7 @@ extern "C" void lp_batch_sync_rounds(const lp_batch* b, double* mean, int* max) 
     double sum = 0;
     int mx = 0, cnt = 0;
     for (int i = 0; i < b->n; i++) {
-        if (b->parse_status[i] || b->items[i].restart_interval) continue;
+        if (b->parse_status[i] || b->items[i].restart_interval || b->items[i].nscans) continue;
         const int r = (int)b->h_items_back[i].pad_;
         sum += r;
         mx = std::max(mx, r);

@@ -10,12 +10,15 @@
 //   jpeg_huff_decode_kernel   entropy-coded segment -> quantised coefficients (int16, natural
 //                             order, zero-initialised buffer).  Bit-serial by nature; this
 //                             first version runs one stream per thread.
+//   jpeg_multiscan_kernel     progressive / one-scan-per-component files: one warp per item clears its blocks, one
+//                             thread walks its scans (jpeg_scan_core.h); scan-order blocks like the parallel path.
 //   jpeg_idct_color_kernel    one CTA per tile of MCU rows x columns: dequantise + IDCT (one thread
 //                             per 8x8 block, two 1-D passes in registers) into shared-memory
 //                             component rows, then triangle upsampling + fixed-point colour
 //                             conversion from there into the packed BGR frame.
 #include "common.cuh"
 #include "kernels.cuh"
+#include "jpeg_scan_core.h"
 
 namespace lp {
 
@@ -123,67 +126,6 @@ __device__ __forceinline__ int16_t* roi_block(const JpegDecodeItem& it, int16_t*
 }
 
 // ------------------------------------------------------------------ entropy decode (serial)
-
-struct BitReader {
-    const uint8_t* p;
-    const uint8_t* end;
-    uint64_t acc;
-    int nbits;
-    bool marker;
-};
-
-__device__ __forceinline__ void br_fill(BitReader& b) {
-    while (b.nbits <= 56) {
-        uint32_t byte = 0;
-        if (!b.marker && b.p < b.end) {
-            byte = *b.p;
-            if (byte == 0xFF) {
-                const uint8_t* q = b.p + 1;
-                while (q < b.end && *q == 0xFF) q++;
-                if (q < b.end && *q == 0x00) {
-                    b.p = q + 1;  // stuffed FF
-                } else {
-                    b.marker = true;  // real marker: feed zeros from here on
-                    byte = 0;
-                }
-            } else {
-                b.p++;
-            }
-        }
-        b.acc |= (uint64_t)byte << (56 - b.nbits);
-        b.nbits += 8;
-    }
-}
-
-__device__ __forceinline__ int huff_symbol(BitReader& b, const JpegHuffSet* hs, int t) {
-    if (b.nbits < 32) br_fill(b);
-    const uint32_t peek = (uint32_t)(b.acc >> 48);
-    const uint32_t e = hs->look[t][peek >> 7];
-    if (e) {
-        const int l = e >> 8;
-        b.acc <<= l;
-        b.nbits -= l;
-        return e & 0xFF;
-    }
-    int l = 10;
-    int code = (int)(peek >> 6);
-    while (l <= 16 && code > hs->maxcode[t][l]) {
-        l++;
-        code = (int)(peek >> (16 - l));
-    }
-    if (l > 16) return -1;
-    b.acc <<= l;
-    b.nbits -= l;
-    return hs->vals[t][(code + hs->valoffset[t][l]) & 0xFF];
-}
-
-__device__ __forceinline__ int receive_extend(BitReader& b, int n) {
-    if (b.nbits < 32) br_fill(b);
-    const int v = (int)(b.acc >> (64 - n));
-    b.acc <<= n;
-    b.nbits -= n;
-    return v < (1 << (n - 1)) ? v - (1 << n) + 1 : v;
-}
 
 __global__ void jpeg_huff_decode_kernel(JpegDecodeItem* items, const JpegHuffSet* tables,
                                         const uint8_t* scan, int16_t* coef, int n) {
@@ -388,190 +330,32 @@ int jpeg_rst_launch(JpegDecodeItem* items, const JpegHuffSet* tables, const uint
     return LP_OK;
 }
 
-// ------------------------------------------------------------------ multi-scan files (serial)
-// Progressive JPEG (T.81 Annex G; libjpeg-turbo's jdphuff.c is what the reference runs) and
-// sequential files with one scan per component.  Every scan refines the same coefficient array,
-// and inside a scan the end-of-band runs chain across blocks, so one thread walks the scans in
-// order.  Restated in oracle/oracle_jpeg_dec.c (prog_*), which is pinned on the reference.
+// ------------------------------------------------------------------ multi-scan files (serial per image)
+// One CTA of one warp per item; items that are not multi-scan return at once.  The warp clears the item's ROI
+// blocks (and, for a window smaller than the frame, its nonzero masks), then lane 0 walks every scan
+// (jpeg_scan_core.h).  Refinement scans carry no restart-free synchronisation point the way a baseline scan does
+// (a refinement bit needs the block's history, the history needs the block's position), so the parallelism is
+// across images: a chunk's multi-scan files decode side by side in one launch.
 
-__device__ __forceinline__ int br_bits(BitReader& b, int n) {
-    if (n == 0) return 0;
-    if (b.nbits < 32) br_fill(b);
-    const int v = (int)(b.acc >> (64 - n));
-    b.acc <<= n;
-    b.nbits -= n;
-    return v;
-}
+constexpr int kMultiscanThreads = 32;
 
-struct ProgState {
-    int Ss, Se, Al;
-    unsigned eobrun;
-};
-
-__device__ int prog_ac_first(BitReader& b, const JpegHuffSet* hs, int ta, ProgState& ps, int16_t* blk, const uint8_t* zz) {
-    if (ps.eobrun > 0) {
-        ps.eobrun--;
-        return 0;
-    }
-    for (int k = ps.Ss; k <= ps.Se; k++) {
-        const int rs = huff_symbol(b, hs, ta);
-        if (rs < 0) return -3;
-        int r = rs >> 4;
-        const int n = rs & 15;
-        if (n) {
-            k += r;
-            if (k > 63) return -3;
-            blk[zz[k]] = (int16_t)((unsigned)receive_extend(b, n) << ps.Al);
-        } else if (r == 15) {
-            k += 15;
-        } else {
-            ps.eobrun = 1u << r;
-            if (r) ps.eobrun += (unsigned)br_bits(b, r);
-            ps.eobrun--;
-            break;
-        }
-    }
-    return 0;
-}
-
-__device__ int prog_ac_refine(BitReader& b, const JpegHuffSet* hs, int ta, ProgState& ps, int16_t* blk, const uint8_t* zz) {
-    const int p1 = 1 << ps.Al, m1 = -(1 << ps.Al);
-    int k = ps.Ss;
-    if (ps.eobrun == 0) {
-        for (; k <= ps.Se; k++) {
-            const int rs = huff_symbol(b, hs, ta);
-            if (rs < 0) return -3;
-            int r = rs >> 4;
-            const int n = rs & 15;
-            int val = 0;
-            if (n) {
-                if (n != 1) return -3;
-                val = br_bits(b, 1) ? p1 : m1;
-            } else if (r != 15) {
-                ps.eobrun = 1u << r;
-                if (r) ps.eobrun += (unsigned)br_bits(b, r);
-                break;
-            }
-            do {
-                int16_t* co = blk + zz[k];
-                if (*co != 0) {
-                    if (br_bits(b, 1)) {
-                        if ((*co & p1) == 0) *co = (int16_t)(*co + (*co >= 0 ? p1 : m1));
-                    }
-                } else {
-                    if (--r < 0) break;
-                }
-                k++;
-            } while (k <= ps.Se);
-            if (val) {
-                if (k > 63) return -3;
-                blk[zz[k]] = (int16_t)val;
-            }
-        }
-    }
-    if (ps.eobrun > 0) {
-        for (; k <= ps.Se; k++) {
-            int16_t* co = blk + zz[k];
-            if (*co != 0 && br_bits(b, 1)) {
-                if ((*co & p1) == 0) *co = (int16_t)(*co + (*co >= 0 ? p1 : m1));
-            }
-        }
-        ps.eobrun--;
-    }
-    return 0;
-}
-
-__global__ void jpeg_multiscan_kernel(JpegDecodeItem* item, const JpegScanDesc* scans, int nscans,
-                                      const JpegHuffSet* sets, const uint8_t* file, int16_t* coef) {
+__global__ void __launch_bounds__(kMultiscanThreads)
+    jpeg_multiscan_kernel(JpegDecodeItem* items, const JpegScanDesc* scans, const JpegHuffSet* sets,
+                          const uint8_t* files, int16_t* coef, uint64_t* masks) {
     __shared__ uint8_t zz[64];
+    JpegDecodeItem& it = items[blockIdx.x];
+    if (it.nscans == 0 || it.status != 0) return;
     for (int k = threadIdx.x; k < 64; k += blockDim.x) zz[k] = c_zigzag[k];
-    __syncthreads();
-    if (threadIdx.x != 0 || blockIdx.x != 0) return;
-    JpegDecodeItem& it = *item;
-    int status = 0;
-    for (int s = 0; s < nscans && status == 0; s++) {
-        const JpegScanDesc sc = scans[s];
-        const JpegHuffSet* hs = sets + sc.table_set;
-        BitReader b{file + sc.data_off, file + sc.data_off + sc.data_len, 0, 0, false};
-        ProgState ps{sc.Ss, sc.Se, sc.Al, 0u};
-        int pred[3] = {0, 0, 0};
-        int mcux, mcuy;
-        if (sc.ns == 1) {  // non-interleaved: one block per MCU over the component's true block grid
-            mcux = (it.dw[sc.ci[0]] + 7) / 8;
-            mcuy = (it.dh[sc.ci[0]] + 7) / 8;
-        } else {
-            mcux = it.mcus_x;
-            mcuy = it.mcus_y;
-        }
-        int todo = sc.restart_interval;
-        for (int my = 0; my < mcuy && status == 0; my++) {
-            for (int mx = 0; mx < mcux && status == 0; mx++) {
-                if (sc.restart_interval && todo == 0) {
-                    b.acc = 0;
-                    b.nbits = 0;
-                    const uint8_t* q = b.p;
-                    while (q + 1 < b.end && !(q[0] == 0xFF && q[1] >= 0xD0 && q[1] <= 0xD7)) q++;
-                    if (q + 1 >= b.end) {
-                        status = -3;
-                        break;
-                    }
-                    b.p = q + 2;
-                    b.marker = false;
-                    pred[0] = pred[1] = pred[2] = 0;
-                    ps.eobrun = 0;
-                    todo = sc.restart_interval;
-                }
-                for (int i = 0; i < sc.ns && status == 0; i++) {
-                    const int c = sc.ci[i];
-                    const int bh = sc.ns == 1 ? 1 : it.h[c], bv = sc.ns == 1 ? 1 : it.v[c];
-                    const int td = sc.td[i], ta = 4 + sc.ta[i];
-                    for (int by = 0; by < bv && status == 0; by++) {
-                        for (int bx = 0; bx < bh && status == 0; bx++) {
-                            int16_t* blk = roi_block(it, coef, c, mx * bh + bx, my * bv + by);
-                            if (!blk) {
-                                status = -3;
-                                break;
-                            }
-                            if (!sc.progressive) {  // sequential block: DC difference + AC run/size pairs
-                                const int sz = huff_symbol(b, hs, td);
-                                if (sz < 0 || sz > 15) { status = -3; break; }
-                                if (sz) pred[i] += receive_extend(b, sz);
-                                blk[0] = (int16_t)pred[i];
-                                for (int k = 1; k < 64;) {
-                                    const int rs = huff_symbol(b, hs, ta);
-                                    if (rs < 0) { status = -3; break; }
-                                    const int r = rs >> 4, n = rs & 15;
-                                    if (n == 0) {
-                                        if (r != 15) break;
-                                        k += 16;
-                                        continue;
-                                    }
-                                    k += r;
-                                    if (k > 63) { status = -3; break; }
-                                    blk[zz[k]] = (int16_t)receive_extend(b, n);
-                                    k++;
-                                }
-                            } else if (sc.Ss == 0) {
-                                if (sc.Ah == 0) {  // DC first pass
-                                    const int sz = huff_symbol(b, hs, td);
-                                    if (sz < 0 || sz > 15) { status = -3; break; }
-                                    if (sz) pred[i] += receive_extend(b, sz);
-                                    blk[0] = (int16_t)((unsigned)pred[i] << sc.Al);
-                                } else if (br_bits(b, 1)) {  // DC refinement
-                                    blk[0] |= (int16_t)(1 << sc.Al);
-                                }
-                            } else {
-                                status = sc.Ah == 0 ? prog_ac_first(b, hs, ta, ps, blk, zz)
-                                                    : prog_ac_refine(b, hs, ta, ps, blk, zz);
-                            }
-                        }
-                    }
-                }
-                if (sc.restart_interval) todo--;
-            }
-        }
+    const ScanOrder so = scan_order(it);
+    uint4* const z = reinterpret_cast<uint4*>(coef + it.coef_off);
+    const size_t nz = (size_t)roi_blocks(it, so) * 8;  // 16-byte words
+    for (size_t k = threadIdx.x; k < nz; k += blockDim.x) z[k] = make_uint4(0, 0, 0, 0);
+    if (masks && !roi_is_frame(it)) {
+        uint64_t* const m = masks + it.dcdiff_off;
+        for (uint32_t k = threadIdx.x; k < so.total; k += blockDim.x) m[k] = 0;
     }
-    it.status = status;
+    __syncthreads();
+    if (threadIdx.x == 0) it.status = multiscan_decode(it, scans, sets, files, coef, masks, zz);
 }
 
 // ------------------------------------------------------------------ dequant + ISLOW IDCT
@@ -683,8 +467,8 @@ __device__ __forceinline__ int tile_row(const TileCtx& t, int c, int cy) {
 }
 
 // Dequantise + IDCT ROI MCU row m_ring of the ring components and m_flat of the others (-1: none) over the
-// tile's columns into shared memory, one thread per block.  The serial and multi-scan entropy decoders store
-// blocks per component in raster order; the parallel decoders store them in scan order (jpeg_huff_parallel.cu):
+// tile's columns into shared memory, one thread per block.  The serial baseline decoder stores blocks per
+// component in raster order; the parallel and multi-scan decoders store them in scan order (jpeg_huff_parallel.cu):
 // block (X % h, Y % v) of component c inside ROI MCU (X / h, Y / v).
 __device__ __forceinline__ void idct_phase(const JpegDecodeItem& it, const TileCtx& t, const int16_t* coef,
                                            int mcu_order, const uint16_t (*qt)[64], uint8_t* tile, int m_flat,
@@ -941,33 +725,34 @@ __global__ void __launch_bounds__(kIdctColorThreads, 5)
 
 int jpeg_decode_launch(const JpegDecodeBatch& b, cudaStream_t st, cudaEvent_t ev_after_huff) {
     if (b.n <= 0) return LP_OK;
-    // The serial and multi-scan decoders store only the nonzero coefficients of a zeroed array.  The
-    // parallel decoders (self-synchronising and restart-interval) clear every block of the region of
-    // interest themselves as they open it, so their array is not cleared: at 4096 1080p images that
-    // memset alone would write 15 GB per batch.  Blocks of an image that fails are not read.
-    if (b.scans || !b.use_parallel_huffman)
-        LP_CUDA_OK(cudaMemsetAsync(b.coef, 0, b.coef_elems_total * sizeof(int16_t), st));
-    if (b.scans) {
-        jpeg_multiscan_kernel<<<1, 32, 0, st>>>(b.items, b.scans, b.nscans, b.tables, b.scan, b.coef);
-        g_launches++;
-        LP_CUDA_OK(cudaGetLastError());
-    } else if (b.use_parallel_huffman) {
+    if (b.use_parallel_huffman) {
+        // The parallel decoders (self-synchronising and restart-interval) clear every block of the region of
+        // interest themselves as they open it, so their array is not cleared: at 4096 1080p images a memset
+        // alone would write 15 GB per batch.  Blocks of an image that fails are not read.  Both skip multi-scan
+        // items.
         JpegHuffParallelArgs a{b.items, b.tables, b.scan, b.clean, b.states, b.nslots, b.coef, b.dcdiff, b.n};
         int rc = jpeg_huff_parallel_launch(a, st);  // skips the images that carry restart markers
         if (rc) return rc;
         rc = jpeg_rst_launch(b.items, b.tables, b.scan, b.nslots, b.rst_work, b.n_rst_work, b.n, b.coef, st);
         if (rc) return rc;
-    } else {
+    } else if (b.n_multiscan < b.n) {
+        // the serial decoder stores only the nonzero coefficients of a zeroed array
+        LP_CUDA_OK(cudaMemsetAsync(b.coef, 0, b.coef_elems_total * sizeof(int16_t), st));
         const int threads = 32;
         jpeg_huff_decode_kernel<<<ceil_div(b.n, threads), threads, 0, st>>>(b.items, b.tables, b.scan,
                                                                            b.coef, b.n);
         g_launches++;
         LP_CUDA_OK(cudaGetLastError());
     }
+    if (b.n_multiscan > 0) {  // clears its own blocks
+        jpeg_multiscan_kernel<<<b.n, kMultiscanThreads, 0, st>>>(b.items, b.scans, b.tables, b.scan, b.coef, b.masks);
+        g_launches++;
+        LP_CUDA_OK(cudaGetLastError());
+    }
     if (ev_after_huff) LP_CUDA_OK(cudaEventRecord(ev_after_huff, st));
     if (b.max_tiles_per_image > 0) {
         const dim3 grid((unsigned)b.max_tiles_per_image, b.n);
-        const int mcu_order = !b.scans && b.use_parallel_huffman;
+        const int mcu_order = b.use_parallel_huffman || b.n_multiscan > 0;
         jpeg_idct_color_kernel<<<grid, kIdctColorThreads, kTileSmemBytes, st>>>(b.items, b.coef, b.frames, mcu_order);
         g_launches++;
         LP_CUDA_OK(cudaGetLastError());

@@ -103,7 +103,9 @@ __global__ void __launch_bounds__(kHuffThreads)
     const uint32_t len = it.scan_len;
     uint8_t* dst = clean + it.clean_off;
     const int tid = threadIdx.x, lane = tid & 31;
-    if (it.restart_interval != 0) return;  // restart-interval-parallel path (jpeg_decode.cu): clean_len holds its interval count
+    // restart-interval-parallel path (jpeg_decode.cu): clean_len holds its interval count; multi-scan items: the
+    // serial multi-scan kernel
+    if (it.restart_interval != 0 || it.nscans != 0) return;
     if (it.status != 0) {
         if (tid == 0) it.clean_len = 0;
         return;
@@ -505,7 +507,7 @@ __global__ void __launch_bounds__(kHuffThreads, LP_HUFF_MIN_CTAS)
     __shared__ int s_status;
     JpegDecodeItem& it = items[blockIdx.x];
     const int tid = threadIdx.x;
-    if (it.status != 0 || it.restart_interval != 0) return;  // (DRI images: one thread per restart interval instead)
+    if (it.status != 0 || it.restart_interval != 0 || it.nscans != 0) return;  // (DRI images: one thread per restart interval instead)
     __shared__ long long s_tphase;  // (shared, not a register pair every thread would carry through the loops)
     if (tid == 0) s_tphase = clock64();
     // ---- build the per-CTA tables

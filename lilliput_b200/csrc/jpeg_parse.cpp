@@ -4,6 +4,7 @@
 // Stands where cv::ImageDecoder::readHeader does for the reference
 // (ref opencv.cpp:126-164): width / height / channel count / EXIF orientation.
 #include <cstring>
+#include <vector>
 
 #include "kernels.cuh"
 #include "jpeg_std_tables.h"
@@ -291,7 +292,7 @@ int jpeg_parse_header(const uint8_t* in, size_t len, JpegHeader* out) {
 
 // Second walk for multi-scan files: one JpegScanDesc per SOS, with the DHT / DRI state at that point.
 int jpeg_parse_scans(const uint8_t* in, size_t len, const JpegHeader& h0, JpegScanDesc* scans, int max_scans,
-                     int* nscans, JpegHuffSet* sets, int max_sets, int* nsets) {
+                     int* nscans, JpegHeader* sets, int max_sets, int* nsets) {
     JpegHeader h = h0;  // tracks DHT redefinitions between scans
     memset(h.huff_present, 0, sizeof(h.huff_present));
     h.restart_interval = 0;
@@ -358,7 +359,7 @@ int jpeg_parse_scans(const uint8_t* in, size_t len, const JpegHeader& h0, JpegSc
             }
             if (dirty) {
                 if (*nsets >= max_sets) return LP_ERR_UNSUPPORTED;
-                jpeg_build_huff_set(h, &sets[*nsets]);
+                if (sets) sets[*nsets] = h;
                 (*nsets)++;
                 dirty = false;
             }
@@ -380,6 +381,25 @@ int jpeg_parse_scans(const uint8_t* in, size_t len, const JpegHeader& h0, JpegSc
         pos += 2 + seg;
     }
     return *nscans > 0 ? LP_OK : LP_ERR_INVALID_IMAGE;
+}
+
+int jpeg_parse_scans(const uint8_t* in, size_t len, const JpegHeader& h, JpegScanDesc* scans, int max_scans,
+                     int* nscans, JpegHuffSet* sets, int max_sets, int* nsets) {
+    std::vector<JpegHeader> tables((size_t)(max_sets > 0 ? max_sets : 0));
+    const int rc = jpeg_parse_scans(in, len, h, scans, max_scans, nscans, tables.data(), max_sets, nsets);
+    if (rc == 0)
+        for (int k = 0; k < *nsets; k++) jpeg_build_huff_set(tables[k], &sets[k]);
+    return rc;
+}
+
+size_t jpeg_multiscan_visits(const JpegHeader& h, const JpegScanDesc* scans, int nscans) {
+    size_t visits = 0;
+    for (int k = 0; k < nscans; k++)
+        for (int c = 0; c < scans[k].ns; c++) {
+            const int ci = scans[k].ci[c];
+            visits += (size_t)h.mcus_x * h.mcus_y * h.comp[ci].h * h.comp[ci].v;
+        }
+    return visits;
 }
 
 // Canonical Huffman decode tables (T.81 Annex C / F.2.2.3) in the device layout.

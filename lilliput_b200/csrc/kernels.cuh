@@ -7,6 +7,8 @@
 #include <cstdint>
 #include <vector>
 
+#include "jpeg_types.h"
+
 namespace lp {
 
 // ---- resize.cu ---------------------------------------------------------------------------
@@ -48,53 +50,8 @@ struct JpegHeader {
 // Parses markers up to and including the first SOS.  Returns 0, or a negative lp_status.
 int jpeg_parse_header(const uint8_t* data, size_t len, JpegHeader* out);
 
-// One scan of a multi-scan file (progressive: T.81 Annex G; or non-interleaved sequential).
-struct JpegScanDesc {
-    uint32_t data_off, data_len;  // entropy-coded segment inside the uploaded FILE
-    int32_t ns;                   // components in the scan
-    int32_t ci[3], td[3], ta[3];  // frame component index, DC / AC table ids
-    int32_t Ss, Se, Ah, Al;       // spectral band and successive-approximation bit positions
-    int32_t restart_interval;
-    int32_t table_set;            // Huffman tables in force at this scan
-    int32_t progressive;
-};
 
 // ---- jpeg_decode.cu ------------------------------------------------------------------------
-// Device-side description of one image to decode (array of these lives in HBM).
-struct JpegDecodeItem {
-    uint64_t scan_off;    // offset of the entropy-coded segment in the batch scan buffer
-    uint32_t scan_len;    // bytes
-    uint32_t table_set;   // index into the Huffman table-set array
-    uint64_t coef_off;    // int16 offset of this image's coefficient blocks
-    uint64_t frame_off;   // byte offset of this image's packed output frame
-    int32_t width, height, ncomp;
-    int32_t mcus_x, mcus_y, restart_interval;
-    int32_t h[3], v[3];   // sampling factors
-    int32_t bw[3], bh[3]; // blocks per component plane (padded to the MCU grid)
-    int32_t dw[3], dh[3]; // true downsampled component size in samples
-    uint32_t block_off[3];  // first block of component c inside the image's coef area
-    // tiles of jpeg_idct_color_kernel (one CTA each): tiles_x spans of tile_mcx ROI MCU columns, bands of tile_mcy
-    // ROI MCU rows
-    int32_t tile_mcx, tile_mcy, tiles_x;
-    uint16_t qt[3][64];     // per-component quantisation table, natural order
-    int32_t td[3], ta[3];
-    int32_t status;         // written by the decode kernel: 0 ok, <0 corrupt
-    int32_t frame_channels; // 1 or 3
-    // parallel Huffman path (jpeg_huff_parallel.cu)
-    uint64_t clean_off;     // byte offset of this image's unstuffed bit string
-    uint64_t state_off;     // SubState offset (2 * nsub entries reserved)
-    uint64_t dcdiff_off;    // int16 offset of this image's DC-difference array (MCU order)
-    uint32_t clean_len;     // written by jpeg_unstuff_kernel
-    uint32_t pad_;
-    // Region of interest.  Only MCUs [roi_mx0, roi_mx0+roi_mcx) x [roi_my0, roi_my0+roi_mcy) get
-    // coefficients (bw, bh, block_off describe THAT grid); the packed frame holds
-    // the pixel window [win_x0, win_x0+win_w) x [win_y0, win_y0+win_h) with rows win_stride apart.
-    // A full decode has roi = every MCU and win = the whole image.
-    int32_t roi_mx0, roi_my0, roi_mcx, roi_mcy;
-    int32_t win_x0, win_y0, win_w, win_h;
-    uint32_t win_stride;
-    uint32_t pad2_;
-};
 
 // Fills the ROI / window / layout fields of `it` (whose width, height, ncomp, h, v, mcus_* are set)
 // for the pixel window [x0,x1) x [y0,y1).  align16 rounds the window's x range outwards to 16 px so
@@ -103,33 +60,29 @@ struct JpegDecodeItem {
 uint32_t jpeg_item_set_window(JpegDecodeItem* it, int x0, int y0, int x1, int y1, bool align16,
                               uint32_t* tiles);
 
-// Huffman decode tables for one image (or many images sharing them), device format.
-constexpr int kHuffAcLookBits = 12;    // AC lookahead of the parallel decoder (jpeg_huff_parallel.cu)
-constexpr int kHuffLongPrefixes = 16;  // second-level tables per AC table for codes longer than that
-struct JpegHuffSet {
-    // [class*4+id]: 9-bit lookahead: (len<<8)|symbol, 0 when the code is longer than 9 bits
-    uint16_t look[8][512];
-    int32_t maxcode[8][18];  // canonical decode for long codes; maxcode[17] = sentinel
-    int32_t valoffset[8][17];
-    uint8_t vals[8][256];
-    // AC codes longer than kHuffAcLookBits, two-level: long_prefix[id][j] = their first kHuffAcLookBits
-    // bits (0xFFFF = unused slot), long_sub[id][j][next 4 bits] = (len<<8)|symbol, 0 = not a codeword.
-    // Canonical codes put every long code behind a handful of all-ones prefixes (8 for the Annex K
-    // tables); prefixes that do not fit here are left to the bit-by-bit walk.
-    uint16_t long_prefix[4][kHuffLongPrefixes];
-    uint16_t long_sub[4][kHuffLongPrefixes][16];
-};
 void jpeg_build_huff_set(const JpegHeader& h, JpegHuffSet* out);
 // Walks every SOS of a multi-scan file, snapshotting the Huffman tables / restart interval in force.
-// `sets`/`scans` are caller arrays (max_sets / max_scans entries).  Returns 0 or a negative lp_status.
+// `scans` is a caller array of max_scans entries; each new set of tables in force is copied into `sets` (a header
+// whose huff_* fields hold them; nullptr: only counted) and numbered in JpegScanDesc::table_set from 0.  Returns 0
+// or a negative lp_status.
+int jpeg_parse_scans(const uint8_t* data, size_t len, const JpegHeader& h, JpegScanDesc* scans, int max_scans,
+                     int* nscans, JpegHeader* sets, int max_sets, int* nsets);
+// The same, with the sets built into device-format tables.
 int jpeg_parse_scans(const uint8_t* data, size_t len, const JpegHeader& h, JpegScanDesc* scans, int max_scans,
                      int* nscans, JpegHuffSet* sets, int max_sets, int* nsets);
+// Per-file caps of jpeg_parse_scans' arrays, and the work budget of the serial multi-scan decoder: one thread
+// walks every block of every scan, so a hostile file (up to 256 scans over a large frame) is refused rather than
+// queued.  Real progressive files have ~10 scans; an 8192 x 8192 4:4:4 frame with 20 scans still passes.
+constexpr int kMultiscanMaxScans = 256, kMultiscanMaxSets = 64;
+constexpr size_t kMultiscanMaxVisits = (size_t)1 << 26;
+// Block visits of all scans of a multi-scan file.
+size_t jpeg_multiscan_visits(const JpegHeader& h, const JpegScanDesc* scans, int nscans);
 
 struct JpegDecodeBatch {
     JpegDecodeItem* items;      // device
     const JpegHuffSet* tables;  // device
     const uint8_t* scan;        // device, concatenated entropy-coded segments
-    int16_t* coef;              // device, zeroed by the launcher
+    int16_t* coef;              // device
     uint8_t* frames;            // device, packed BGR / gray frames
     int n;
     size_t coef_elems_total;    // for the memset
@@ -140,9 +93,12 @@ struct JpegDecodeBatch {
     void* states = nullptr;      // SubState[]
     uint32_t* nslots = nullptr;
     int16_t* dcdiff = nullptr;   // DC differences of ALL blocks of an image, MCU order
-    // multi-scan files (n == 1): every scan decoded in order by one thread; `scan` holds the whole file
+    // multi-scan items (JpegDecodeItem::nscans > 0): one thread walks each one's scans (jpeg_scan_core.h); `scan`
+    // holds their whole files, `scans` their scan descriptors, `masks` the nonzero masks of blocks outside the
+    // region of interest (nullptr when every such item decodes its whole frame)
+    int n_multiscan = 0;
     const JpegScanDesc* scans = nullptr;
-    int nscans = 0;
+    uint64_t* masks = nullptr;
     // images with restart markers inside a parallel-Huffman launch: (image, interval) work list (device), one
     // thread per restart interval; their marker offsets live in `nslots` at the image's state_off, the number of
     // intervals the host expects in clean_len

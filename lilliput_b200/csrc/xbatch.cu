@@ -7,14 +7,16 @@
 //   1. headers of all items are parsed on the host by a few threads (format sniff as lilliput.go:129-164);
 //   2. items are grouped by (decoder kind, source geometry) -- a group shares its Fit crop / output size
 //      (ref ops.go:243-255, opencv.go:331-363), so every stage of a group is ONE launch over all its images:
-//        JPEG  -> the lp_batch pipeline (batch.cu): parallel Huffman, IDCT, colour, resize, encode
+//        JPEG  -> the lp_batch pipeline (batch.cu): parallel Huffman, IDCT, colour, resize, encode; multi-scan
+//                 (progressive) files form groups of their own, so a chunk of baseline files never waits for the
+//                 serial decode of a large progressive one
 //        PNG   -> IDAT gather + warp-parallel inflate + defilter + convert (png_decode.cu), resize
 //        WebP  -> VP8 key frames, one frame per warp (webp_decode.cu), resize
 //        GIF   -> every frame of every animation: LZW (one warp per frame), per-pixel compositor over the
 //                 frame sequence (gif_decode.cu), resize of every composited canvas
 //      and the sinks: JPEG (jpeg_encode.cu), lossy WebP still / animation (webp_encode.cu), GIF from GIF sources
 //      (palette mapping + LZW of every frame of the task, gif_decode.cu; the container assembled on the host);
-//   3. anything the grid path does not cover (progressive JPEG sources, EXIF-rotated sources, ICC profiles to carry,
+//   3. anything the grid path does not cover (gray or over-budget multi-scan JPEGs, EXIF-rotated sources, ICC profiles to carry,
 //      lossless WebP output, PNG output, GIF output from other formats ...) and any item whose grid stage fails goes through
 //      lp_transform on a worker thread -- still this library's device kernels, one image per call -- so the
 //      status and bytes of EVERY item are what lp_transform would have returned.
@@ -42,7 +44,8 @@ using namespace lp;
 
 namespace lp {
 lp_batch* batch_create_in(const lp_batch_config* cfg, uint8_t* dev_arena, size_t dev_bytes, uint8_t* host_arena,
-                          size_t host_bytes, bool progressive_jpeg);
+                          size_t host_bytes, bool progressive_jpeg, bool multiscan_sources);
+size_t batch_multiscan_pool_bytes(size_t n);
 }  // namespace lp
 
 namespace {
@@ -56,6 +59,7 @@ struct XItem {
     int ow = 0, oh = 0;             // output size
     int cx = 0, cy = 0, cw = 0, chh = 0;  // crop rectangle fed to the resize
     int jpeg_sampling = 0;          // (h0<<12)|(v0<<8)|... groups JPEGs of one component layout
+    bool jpeg_multiscan = false;    // progressive, or one scan per component
     std::unique_ptr<PngHeader> png;
     WebpStillInfo webp;
     GifAnimPlan* gif = nullptr;
@@ -167,10 +171,19 @@ static void parse_item(lp_xbatch* X, int i) {
     if (d[0] == 0xFF && d[1] == 0xD8) {
         if (X->sink != S_JPEG) return;  // JPEG -> WebP carries the ICC profile and is not a measured path: per image
         JpegHeader h;
-        if (jpeg_parse_header(d, n, &h) != LP_OK || !h.supported || h.multiscan) return;
+        if (jpeg_parse_header(d, n, &h) != LP_OK || (!h.supported && !h.multiscan)) return;
         if (h.ncomp != 3) return;
         if (h.orientation >= 2 && h.orientation <= 8) return;
         if (h.width > max_side || h.height > max_side) return;
+        if (!h.supported) {  // multi-scan: damaged scans and files over the serial decoder's budget go per image
+            std::vector<JpegScanDesc> scans(kMultiscanMaxScans);
+            int nscans = 0, nsets = 0;
+            if (jpeg_parse_scans(d, n, h, scans.data(), (int)scans.size(), &nscans, (JpegHeader*)nullptr, kMultiscanMaxSets,
+                                 &nsets) != LP_OK ||
+                jpeg_multiscan_visits(h, scans.data(), nscans) > kMultiscanMaxVisits)
+                return;
+            it.jpeg_multiscan = true;
+        }
         it.w = h.width;
         it.h = h.height;
         it.ch = 3;
@@ -772,8 +785,10 @@ static void run_jpeg(lp_xbatch* X, Lane& L, const std::vector<int>& idx) {
     if (c.out_cap >= 256) c.out_cap = c.out_cap / 256 * 256;
     // images per chunk: whole Huffman waves while the per-chunk scratch fits the lane's arena
     const size_t mcus = (size_t)ceil_div(g.w, 8) * ceil_div(g.h, 8);
-    const size_t per_img = (mcus * 3 + 64) * (128 + 64 + 2) + (size_t)g.w * g.h * 3 + 65536;
-    const size_t fixed = 2 * in_bytes + (size_t)n * (c.out_cap + (size_t)g.ow * g.oh * 3 + 4096) + (64u << 20);
+    // multi-scan groups: + the nonzero masks per block, + the scan and table-set pools (batch.cu)
+    const size_t per_img = (mcus * 3 + 64) * (128 + 64 + 2 + (g.jpeg_multiscan ? 8 : 0)) + (size_t)g.w * g.h * 3 + 65536;
+    const size_t pools = g.jpeg_multiscan ? batch_multiscan_pool_bytes((size_t)n) : 0;
+    const size_t fixed = 2 * in_bytes + (size_t)n * (c.out_cap + (size_t)g.ow * g.oh * 3 + 4096) + (64u << 20) + pools;
     const int slots = jpeg_huff_parallel_slots();
     long fit = L.dev_bytes > fixed ? (long)((L.dev_bytes - fixed) / per_img) : 0;
     if (fit < 1) {
@@ -783,7 +798,7 @@ static void run_jpeg(lp_xbatch* X, Lane& L, const std::vector<int>& idx) {
     int chunk = (int)std::min<long>(fit, 3L * std::max(slots, 1));
     if (slots > 0 && chunk > slots) chunk = chunk / slots * slots;
     c.chunk = std::max(1, std::min(chunk, n));
-    lp_batch* b = batch_create_in(&c, L.dev, L.dev_bytes, L.host, L.host_bytes, X->progressive);
+    lp_batch* b = batch_create_in(&c, L.dev, L.dev_bytes, L.host, L.host_bytes, X->progressive, g.jpeg_multiscan);
     if (!b) {
         for (int i : idx) push_fallback(X, i);
         return;
@@ -967,7 +982,7 @@ extern "C" int lp_xbatch_transform(lp_xbatch* X, const uint8_t* const* in, const
     for (int i = 0; i < n; i++) {
         const XItem& it = X->items[i];
         if (it.kind == K_FALLBACK) X->fallback.push_back(i);
-        else groups[std::make_tuple((int)it.kind, it.w, it.h, it.ch, it.jpeg_sampling)].push_back(i);
+        else groups[std::make_tuple((int)it.kind, it.w, it.h, it.ch, it.jpeg_sampling | (it.jpeg_multiscan ? 1 << 24 : 0))].push_back(i);
     }
     std::vector<Task> tasks;
     std::vector<double> cost;  // rough device time: the longest tasks start first
