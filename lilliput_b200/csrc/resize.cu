@@ -772,6 +772,20 @@ int resize_launch(const ResizeArgs& a, cudaStream_t st) {
     if (a.crop_w < 1 || a.crop_h < 1 || a.dst_w < 1 || a.dst_h < 1) return LP_ERR_BAD_ARGUMENT;
     if (a.channels != 1 && a.channels != 3 && a.channels != 4) return LP_ERR_BAD_ARGUMENT;
     if (a.interpolation != 1 && a.interpolation != 2 && a.interpolation != 3) return LP_ERR_UNSUPPORTED;
+    // Every kernel below takes the image from blockIdx.z, and gridDim.z is at most 65535: a larger batch (the frames of
+    // a GIF task in lp_xbatch can exceed it) goes in slices of that many images.
+    constexpr int kMaxImagesPerLaunch = 65535;
+    if (a.n > kMaxImagesPerLaunch) {
+        for (int i0 = 0; i0 < a.n; i0 += kMaxImagesPerLaunch) {
+            ResizeArgs s = a;
+            s.src += (size_t)i0 * a.src_img_stride;
+            s.dst += (size_t)i0 * a.dst_img_stride;
+            s.n = std::min(kMaxImagesPerLaunch, a.n - i0);
+            const int rc = resize_launch(s, st);
+            if (rc) return rc;
+        }
+        return LP_OK;
+    }
     const int C = a.channels;
     if (a.crop_w == a.dst_w && a.crop_h == a.dst_h) {  // cv::resize: same size is a copy
         LP_CUDA_OK(cudaMemcpy2DAsync(a.dst, a.dst_row_stride,
