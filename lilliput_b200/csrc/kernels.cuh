@@ -227,14 +227,37 @@ void webp_assemble(const WebpEncodedFrame* frames, int n, const uint8_t* icc, si
                    uint32_t loop_count, std::vector<uint8_t>* file);
 
 // ---- batch helpers of webp_decode.cu / gif_decode.cu (used by xbatch.cu) ------------------------
-struct WebpStillInfo {
-    int width = 0, height = 0;
-    size_t vp8_off = 0, vp8_len = 0;  // "VP8 " payload inside the file
-    bool simple_lossy = false;        // one VP8 key frame, no ALPH / ICCP / animation
+// A WebP file as the per-image decoder (webp_decoder_*) sees it: spans inside the file, frame properties as
+// webp_decoder_get_prev_frame_* report them, background / loop count as webp_decoder_create normalises them.
+struct WebpFramePlan {
+    size_t img_off = 0, img_len = 0;    // "VP8 " / "VP8L" payload (with the RIFF padding byte, as decoded per image)
+    size_t alph_off = 0, alph_len = 0;  // "ALPH" payload, when has_alph
+    bool lossless = false, has_alph = false;
+    int x = 0, y = 0, width = 0, height = 0;
+    int duration = 0;
+    int dispose = 0;  // 1 = dispose to background (clear the rectangle after the frame)
+    int blend = 0;    // 1 = do not blend (copy the rectangle)
 };
-bool webp_still_info(const uint8_t* data, size_t len, WebpStillInfo* out);
-int webp_vp8_decode_batch(const uint8_t* d_in, const uint64_t* in_off, const uint32_t* in_len, int n, const int* width,
-                          const int* height, uint8_t* d_frames, const uint64_t* frame_off, int* h_status, cudaStream_t st);
+struct WebpPlan {
+    int width = 0, height = 0, channels = 3;  // canvas; 4 when the container has the alpha flag
+    bool animated = false;                    // the container's animation flag
+    uint32_t bgcolor = 0xFFFFFFFFu, loop_count = 0;
+    size_t icc_off = 0, icc_len = 0;          // ICCP payload (icc_len 0: none)
+    std::vector<WebpFramePlan> frames;
+};
+bool webp_plan_parse(const uint8_t* data, size_t len, WebpPlan* out);
+// device scratch webp_decode_batch lays out for one plan (uploaded file, VP8 work areas, lossless pixels, alpha planes,
+// job records), not counting the shared VP8L arena
+size_t webp_plan_device_bytes(const WebpPlan& p, size_t file_len);
+// the VP8L arena all lossless / ALPH streams of a plan need to run in one wave (the per-image decoder's bound each)
+size_t webp_plan_arena_bytes(const WebpPlan& p);
+// decodes + composites every frame of `n` WebP files: file a's composited canvas f (plan width x height x channels,
+// round_up(w * h * ch, 256) apart) lands at d_canvases + canvas_off[a] + f * that stride.  Lossless frames and ALPH
+// planes decode in waves of streams whose arena slices fit d_arena.  h_status per file: 0, or the frame failed.
+// ev_uploaded (optional) is recorded once the files are on the device.
+int webp_decode_batch(const WebpPlan* const* plans, const uint8_t* const* files, const size_t* file_len, int n,
+                      uint8_t* d_scratch, size_t scratch_bytes, uint8_t* d_arena, size_t arena_bytes, uint8_t* d_canvases,
+                      const uint64_t* canvas_off, int* h_status, cudaEvent_t ev_uploaded, cudaStream_t st);
 struct GifAnimPlan;
 GifAnimPlan* gif_plan_parse(const uint8_t* data, size_t len, int max_frames);
 void gif_plan_free(GifAnimPlan* p);

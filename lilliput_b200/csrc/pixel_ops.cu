@@ -7,6 +7,7 @@
 // rounded on its own (explicit __f*_rn intrinsics: no FMA contraction), RNE to u8.
 #include "common.cuh"
 #include "kernels.cuh"
+#include "pixel_blend.cuh"
 
 namespace lp {
 
@@ -70,33 +71,13 @@ int copy_region_launch(const uint8_t* src, size_t sstep, int sc, uint8_t* dst, s
     return LP_OK;
 }
 
-__device__ __forceinline__ uint8_t sat_rne(float f) {
-    if (f != f) return 0;  // 0/0 -> NaN -> cvtss2si gives INT_MIN -> saturates to 0
-    const int v = __float2int_rn(f);
-    return (uint8_t)min(max(v, 0), 255);
-}
-
-// "over" compositing exactly as the reference spells it with cv::Mat expressions.
+// "over" compositing exactly as the reference spells it with cv::Mat expressions (pixel_blend.cuh).
 __global__ void blend_region_kernel(const uint8_t* __restrict__ src, size_t sstep, int sc,
                                     uint8_t* __restrict__ dst, size_t dstep, int dc, int w, int h) {
     const int x = blockIdx.x * blockDim.x + threadIdx.x;
     const int y = blockIdx.y;
     if (x >= w || y >= h) return;
-    const uint8_t* s = src + (size_t)y * sstep + (size_t)x * sc;
-    uint8_t* d = dst + (size_t)y * dstep + (size_t)x * dc;
-    const float k = (float)(1.0 / 255.0);
-    const int g = sc == 1;  // grayscale source is expanded to BGR first
-    const float sa = __fmul_rn((float)(sc == 4 ? s[3] : 255), k);
-    const float da = __fmul_rn((float)(dc == 4 ? d[3] : 255), k);
-    const float oma = __fsub_rn(1.0f, sa);
-    const float oa = __fadd_rn(sa, __fmul_rn(da, oma));
-#pragma unroll
-    for (int c = 0; c < 3; c++) {
-        const float scf = __fmul_rn((float)s[g ? 0 : c], k), dcf = __fmul_rn((float)d[c], k);
-        const float num = __fadd_rn(__fmul_rn(scf, sa), __fmul_rn(__fmul_rn(dcf, da), oma));
-        d[c] = sat_rne(__fmul_rn(__fdiv_rn(num, oa), 255.0f));
-    }
-    if (dc == 4) d[3] = sat_rne(__fmul_rn(oa, 255.0f));
+    blend_px(src + (size_t)y * sstep + (size_t)x * sc, sc, dst + (size_t)y * dstep + (size_t)x * dc, dc);
 }
 
 int blend_region_launch(const uint8_t* src, size_t sstep, int sc, uint8_t* dst, size_t dstep, int dc,

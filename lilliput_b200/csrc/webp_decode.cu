@@ -12,12 +12,14 @@
 // planes in HBM; the loop filter then runs warp-wide (32 lanes = the 16 luma + 8 + 8 chroma sample
 // positions of one macroblock edge); a second, fully parallel kernel does libwebp's "fancy"
 // chroma upsampling and the fixed-point YUV->BGR(A) conversion per output pixel.
+#include <algorithm>
 #include <cstring>
 #include <vector>
 
 #include "common.cuh"
 #include "kernels.cuh"
 #include "lp_webp.h"
+#include "pixel_blend.cuh"
 
 #define LP_VP8_FN static __device__
 #define LP_VP8_INL static __device__ __forceinline__
@@ -318,8 +320,8 @@ __global__ void vp8_output_kernel(uint8_t* work, size_t work_stride, int mb_w, i
 }
 
 // VP8L (lossless) frames and ALPH planes: an LZ77 + prefix-coded stream is one serial chain, so
-// one thread walks it (vp8l_core.h) inside a bump arena in HBM; the colour-order conversion to the
-// mat is a separate, parallel kernel.
+// lane 0 of one warp per stream walks it (vp8l_core.h) inside its own slice of a bump arena in HBM.
+// The colour-order conversion to the mat (or to the canvas) is a separate, parallel kernel.
 struct Vp8lItem {
     const uint8_t* data;   // "VP8L" chunk payload, or "ALPH" chunk payload
     uint32_t size;
@@ -328,22 +330,99 @@ struct Vp8lItem {
     size_t arena_cap;
     int is_alph;
     uint8_t* alpha_out;    // is_alph: width*height plane
-    uint32_t** px_out;     // !is_alph: where to leave the pointer to the final ARGB pixels
+    uint32_t** px_out;     // !is_alph, or null: where to leave the pointer to the final ARGB pixels
+    uint32_t* argb_out;    // !is_alph, or null: where the warp copies them (the arena is reused by the next wave)
     int* status;
 };
 
-__global__ void vp8l_decode_kernel(Vp8lItem it) {
-    if (threadIdx.x != 0 || blockIdx.x != 0) return;
-    vp8l::Arena a{it.arena, it.arena_cap, 0};
-    int rc;
-    if (it.is_alph) {
-        rc = vp8l::decode_alph(it.data, it.size, it.width, it.height, a, it.alpha_out);
-    } else {
-        uint32_t* px = nullptr;
-        rc = vp8l::decode_vp8l(it.data, it.size, it.width, it.height, a, &px);
-        *it.px_out = px;
+constexpr int kVp8lWarpsPerBlock = 4;
+
+__global__ void __launch_bounds__(kVp8lWarpsPerBlock * 32) vp8l_decode_kernel(const Vp8lItem* items, int n) {
+    const int idx = blockIdx.x * kVp8lWarpsPerBlock + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+    if (idx >= n) return;
+    const Vp8lItem& it = items[idx];
+    int rc = 0;
+    uint32_t* px = nullptr;
+    if (lane == 0) {
+        vp8l::Arena a{it.arena, it.arena_cap, 0};
+        if (it.is_alph) {
+            rc = vp8l::decode_alph(it.data, it.size, it.width, it.height, a, it.alpha_out);
+        } else {
+            rc = vp8l::decode_vp8l(it.data, it.size, it.width, it.height, a, &px);
+            if (it.px_out) *it.px_out = px;
+        }
+        if (rc) *it.status = rc;
     }
-    if (rc) *it.status = rc;
+    if (it.is_alph || !it.argb_out) return;
+    rc = __shfl_sync(0xffffffffu, rc, 0);
+    px = reinterpret_cast<uint32_t*>(__shfl_sync(0xffffffffu, reinterpret_cast<unsigned long long>(px), 0));
+    if (rc || !px) return;
+    const size_t npix = (size_t)it.width * it.height;
+    for (size_t i = lane; i < npix; i += 32) it.argb_out[i] = px[i];
+}
+
+static int vp8l_decode_launch(const Vp8lItem* d_items, int n, cudaStream_t st) {
+    if (n <= 0) return LP_OK;
+    vp8l_decode_kernel<<<ceil_div(n, kVp8lWarpsPerBlock), kVp8lWarpsPerBlock * 32, 0, st>>>(d_items, n);
+    g_launches++;
+    LP_CUDA_OK(cudaGetLastError());
+    return LP_OK;
+}
+
+// ------------------------------------------------------------------ frame compositor (batch path)
+// Every frame of every animation (a still is one frame, copied) straight from the decoders' output onto its canvas:
+// one thread per canvas pixel walks the frame sequence with the pixel's state in registers, exactly the per-image
+// region-op sequence of ImageOps (ref ops.go:170-238, 552-582): blend or copy the frame's pixel -> store the composited
+// canvas -> clear the pixel if the frame disposes to background.  Every step is a function of one pixel.
+struct WebpFrameJob {
+    uint64_t work_off;   // lossy: VP8 work area, from the scratch base
+    uint64_t px_off;     // lossless: ARGB words; lossy: ALPH plane (~0: none, alpha 255)
+    int32_t x, y, w, h;
+    int32_t lossless, blend, dispose, mb_w, mb_h, pad_;
+};
+struct WebpAnimJob {
+    uint64_t canvas_off, canvas_stride;
+    int32_t first_frame, nframes, width, height, channels, pad_;
+};
+
+__global__ void webp_compose_kernel(const WebpAnimJob* anims, const WebpFrameJob* jobs, const uint8_t* base, uint8_t* canvases) {
+    const int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y;
+    const WebpAnimJob a = anims[blockIdx.z];
+    if (x >= a.width || y >= a.height) return;
+    const int ch = a.channels;
+    uint8_t px[4] = {0, 0, 0, 0};  // the composite buffer starts transparent (ClearToTransparent of the whole canvas)
+    uint8_t* out = canvases + a.canvas_off + ((size_t)y * a.width + x) * ch;
+    for (int k = 0; k < a.nframes; k++) {
+        const WebpFrameJob& f = jobs[a.first_frame + k];
+        const int fx = x - f.x, fy = y - f.y;
+        const bool inside = fx >= 0 && fx < f.w && fy >= 0 && fy < f.h;
+        if (inside) {
+            uint8_t s[4];
+            const size_t at = (size_t)fy * f.w + fx;
+            if (f.lossless) {
+                const uint32_t v = reinterpret_cast<const uint32_t*>(base + f.px_off)[at];
+                s[0] = (uint8_t)v;
+                s[1] = (uint8_t)(v >> 8);
+                s[2] = (uint8_t)(v >> 16);
+                s[3] = (uint8_t)(v >> 24);
+            } else {
+                vp8::Work w;
+                vp8::work_carve(const_cast<uint8_t*>(base) + f.work_off, f.mb_w, f.mb_h, w);
+                const int u = vp8::upsample_at(w.u, f.mb_w * 8, f.w, f.h, fx, fy);
+                const int v = vp8::upsample_at(w.v, f.mb_w * 8, f.w, f.h, fx, fy);
+                vp8::yuv_to_bgr(w.y[(size_t)fy * (f.mb_w * 16) + fx], u, v, s);
+                s[3] = f.px_off != ~0ull ? base[f.px_off + at] : 255;
+            }
+            if (f.blend) {  // NoBlend: copyTo, equal channel counts
+                for (int c = 0; c < ch; c++) px[c] = s[c];
+            } else {
+                blend_px(s, ch, px, ch);
+            }
+        }
+        uint8_t* d = out + (size_t)k * a.canvas_stride;
+        for (int c = 0; c < ch; c++) d[c] = px[c];
+        if (inside && f.dispose) px[0] = px[1] = px[2] = px[3] = 0;
+    }
 }
 
 __global__ void argb_output_kernel(uint32_t* const* px_ptr, int width, int height, uint8_t* dst, size_t dst_step,
@@ -557,69 +636,196 @@ static bool webp_parse(const uint8_t* b, size_t size, WebpContainer* c) {
 
 // ------------------------------------------------------------------ batch helpers (xbatch.cu)
 
-// What the batch path needs to know about a file: is it ONE lossy key frame without alpha, profile or
-// animation (then its VP8 payload can join a grid launch), and where that payload lies.
-bool webp_still_info(const uint8_t* data, size_t len, WebpStillInfo* out) {
+// The per-image decoder's view of a file (webp_decoder_create / _decode / _get_prev_frame_*), from the same walk.
+bool webp_plan_parse(const uint8_t* data, size_t len, WebpPlan* out) {
     WebpContainer c;
     if (!webp_parse(data, len, &c)) return false;
-    if (c.frames.size() != 1) return true;
-    const WebpFrame& f = c.frames[0];
     out->width = c.canvas_w;
     out->height = c.canvas_h;
-    out->vp8_off = f.img_off;
-    out->vp8_len = f.img_len;
-    out->simple_lossy = !f.lossless && !f.has_alph && !c.has_icc && !(c.flags & kFlagAnim) && !(c.flags & kFlagAlpha) &&
-                        f.width == c.canvas_w && f.height == c.canvas_h && f.img_off + f.img_len <= len;
+    out->channels = (c.flags & kFlagAlpha) ? 4 : 3;  // webp_decoder_get_pixel_type
+    out->animated = (c.flags & kFlagAnim) != 0;
+    out->bgcolor = out->animated ? c.bgcolor : 0xFFFFFFFFu;
+    out->loop_count = out->animated ? c.loop_count : 0;
+    out->icc_off = c.has_icc ? c.icc_off : 0;
+    out->icc_len = c.has_icc ? c.icc_len : 0;
+    out->frames.clear();
+    for (const WebpFrame& f : c.frames) {
+        WebpFramePlan p;
+        p.img_off = f.img_off;
+        p.img_len = f.img_len;
+        p.alph_off = f.alph_off;
+        p.alph_len = f.alph_len;
+        p.lossless = f.lossless;
+        p.has_alph = f.has_alph;
+        p.x = f.x_off;
+        p.y = f.y_off;
+        p.width = f.width;
+        p.height = f.height;
+        p.duration = f.duration;
+        p.dispose = f.dispose;
+        p.blend = f.blend;
+        out->frames.push_back(p);
+    }
     return true;
 }
 
-// n VP8 key frames (any sizes, equal sizes adjacent): one warp per frame (vp8_decode_kernel) in ONE launch,
-// then every pixel of every frame through the fancy upsampler + colour conversion, one launch per run of
-// equal geometry.  Packed BGR frames at d_frames + frame_off[i].
-int webp_vp8_decode_batch(const uint8_t* d_in, const uint64_t* in_off, const uint32_t* in_len, int n, const int* width,
-                          const int* height, uint8_t* d_frames, const uint64_t* frame_off, int* h_status, cudaStream_t st) {
+// the per-image decoder's VP8L arena bound, per stream
+static size_t vp8l_slice_bytes(const WebpFramePlan& f) { return round_up((size_t)f.width * f.height * 12 + (16u << 20), (size_t)256); }
+// the ALPH plane is decoded only onto a 4-channel canvas (webp_decoder_decode's need_alph)
+static bool frame_needs_alph(const WebpPlan& p, const WebpFramePlan& f) { return f.has_alph && !f.lossless && p.channels == 4; }
+static size_t file_slot_bytes(size_t file_len) { return round_up(file_len + 4096, (size_t)256); }
+// VP8 work area, lossless ARGB words or the ALPH plane of one frame
+static size_t frame_slot_bytes(const WebpPlan& p, const WebpFramePlan& f) {
+    const size_t npix = (size_t)f.width * f.height;
+    if (f.lossless) return round_up(npix * 4, (size_t)256);
+    return round_up(vp8::work_bytes((f.width + 15) >> 4, (f.height + 15) >> 4), (size_t)256) +
+           (frame_needs_alph(p, f) ? round_up(npix, (size_t)256) : 0);
+}
+static constexpr size_t kFrameRecordBytes = sizeof(WebpFrameJob) + sizeof(Vp8Item) + sizeof(Vp8lItem) + 4;
+
+size_t webp_plan_device_bytes(const WebpPlan& p, size_t file_len) {
+    size_t b = file_slot_bytes(file_len) + sizeof(WebpAnimJob) + 5 * 256;
+    for (const WebpFramePlan& f : p.frames) b += frame_slot_bytes(p, f) + kFrameRecordBytes;
+    return b;
+}
+
+size_t webp_plan_arena_bytes(const WebpPlan& p) {
+    size_t b = 0;
+    for (const WebpFramePlan& f : p.frames)
+        if (f.lossless || frame_needs_alph(p, f)) b += vp8l_slice_bytes(f);
+    return b;
+}
+
+// Uploads the files, then: ONE vp8_decode_kernel launch over every lossy frame (one warp per frame), the VP8L / ALPH
+// streams in waves of one launch each (one warp per stream, each with its own arena slice), and ONE compositor launch
+// over every canvas pixel of every file (per run of equal canvas size).
+int webp_decode_batch(const WebpPlan* const* plans, const uint8_t* const* files, const size_t* file_len, int n,
+                      uint8_t* d_scratch, size_t scratch_bytes, uint8_t* d_arena, size_t arena_bytes, uint8_t* d_canvases,
+                      const uint64_t* canvas_off, int* h_status, cudaEvent_t ev_uploaded, cudaStream_t st) {
     if (n <= 0) return LP_OK;
-    std::vector<size_t> work_off((size_t)n + 1, 0);
-    for (int i = 0; i < n; i++) work_off[i + 1] = work_off[i] + vp8::work_bytes((width[i] + 15) >> 4, (height[i] + 15) >> 4);
-    uint8_t* scratch = nullptr;
-    const size_t items_b = round_up((size_t)n * sizeof(Vp8Item), (size_t)256), stat_b = round_up((size_t)n * 4, (size_t)256);
-    if (cudaMallocAsync(&scratch, items_b + stat_b + work_off[n], st) != cudaSuccess) {
-        cudaGetLastError();
-        return LP_ERR_CUDA;
-    }
-    Vp8Item* d_items = reinterpret_cast<Vp8Item*>(scratch);
-    int* d_status = reinterpret_cast<int*>(scratch + items_b);
-    uint8_t* d_work = scratch + items_b + stat_b;
-    std::vector<Vp8Item> items((size_t)n);
-    for (int i = 0; i < n; i++)
-        items[i] = Vp8Item{d_in + in_off[i], in_len[i], d_work + work_off[i], d_status + i, (width[i] + 15) >> 4, (height[i] + 15) >> 4};
-    int rc = LP_OK;
-    cudaMemsetAsync(d_status, 0, (size_t)n * 4, st);
-    if (cudaMemcpyAsync(d_items, items.data(), (size_t)n * sizeof(Vp8Item), cudaMemcpyHostToDevice, st) != cudaSuccess) rc = LP_ERR_CUDA;
-    if (!rc) {
-        vp8_decode_kernel<<<ceil_div(n, kVp8WarpsPerBlock), kVp8WarpsPerBlock * 32, 0, st>>>(d_items, n);
-        g_launches++;
-        for (int i0 = 0; i0 < n;) {
-            // frames of one geometry lie back to back, round_up(w * h * 3, 256) apart (the caller's layout)
-            const size_t fstride = round_up((size_t)width[i0] * height[i0] * 3, (size_t)256);
-            int i1 = i0 + 1;
-            while (i1 < n && width[i1] == width[i0] && height[i1] == height[i0] &&
-                   frame_off[i1] == frame_off[i0] + (uint64_t)(i1 - i0) * fstride)
-                i1++;
-            const int mb_w = (width[i0] + 15) >> 4, mb_h = (height[i0] + 15) >> 4;
-            dim3 grid(ceil_div(width[i0], 128), height[i0], i1 - i0);
-            vp8_output_kernel<<<grid, 128, 0, st>>>(d_work + work_off[i0], vp8::work_bytes(mb_w, mb_h), mb_w, mb_h, width[i0],
-                                                    height[i0], d_frames + frame_off[i0], fstride, (size_t)width[i0] * 3, 3, nullptr);
-            g_launches++;
-            i0 = i1;
+    int nf = 0;
+    for (int a = 0; a < n; a++) nf += (int)plans[a]->frames.size();
+    // records first, then the files, then the per-frame slots
+    size_t used = 0;
+    auto take = [&](size_t bytes) {
+        const size_t at = used;
+        used += round_up(bytes, (size_t)256);
+        return at;
+    };
+    const size_t anims_at = take((size_t)n * sizeof(WebpAnimJob)), jobs_at = take((size_t)nf * sizeof(WebpFrameJob));
+    const size_t vp8_at = take((size_t)nf * sizeof(Vp8Item)), vp8l_at = take((size_t)nf * sizeof(Vp8lItem));
+    const size_t status_at = take((size_t)nf * 4);
+    std::vector<size_t> file_at((size_t)n);
+    for (int a = 0; a < n; a++) file_at[a] = take(file_slot_bytes(file_len[a]));
+    std::vector<WebpAnimJob> anims((size_t)n);
+    std::vector<WebpFrameJob> jobs((size_t)nf);
+    std::vector<Vp8Item> vp8;
+    std::vector<Vp8lItem> vp8l;
+    std::vector<size_t> slice;  // arena bytes of every VP8L / ALPH stream
+    int* d_status = reinterpret_cast<int*>(d_scratch + status_at);
+    for (int a = 0, k = 0; a < n; a++) {
+        const WebpPlan& p = *plans[a];
+        WebpAnimJob& aj = anims[a];
+        memset(&aj, 0, sizeof(aj));
+        aj.canvas_off = canvas_off[a];
+        aj.canvas_stride = round_up((size_t)p.width * p.height * p.channels, (size_t)256);
+        aj.first_frame = k;
+        aj.nframes = (int)p.frames.size();
+        aj.width = p.width;
+        aj.height = p.height;
+        aj.channels = p.channels;
+        const uint8_t* d_file = d_scratch + file_at[a];
+        for (const WebpFramePlan& f : p.frames) {
+            WebpFrameJob& j = jobs[k];
+            memset(&j, 0, sizeof(j));
+            j.x = f.x;
+            j.y = f.y;
+            j.w = f.width;
+            j.h = f.height;
+            j.lossless = f.lossless;
+            j.blend = f.blend;
+            j.dispose = f.dispose;
+            j.mb_w = (f.width + 15) >> 4;
+            j.mb_h = (f.height + 15) >> 4;
+            j.px_off = ~0ull;
+            const size_t npix = (size_t)f.width * f.height;
+            if (f.lossless) {
+                j.px_off = take(npix * 4);
+                vp8l.push_back(Vp8lItem{d_file + f.img_off, (uint32_t)f.img_len, f.width, f.height, nullptr, 0, 0, nullptr, nullptr,
+                                        reinterpret_cast<uint32_t*>(d_scratch + j.px_off), d_status + k});
+                slice.push_back(vp8l_slice_bytes(f));
+            } else {
+                j.work_off = take(vp8::work_bytes(j.mb_w, j.mb_h));
+                vp8.push_back(Vp8Item{d_file + f.img_off, (uint32_t)f.img_len, d_scratch + j.work_off, d_status + k, j.mb_w, j.mb_h});
+                if (frame_needs_alph(p, f)) {
+                    j.px_off = take(npix);
+                    vp8l.push_back(Vp8lItem{d_file + f.alph_off, (uint32_t)f.alph_len, f.width, f.height, nullptr, 0, 1,
+                                            d_scratch + j.px_off, nullptr, nullptr, d_status + k});
+                    slice.push_back(vp8l_slice_bytes(f));
+                }
+            }
+            k++;
         }
+    }
+    if (used > scratch_bytes) return LP_ERR_BUF_TOO_SMALL;
+    // VP8L / ALPH waves: consecutive streams while their slices fit the arena (a stream larger than the whole arena
+    // gets all of it: arena exhaustion is a clean decode error, and its file goes to the caller's fallback)
+    std::vector<int> wave_first;
+    for (size_t s = 0, fill = 0; s < vp8l.size(); s++) {
+        const size_t need = std::min(slice[s], arena_bytes);
+        if (s == 0 || fill + need > arena_bytes) {
+            wave_first.push_back((int)s);
+            fill = 0;
+        }
+        vp8l[s].arena = d_arena + fill;
+        vp8l[s].arena_cap = need;
+        fill += need;
+    }
+    wave_first.push_back((int)vp8l.size());
+    if (!vp8l.empty() && (!d_arena || arena_bytes == 0)) return LP_ERR_BUF_TOO_SMALL;
+    int rc = LP_OK;
+    auto up = [&](size_t at, const void* src, size_t bytes) {
+        if (!rc && bytes && cudaMemcpyAsync(d_scratch + at, src, bytes, cudaMemcpyHostToDevice, st) != cudaSuccess) rc = LP_ERR_CUDA;
+    };
+    for (int a = 0; a < n; a++) up(file_at[a], files[a], file_len[a]);
+    up(anims_at, anims.data(), anims.size() * sizeof(WebpAnimJob));
+    up(jobs_at, jobs.data(), jobs.size() * sizeof(WebpFrameJob));
+    up(vp8_at, vp8.data(), vp8.size() * sizeof(Vp8Item));
+    up(vp8l_at, vp8l.data(), vp8l.size() * sizeof(Vp8lItem));
+    if (!rc && cudaMemsetAsync(d_status, 0, (size_t)nf * 4, st) != cudaSuccess) rc = LP_ERR_CUDA;
+    if (ev_uploaded) cudaEventRecord(ev_uploaded, st);
+    if (!rc && !vp8.empty()) {
+        const int m = (int)vp8.size();
+        vp8_decode_kernel<<<ceil_div(m, kVp8WarpsPerBlock), kVp8WarpsPerBlock * 32, 0, st>>>(
+            reinterpret_cast<const Vp8Item*>(d_scratch + vp8_at), m);
+        g_launches++;
         if (cudaGetLastError() != cudaSuccess) rc = LP_ERR_CUDA;
     }
-    if (!rc && (cudaMemcpyAsync(h_status, d_status, (size_t)n * 4, cudaMemcpyDeviceToHost, st) != cudaSuccess ||
-                cudaStreamSynchronize(st) != cudaSuccess))  // (also keeps `items` alive until the copy has been consumed)
+    const Vp8lItem* d_vp8l = reinterpret_cast<const Vp8lItem*>(d_scratch + vp8l_at);
+    for (size_t w = 0; !rc && w + 1 < wave_first.size(); w++)
+        rc = vp8l_decode_launch(d_vp8l + wave_first[w], wave_first[w + 1] - wave_first[w], st);
+    // one compositor launch per run of equal canvas size (the caller keeps equal sizes adjacent), <= 65535 files each
+    for (int a0 = 0; !rc && a0 < n;) {
+        int a1 = a0 + 1;
+        while (a1 < n && a1 - a0 < 65535 && plans[a1]->width == plans[a0]->width && plans[a1]->height == plans[a0]->height) a1++;
+        webp_compose_kernel<<<dim3(ceil_div(plans[a0]->width, 128), plans[a0]->height, a1 - a0), 128, 0, st>>>(
+            reinterpret_cast<const WebpAnimJob*>(d_scratch + anims_at) + a0, reinterpret_cast<const WebpFrameJob*>(d_scratch + jobs_at),
+            d_scratch, d_canvases);
+        g_launches++;
+        if (cudaGetLastError() != cudaSuccess) rc = LP_ERR_CUDA;
+        a0 = a1;
+    }
+    std::vector<int> fst((size_t)nf, 0);
+    if (!rc && (cudaMemcpyAsync(fst.data(), d_status, (size_t)nf * 4, cudaMemcpyDeviceToHost, st) != cudaSuccess ||
+                cudaStreamSynchronize(st) != cudaSuccess))  // (also keeps the host records alive until the copies are done)
         rc = LP_ERR_CUDA;
-    cudaFreeAsync(scratch, st);
-    return rc;
+    if (rc) return rc;
+    for (int a = 0; a < n; a++) {
+        h_status[a] = 0;
+        for (int k = anims[a].first_frame; k < anims[a].first_frame + anims[a].nframes; k++)
+            if (fst[k]) h_status[a] = fst[k];
+    }
+    return LP_OK;
 }
 
 // The mat handle is defined in abi_opencv.cu.
@@ -644,6 +850,7 @@ struct webp_decoder_struct {
     uint8_t* d_in = nullptr;
     uint8_t* d_work = nullptr;
     Vp8Item* d_item = nullptr;
+    Vp8lItem* d_litem = nullptr;
     int* d_status = nullptr;
     uint8_t* d_arena = nullptr;   // VP8L / ALPH bump arena
     uint8_t* d_alpha = nullptr;   // decoded ALPH plane
@@ -710,6 +917,7 @@ void webp_decoder_release(webp_decoder d) {
     if (d->d_in) cudaFreeAsync(d->d_in, st);
     if (d->d_work) cudaFreeAsync(d->d_work, st);
     if (d->d_item) cudaFreeAsync(d->d_item, st);
+    if (d->d_litem) cudaFreeAsync(d->d_litem, st);
     if (d->d_status) cudaFreeAsync(d->d_status, st);
     if (d->d_arena) cudaFreeAsync(d->d_arena, st);
     if (d->d_alpha) cudaFreeAsync(d->d_alpha, st);
@@ -744,6 +952,7 @@ bool webp_decoder_decode(const webp_decoder d, opencv_mat mat) {
     };
     if (!d->d_item) {
         if (cudaMallocAsync(&d->d_item, sizeof(Vp8Item), st) != cudaSuccess) return false;
+        if (cudaMallocAsync(&d->d_litem, sizeof(Vp8lItem), st) != cudaSuccess) return false;
         if (cudaMallocAsync(&d->d_status, sizeof(int), st) != cudaSuccess) return false;
         if (cudaMallocAsync(&d->d_px, sizeof(uint32_t*), st) != cudaSuccess) return false;
     }
@@ -758,9 +967,9 @@ bool webp_decoder_decode(const webp_decoder d, opencv_mat mat) {
         if (!grow(&d->d_arena, &d->arena_cap, arena_need)) return false;
     }
     if (f.lossless) {
-        Vp8lItem li{d->d_in, (uint32_t)f.img_len, f.width, f.height, d->d_arena, d->arena_cap, 0, nullptr, d->d_px, d->d_status};
-        vp8l_decode_kernel<<<1, 32, 0, st>>>(li);
-        g_launches++;
+        Vp8lItem li{d->d_in, (uint32_t)f.img_len, f.width, f.height, d->d_arena, d->arena_cap, 0, nullptr, d->d_px, nullptr, d->d_status};
+        cudaMemcpyAsync(d->d_litem, &li, sizeof(li), cudaMemcpyHostToDevice, st);
+        if (vp8l_decode_launch(d->d_litem, 1, st)) return false;
         dim3 grid(ceil_div(f.width, 128), f.height);
         argb_output_kernel<<<grid, 128, 0, st>>>(d->d_px, f.width, f.height, frame_dev, frame_step, channels);
         g_launches++;
@@ -771,9 +980,9 @@ bool webp_decoder_decode(const webp_decoder d, opencv_mat mat) {
             if (!grow(&d->d_alph_in, &d->alph_in_cap, f.alph_len + 4096)) return false;
             if (!grow(&d->d_alpha, &d->alpha_cap, npix + 256)) return false;
             cudaMemcpyAsync(d->d_alph_in, d->bytes + f.alph_off, f.alph_len, cudaMemcpyHostToDevice, st);
-            Vp8lItem ai{d->d_alph_in, (uint32_t)f.alph_len, f.width, f.height, d->d_arena, d->arena_cap, 1, d->d_alpha, nullptr, d->d_status};
-            vp8l_decode_kernel<<<1, 32, 0, st>>>(ai);
-            g_launches++;
+            Vp8lItem ai{d->d_alph_in, (uint32_t)f.alph_len, f.width, f.height, d->d_arena, d->arena_cap, 1, d->d_alpha, nullptr, nullptr, d->d_status};
+            cudaMemcpyAsync(d->d_litem, &ai, sizeof(ai), cudaMemcpyHostToDevice, st);
+            if (vp8l_decode_launch(d->d_litem, 1, st)) return false;
         }
         Vp8Item item{d->d_in, (uint32_t)f.img_len, d->d_work, d->d_status, mb_w, mb_h};
         cudaMemcpyAsync(d->d_item, &item, sizeof(item), cudaMemcpyHostToDevice, st);

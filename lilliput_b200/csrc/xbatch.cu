@@ -11,7 +11,8 @@
 //                 (progressive) files form groups of their own, so a chunk of baseline files never waits for the
 //                 serial decode of a large progressive one
 //        PNG   -> IDAT gather + warp-parallel inflate + defilter + convert (png_decode.cu), resize
-//        WebP  -> VP8 key frames, one frame per warp (webp_decode.cu), resize
+//        WebP  -> stills and animations: VP8 frames one per warp, VP8L / ALPH streams one per warp in arena-sized waves,
+//                 a per-pixel compositor over every file's frame sequence (webp_decode.cu), resize of every canvas
 //        GIF   -> every frame of every animation: LZW (one warp per frame), per-pixel compositor over the
 //                 frame sequence (gif_decode.cu), resize of every composited canvas
 //      and the sinks: JPEG (jpeg_encode.cu), lossy WebP still / animation (webp_encode.cu), GIF from GIF sources
@@ -61,7 +62,7 @@ struct XItem {
     int jpeg_sampling = 0;          // (h0<<12)|(v0<<8)|... groups JPEGs of one component layout
     bool jpeg_multiscan = false;    // progressive, or one scan per component
     std::unique_ptr<PngHeader> png;
-    WebpStillInfo webp;
+    std::unique_ptr<WebpPlan> webp;  // (for WebP: the frames' spans, rectangles and blend / dispose)
     GifAnimPlan* gif = nullptr;
     int gif_frames = 0;
 };
@@ -221,14 +222,31 @@ static void parse_item(lp_xbatch* X, int i) {
     }
     if (!memcmp(d, "RIFF", 4) && !memcmp(d + 8, "WEBP", 4)) {
         if (X->sink == S_GIF) return;
-        WebpStillInfo w;
-        if (!webp_still_info(d, n, &w) || !w.simple_lossy) return;
-        if (w.width > max_side || w.height > max_side) return;
-        it.webp = w;
-        it.w = w.width;
-        it.h = w.height;
-        it.ch = 3;
+        std::unique_ptr<WebpPlan> p(new WebpPlan);
+        if (!webp_plan_parse(d, n, p.get())) return;  // damaged containers: per image
+        if (p->width > max_side || p->height > max_side) return;
+        WebpFramePlan& f0 = p->frames[0];
+        if (p->frames.size() == 1) {
+            // Transform does not composite a still: it resizes the decoded frame, which must then be the canvas
+            if (f0.x || f0.y || f0.width != p->width || f0.height != p->height) return;
+            // a still written to WebP with no time to encode: lp_transform's deadline check follows the frame.  Only the
+            // simple lossy stills the grid has always taken keep going there; the others stay with lp_transform
+            const bool simple = !f0.lossless && !f0.has_alph && !p->icc_len && !p->animated && p->channels == 3;
+            if (X->sink == S_WEBP && X->opt.encode_timeout_ns <= 0 && !simple) return;
+            f0.blend = 1;  // copied onto a canvas of its own size, never disposed
+            f0.dispose = 0;
+        } else {
+            // animations -> animated WebP, with the option gates of GIF -> WebP; Transform checks its deadline after
+            // every non-final frame, so a zero budget fails there (ErrEncodeTimeout): per image
+            if (X->sink != S_WEBP || X->opt.disable_animated_output || X->opt.max_encode_frames != 0 ||
+                X->opt.max_encode_duration_ns != 0 || X->opt.encode_timeout_ns <= 0)
+                return;
+        }
+        it.w = p->width;
+        it.h = p->height;
+        it.ch = p->channels;
         if (!plan_geometry(X->opt, &it)) return;
+        it.webp = std::move(p);
         it.kind = K_WEBP;
         return;
     }
@@ -381,54 +399,6 @@ static std::vector<Run> runs_of(const lp_xbatch* X, const std::vector<int>& idx)
         k = e;
     }
     return r;
-}
-
-// resize of every run + sinks.  frame_off / frame_stride describe the decoded frames; ok[k] = decode succeeded.
-static void resize_and_encode(lp_xbatch* X, Lane& L, Bump& bump, const std::vector<int>& idx, const std::vector<Run>& runs,
-                              const uint8_t* d_frames, const std::vector<uint64_t>& frame_off, const std::vector<char>& ok,
-                              std::vector<int>* failed) {
-    struct Out { uint8_t* d; size_t stride; };
-    std::vector<Out> outs(runs.size());
-    bool good = true;
-    cudaEventRecord(L.ev[1], L.st);
-    for (size_t r = 0; r < runs.size() && good; r++) {
-        const XItem& g = X->items[idx[runs[r].k0]];
-        const int n = runs[r].k1 - runs[r].k0;
-        const size_t fs = round_up((size_t)g.w * g.h * g.ch, (size_t)256);
-        outs[r].stride = round_up((size_t)g.ow * g.oh * g.ch, (size_t)256);
-        outs[r].d = bump.take<uint8_t>((size_t)n * outs[r].stride + 256);
-        if (!outs[r].d) { good = false; break; }
-        ResizeArgs a{d_frames + frame_off[runs[r].k0], fs, (size_t)g.w * g.ch, g.ch, g.cx, g.cy, g.cw, g.chh, outs[r].d,
-                     outs[r].stride, (size_t)g.ow * g.ch, g.ow, g.oh, n, 3};
-        good = resize_launch(a, L.st) == LP_OK;
-    }
-    cudaEventRecord(L.ev[2], L.st);
-    if (good) good = cudaStreamSynchronize(L.st) == cudaSuccess;
-    if (!good) {
-        cudaGetLastError();
-        failed->insert(failed->end(), idx.begin(), idx.end());
-        return;
-    }
-    lane_time(L, 0, 1, &L.ms_decode);
-    lane_time(L, 1, 2, &L.ms_resize);
-    cudaEventRecord(L.ev[2], L.st);
-    for (size_t r = 0; r < runs.size(); r++) {
-        const XItem& g = X->items[idx[runs[r].k0]];
-        std::vector<int> sub;
-        bool all = true;
-        for (int k = runs[r].k0; k < runs[r].k1; k++) {
-            all = all && ok[k];
-            sub.push_back(idx[k]);
-        }
-        if (!all) {  // rare: a corrupt stream in the run -- the run's items take the per-image path, which reports the precise error
-            failed->insert(failed->end(), sub.begin(), sub.end());
-            continue;
-        }
-        sink_encode(X, L, bump, sub, outs[r].d, outs[r].stride, g.ow, g.oh, g.ch, failed);
-    }
-    cudaEventRecord(L.ev[3], L.st);
-    cudaEventSynchronize(L.ev[3]);
-    lane_time(L, 2, 3, &L.ms_encode);
 }
 
 // resize of items [k0, k1) of a task (their frames at d_frames + frame_off[k]) into the task's output area
@@ -598,43 +568,129 @@ static void run_png(lp_xbatch* X, Lane& L, const std::vector<int>& idx) {
     for (int i : failed) push_fallback(X, i);
 }
 
+// ICC profile a WebP source hands to the WebP writer: webp_decoder_get_icc's 32 KiB buffer, then ICCHeaderIsSane
+// (ref color_info.cpp:70-79: a profile whose declared size disagrees with its length is dropped)
+static size_t webp_source_icc(const lp_xbatch* X, int i, const uint8_t** icc) {
+    const WebpPlan& p = *X->items[i].webp;
+    *icc = nullptr;
+    if (p.icc_len < 128 || p.icc_len > 32768) return 0;
+    const uint8_t* q = X->in[i] + p.icc_off;
+    const size_t declared = ((size_t)q[0] << 24) | ((size_t)q[1] << 16) | ((size_t)q[2] << 8) | q[3];
+    if (declared != p.icc_len) return 0;
+    *icc = q;
+    return p.icc_len;
+}
+
+// WebP task: stills and animations of any canvas size, every frame of every file.  Decode + composite is one set of
+// launches over the task (webp_decode_batch: VP8 frames, VP8L / ALPH waves, the per-pixel compositor); a still is one
+// frame copied onto its canvas.  Then one resize per run of equal canvas geometry (its files' canvases lie back to back)
+// and the sinks: JPEG as for every still, WebP as one lossy encode of all the run's frames + the container per file with
+// the source's ICC profile, background, loop count and frame durations (what WebpEncoder::Create / Encode pass on).
 static void run_webp(lp_xbatch* X, Lane& L, const std::vector<int>& idx) {
     const int n = (int)idx.size();
-    const std::vector<Run> runs = runs_of(X, idx);
     Bump bump{L.dev, L.dev_bytes};
-    std::vector<uint64_t> off((size_t)n), frame_off((size_t)n);
-    std::vector<uint32_t> len((size_t)n);
-    std::vector<int> ws((size_t)n), hs((size_t)n);
-    size_t in_bytes = 0, frame_bytes = 0;
+    std::vector<const WebpPlan*> plans((size_t)n);
+    std::vector<const uint8_t*> files((size_t)n);
+    std::vector<size_t> flen((size_t)n);
+    std::vector<uint64_t> canvas_off((size_t)n), out_off((size_t)n);
+    std::vector<int> first((size_t)n + 1, 0);
+    size_t scratch = 4096, arena = 0, canvas_bytes = 0, out_bytes = 0;
     for (int k = 0; k < n; k++) {
-        const XItem& xi = X->items[idx[k]];
-        off[k] = in_bytes;
-        len[k] = (uint32_t)xi.webp.vp8_len;
-        in_bytes += round_up((size_t)len[k] + 64, (size_t)16);
-        frame_off[k] = frame_bytes;
-        frame_bytes += round_up((size_t)xi.w * xi.h * 3, (size_t)256);
-        ws[k] = xi.w;
-        hs[k] = xi.h;
+        const int i = idx[k];
+        const XItem& it = X->items[i];
+        plans[k] = it.webp.get();
+        files[k] = X->in[i];
+        flen[k] = X->in_len[i];
+        scratch += webp_plan_device_bytes(*plans[k], flen[k]);
+        arena += webp_plan_arena_bytes(*plans[k]);
+        const int nf = (int)plans[k]->frames.size();
+        first[k + 1] = first[k] + nf;
+        canvas_off[k] = canvas_bytes;
+        canvas_bytes += (size_t)nf * round_up((size_t)it.w * it.h * it.ch, (size_t)256);
+        out_off[k] = out_bytes;
+        out_bytes += (size_t)nf * round_up((size_t)it.ow * it.oh * it.ch, (size_t)256);
+        L.h2d += flen[k];
     }
-    uint8_t* d_in = bump.take<uint8_t>(in_bytes + 4096);
-    uint8_t* d_frames = bump.take<uint8_t>(frame_bytes + 256);
-    std::vector<int> st((size_t)n, 0), failed;
-    bool ok = d_in && d_frames;
-    for (int k = 0; k < n && ok; k++) {
-        ok = cudaMemcpyAsync(d_in + off[k], X->in[idx[k]] + X->items[idx[k]].webp.vp8_off, len[k], cudaMemcpyHostToDevice,
-                             L.st) == cudaSuccess;
-        L.h2d += len[k];
+    arena = std::min(arena, L.dev_bytes / 4);  // (split_by_memory keeps a quarter of the lane for it)
+    uint8_t* d_scratch = bump.take<uint8_t>(scratch);
+    uint8_t* d_canvases = bump.take<uint8_t>(canvas_bytes + 256);
+    uint8_t* d_out = bump.take<uint8_t>(out_bytes + 256);
+    uint8_t* d_arena = arena ? bump.take<uint8_t>(arena) : nullptr;
+    std::vector<int> st((size_t)n, 0);
+    bool ok = d_scratch && d_canvases && d_out && (!arena || d_arena);
+    if (ok)  // (the decode time starts once the files are on the device, as for the other kinds)
+        ok = webp_decode_batch(plans.data(), files.data(), flen.data(), n, d_scratch, scratch, d_arena, arena, d_canvases,
+                               canvas_off.data(), st.data(), L.ev[0], L.st) == LP_OK;
+    cudaEventRecord(L.ev[1], L.st);
+    const std::vector<Run> runs = runs_of(X, idx);
+    for (size_t r = 0; r < runs.size() && ok; r++) {
+        const XItem& g = X->items[idx[runs[r].k0]];
+        const size_t cs = round_up((size_t)g.w * g.h * g.ch, (size_t)256), os = round_up((size_t)g.ow * g.oh * g.ch, (size_t)256);
+        ResizeArgs a{d_canvases + canvas_off[runs[r].k0], cs, (size_t)g.w * g.ch, g.ch, g.cx, g.cy, g.cw, g.chh,
+                     d_out + out_off[runs[r].k0], os, (size_t)g.ow * g.ch, g.ow, g.oh, first[runs[r].k1] - first[runs[r].k0], 3};
+        ok = resize_launch(a, L.st) == LP_OK;
     }
-    cudaEventRecord(L.ev[0], L.st);
-    if (ok) ok = webp_vp8_decode_batch(d_in, off.data(), len.data(), n, ws.data(), hs.data(), d_frames, frame_off.data(), st.data(), L.st) == LP_OK;
+    cudaEventRecord(L.ev[2], L.st);
+    if (ok) ok = cudaStreamSynchronize(L.st) == cudaSuccess;
     if (!ok) {
         cudaGetLastError();
         for (int i : idx) push_fallback(X, i);
         return;
     }
-    std::vector<char> good((size_t)n);
-    for (int k = 0; k < n; k++) good[k] = st[k] == 0;
-    resize_and_encode(X, L, bump, idx, runs, d_frames, frame_off, good, &failed);
+    lane_time(L, 0, 1, &L.ms_decode);
+    lane_time(L, 1, 2, &L.ms_resize);
+    std::vector<int> failed;
+    cudaEventRecord(L.ev[2], L.st);
+    std::vector<uint8_t> file;
+    for (const Run& r : runs) {
+        const XItem& g = X->items[idx[r.k0]];
+        const size_t os = round_up((size_t)g.ow * g.oh * g.ch, (size_t)256);
+        if (X->sink == S_JPEG) {  // stills only; a file whose frame failed is encoded with its run, then handed over
+            sink_encode(X, L, bump, std::vector<int>(idx.begin() + r.k0, idx.begin() + r.k1), d_out + out_off[r.k0], os, g.ow,
+                        g.oh, g.ch, &failed);
+            for (int k = r.k0; k < r.k1; k++)
+                if (st[k]) failed.push_back(idx[k]);
+            continue;
+        }
+        const int f0 = first[r.k0];
+        std::vector<WebpEncodedFrame> frames;
+        if (webp_encode_lossy_batch(d_out + out_off[r.k0], os, (size_t)g.ow * g.ch, g.ow, g.oh, g.ch, first[r.k1] - f0,
+                                    X->quality, &frames, L.st)) {
+            cudaGetLastError();
+            failed.insert(failed.end(), idx.begin() + r.k0, idx.begin() + r.k1);
+            continue;
+        }
+        for (int k = r.k0; k < r.k1; k++) {
+            const int i = idx[k];
+            const WebpPlan& p = *X->items[i].webp;
+            bool good = st[k] == 0;
+            for (int f = first[k]; f < first[k + 1] && good; f++) good = !frames[f - f0].image.empty();
+            if (!good) {  // a damaged stream or an encoder refusal: the per-image path reports the precise error
+                failed.push_back(i);
+                continue;
+            }
+            for (int f = first[k]; f < first[k + 1]; f++) {
+                frames[f - f0].duration = p.frames[f - first[k]].duration;
+                L.d2h += frames[f - f0].image.size() + frames[f - f0].alph.size();
+            }
+            const uint8_t* icc = nullptr;
+            const size_t icc_len = webp_source_icc(X, i, &icc);
+            webp_assemble(&frames[first[k] - f0], first[k + 1] - first[k], icc, icc_len, p.bgcolor, p.loop_count, &file);
+            if (file.size() > X->out_cap) {  // ref webp.cpp:546-551 -> size 0 -> ErrInvalidImage (webp.go:249-251)
+                X->status[i] = LP_ERR_INVALID_IMAGE;
+                X->out_len[i] = 0;
+                continue;
+            }
+            memcpy(X->out[i], file.data(), file.size());
+            X->out_len[i] = file.size();
+            X->status[i] = LP_OK;
+        }
+    }
+    cudaEventRecord(L.ev[3], L.st);
+    cudaEventSynchronize(L.ev[3]);
+    lane_time(L, 2, 3, &L.ms_encode);
+    std::sort(failed.begin(), failed.end());
+    failed.erase(std::unique(failed.begin(), failed.end()), failed.end());
     for (int i : failed) push_fallback(X, i);
 }
 
@@ -921,8 +977,9 @@ static size_t item_device_bytes(const lp_xbatch* X, const XItem& it, int i) {
             const size_t raw = ((size_t)it.w * (it.ch == 4 ? 4 : 3) + 2) * it.h * (it.png && it.png->interlace ? 2 : 1);
             return 2 * X->in_len[i] + raw + outb + 8192;
         }
-        case K_WEBP:
-            return X->in_len[i] + (size_t)it.w * it.h * 3 + outb + 4096;
+        case K_WEBP:  // the VP8L arena (at most a quarter of the lane) is shared by the task (reserved by split_by_memory)
+            return webp_plan_device_bytes(*it.webp, X->in_len[i]) +
+                   it.webp->frames.size() * (round_up((size_t)it.w * it.h * it.ch, (size_t)256) + outb) + 8192;
         case K_GIF:
             return gif_plan_device_bytes(it.gif) + (size_t)it.gif_frames * ((size_t)it.w * it.h * 4 + outb) + 8192 +
                    (X->sink == S_GIF ? gif_plan_encode_bytes(it.gif, it.ow, it.oh) : 0);
@@ -999,7 +1056,12 @@ extern "C" int lp_xbatch_transform(lp_xbatch* X, const uint8_t* const* in, const
         for (int i : g) total += item_device_bytes(X, X->items[i], i);
         const size_t half = total / 2 + 1;
         Task cur{kind, {}};
-        const size_t reserve = kind == K_PNG ? lane_cap / 5 + (64u << 20) : (64u << 20);  // PNG: the frame window
+        double work = 64u << 20;  // WebP: the order key counts pixels and payload bytes, not the decoders' scratch
+        // PNG: the frame window; WebP: the VP8L / ALPH arena, when some file has lossless frames or alpha planes
+        size_t arena = 0;
+        if (kind == K_WEBP)
+            for (int i : g) arena = std::min(lane_cap / 4, arena + webp_plan_arena_bytes(*X->items[i].webp));
+        const size_t reserve = (kind == K_PNG ? lane_cap / 5 : arena) + (64u << 20);
         size_t used = reserve;
         for (int i : g) {
             const size_t need = item_device_bytes(X, X->items[i], i) +
@@ -1014,16 +1076,22 @@ extern "C" int lp_xbatch_transform(lp_xbatch* X, const uint8_t* const* in, const
             }
             if (!cur.idx.empty() && (used + need > lane_cap || used > half + reserve)) {
                 tasks.push_back(cur);
-                cost.push_back((double)used);
+                cost.push_back(kind == K_WEBP ? work : (double)used);
                 cur.idx.clear();
                 used = reserve;
+                work = 64u << 20;
             }
             cur.idx.push_back(i);
             used += need;
+            if (kind == K_WEBP) {
+                const XItem& it = X->items[i];
+                work += (double)X->in_len[i] + 4096 +
+                        (double)it.webp->frames.size() * ((double)it.w * it.h * it.ch + (double)it.ow * it.oh * 12 + (256u << 10));
+            }
         }
         if (!cur.idx.empty()) {
             tasks.push_back(cur);
-            cost.push_back((double)used);
+            cost.push_back(kind == K_WEBP ? work : (double)used);
         }
     };
     for (auto& kv : merged) split_by_memory((Kind)kv.first, kv.second);
