@@ -44,6 +44,7 @@ struct lp_batch {
     lp_batch_config cfg;
     bool progressive = false;        // JPEG output is progressive (lp_xbatch with JpegProgressive)
     bool multiscan = true;           // takes multi-scan sources (lp_xbatch groups of single-scan files do not)
+    bool resize_only = false;        // lp_xbatch's WebP sink: the chunk ends with the resized frames (no JPEG encode)
     cudaStream_t st = nullptr;       // kernels
     cudaStream_t st_h2d = nullptr;   // input copies (pipelined transform)
     cudaStream_t st_d2h = nullptr;   // output copies (pipelined transform)
@@ -142,16 +143,20 @@ static void batch_free(lp_batch* b) {
 
 namespace lp {
 lp_batch* batch_create_in(const lp_batch_config* cfg, uint8_t* dev_arena, size_t dev_bytes, uint8_t* host_arena,
-                          size_t host_bytes, bool progressive_jpeg = false, bool multiscan_sources = true);
+                          size_t host_bytes, bool progressive_jpeg = false, bool multiscan_sources = true,
+                          bool resize_only = false);
+int batch_resized_status(lp_batch* b, int* status);
 }
 extern "C" lp_batch* lp_batch_create(const lp_batch_config* cfg) { return lp::batch_create_in(cfg, nullptr, 0, nullptr, 0); }
 
 // dev_arena / host_arena non-null: every device / pinned buffer is carved from them (nothing is allocated or
 // freed by the context); returns nullptr when they are too small.  progressive_jpeg: write progressive JPEG files.
 // multiscan_sources: take multi-scan files (and allocate their pools and masks); otherwise they get
-// LP_ERR_UNSUPPORTED.
+// LP_ERR_UNSUPPORTED.  resize_only: every chunk stops after the resize, so the context has no JPEG encoder scratch and
+// no output slots; it is driven by lp_batch_stage + lp_batch_run, then batch_resized_status (lp_batch_transform and
+// lp_batch_fetch refuse it), and the caller encodes the frames at lp_batch_resized_dev.
 lp_batch* lp::batch_create_in(const lp_batch_config* cfg, uint8_t* dev_arena, size_t dev_bytes, uint8_t* host_arena,
-                              size_t host_bytes, bool progressive_jpeg, bool multiscan_sources) {
+                              size_t host_bytes, bool progressive_jpeg, bool multiscan_sources, bool resize_only) {
     if (!cfg || cfg->max_images < 1 || cfg->src_width < 1 || cfg->src_height < 1) return nullptr;
     if (ensure_device()) return nullptr;
     DeviceGuard dev_guard(cfg->device);
@@ -160,6 +165,7 @@ lp_batch* lp::batch_create_in(const lp_batch_config* cfg, uint8_t* dev_arena, si
     b->cfg = *cfg;
     b->progressive = progressive_jpeg;
     b->multiscan = multiscan_sources;
+    b->resize_only = resize_only;
     b->owns_mem = dev_arena == nullptr;
     size_t dev_used = 0, host_used = 0;
     b->W = cfg->src_width;
@@ -231,19 +237,27 @@ lp_batch* lp::batch_create_in(const lp_batch_config* cfg, uint8_t* dev_arena, si
     BALLOC(b->d_coef, (size_t)b->chunk * max_blocks * 64 * sizeof(int16_t));
     BALLOC(b->d_frames, (size_t)b->chunk * b->frame_bytes + 256);
     BALLOC(b->d_resized, N * b->resized_bytes + 256);
-    BALLOC(b->d_enc_scratch, jpeg_encode_scratch_bytes(b->out_w, b->out_h, 3, b->chunk, cfg->out_cap, b->progressive));
+    if (!b->resize_only) {
+        BALLOC(b->d_enc_scratch, jpeg_encode_scratch_bytes(b->out_w, b->out_h, 3, b->chunk, cfg->out_cap, b->progressive));
+    }
     BALLOC(b->d_clean, cfg->max_in_bytes + 64 * N + 4096);
     b->state_cap = (cfg->max_in_bytes / 128 + 2 * N + 16) * 2;
     BALLOC(b->d_states, b->state_cap * 8);
     BALLOC(b->d_nslots, b->state_cap * 4);
     BALLOC(b->d_dcdiff, (size_t)b->chunk * max_blocks * sizeof(int16_t));
-    BALLOC(b->d_out, N * cfg->out_cap);
-    BALLOC(b->d_out_len, N * sizeof(uint32_t));
+    if (!b->resize_only) {
+        BALLOC(b->d_out, N * cfg->out_cap);
+        BALLOC(b->d_out_len, N * sizeof(uint32_t));
+    }
 #undef BALLOC
-    HALLOC(b->h_out, N * cfg->out_cap);
-    HALLOC(b->h_out_len, N * sizeof(uint32_t));
+    if (!b->resize_only) {
+        HALLOC(b->h_out, N * cfg->out_cap);
+        HALLOC(b->h_out_len, N * sizeof(uint32_t));
+    }
     HALLOC(b->h_items_back, N * sizeof(JpegDecodeItem));
-    HALLOC(b->h_off, (N + (size_t)b->max_chunks + 8) * sizeof(unsigned long long));
+    if (!b->resize_only) {
+        HALLOC(b->h_off, (N + (size_t)b->max_chunks + 8) * sizeof(unsigned long long));
+    }
 #undef HALLOC
     b->ev.resize((size_t)b->max_chunks * 6);
     b->ev_h2d.resize(b->max_chunks);
@@ -534,7 +548,7 @@ static int batch_launch_chunk(lp_batch* b, int i0, int cnt, cudaStream_t st, cud
         // there is no geometry to launch with and nothing to decode
         if (ev)
             for (int k = 0; k < 6; k++) LP_CUDA_OK(cudaEventRecord(ev[k], st));
-        LP_CUDA_OK(cudaMemsetAsync(b->d_out_len + i0, 0, (size_t)cnt * sizeof(uint32_t), st));
+        if (!b->resize_only) LP_CUDA_OK(cudaMemsetAsync(b->d_out_len + i0, 0, (size_t)cnt * sizeof(uint32_t), st));
         return LP_OK;
     }
     lp_batch::ChunkLayout none;
@@ -581,6 +595,13 @@ static int batch_launch_chunk(lp_batch* b, int i0, int cnt, cudaStream_t st, cud
     rc = resize_launch(r, st);
     if (rc) return rc;
     if (ev) LP_CUDA_OK(cudaEventRecord(ev[3], st));
+    if (b->resize_only) {  // (the encode stages take no time)
+        if (ev) {
+            LP_CUDA_OK(cudaEventRecord(ev[4], st));
+            LP_CUDA_OK(cudaEventRecord(ev[5], st));
+        }
+        return LP_OK;
+    }
     JpegEncodeBatch e;
     e.frames = r.dst;
     e.frame_img_stride = b->resized_bytes;
@@ -689,7 +710,7 @@ extern "C" int lp_batch_run(lp_batch* b, float* stage_ms) {
 }
 
 extern "C" int lp_batch_fetch(lp_batch* b, uint8_t* const* out, size_t* out_len, int* status) {
-    if (!b || (b->n > 0 && (!out || !out_len))) return LP_ERR_BAD_ARGUMENT;
+    if (!b || b->resize_only || (b->n > 0 && (!out || !out_len))) return LP_ERR_BAD_ARGUMENT;
     DeviceGuard dev_guard(b->cfg.device);
     if (!dev_guard.ok) return LP_ERR_CUDA;
     if (b->n == 0) return LP_OK;
@@ -706,7 +727,7 @@ extern "C" int lp_batch_fetch(lp_batch* b, uint8_t* const* out, size_t* out_len,
 // and chunk c-1's encoded bytes come back.
 extern "C" int lp_batch_transform(lp_batch* b, const uint8_t* const* in, const size_t* in_len, int n,
                                   uint8_t* const* out, size_t* out_len, int* status) {
-    if (!b || n < 0 || n > b->cfg.max_images || (n > 0 && (!in || !in_len || !out || !out_len)))
+    if (!b || b->resize_only || n < 0 || n > b->cfg.max_images || (n > 0 && (!in || !in_len || !out || !out_len)))
         return LP_ERR_BAD_ARGUMENT;
     DeviceGuard dev_guard(b->cfg.device);
     if (!dev_guard.ok) return LP_ERR_CUDA;
@@ -770,6 +791,22 @@ extern "C" int lp_batch_transform(lp_batch* b, const uint8_t* const* in, const s
         batch_finish_chunk(b, sched[finished].first, sched[finished].second, out, out_len, status);
     }
     b->last_launches = (int)(g_launches - launches0);
+    return LP_OK;
+}
+
+// A resize-only context after lp_batch_stage + lp_batch_run: the status of every image (its parse error, or
+// LP_ERR_DECODING_FAILED when the device decode refused it); the frames of the LP_OK ones are at lp_batch_resized_dev.
+int lp::batch_resized_status(lp_batch* b, int* status) {
+    if (!b || !b->resize_only) return LP_ERR_BAD_ARGUMENT;
+    DeviceGuard dev_guard(b->cfg.device);
+    if (!dev_guard.ok) return LP_ERR_CUDA;
+    if (b->n == 0) return LP_OK;
+    LP_CUDA_OK(cudaMemcpyAsync(b->h_items_back, b->d_items, (size_t)b->n * sizeof(JpegDecodeItem), cudaMemcpyDeviceToHost, b->st));
+    LP_CUDA_OK(cudaStreamSynchronize(b->st));
+    for (int i = 0; i < b->n; i++) {
+        status[i] = b->parse_status[i];
+        if (!status[i] && b->h_items_back[i].status != 0) status[i] = LP_ERR_DECODING_FAILED;
+    }
     return LP_OK;
 }
 

@@ -223,6 +223,8 @@ struct WebpEncodedFrame {
 // frames with transparency), ref webp.cpp:711-729 / 650-700 per frame.
 int webp_encode_lossy_batch(const uint8_t* d_frames, size_t img_stride, size_t row_step, int width, int height,
                             int channels, int n, int quality, std::vector<WebpEncodedFrame>* out, cudaStream_t st);
+// Device bytes webp_encode_lossy_batch allocates for n frames of one geometry (its scratch, outside any arena)
+size_t webp_encode_lossy_scratch_bytes(int width, int height, int channels, int n);
 void webp_assemble(const WebpEncodedFrame* frames, int n, const uint8_t* icc, size_t icc_len, uint32_t bgcolor,
                    uint32_t loop_count, std::vector<uint8_t>* file);
 

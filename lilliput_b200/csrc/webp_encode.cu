@@ -756,22 +756,19 @@ __global__ void __launch_bounds__(kPackThreads)
     if (threadIdx.x == 0) total_bits[f] = base;
 }
 
-// `too_large[i]` = 1 when frame i failed only because its first partition outgrew the format's limit
-static int lossy_batch(const uint8_t* d_frames, size_t img_stride, size_t row_step, int width, int height, int channels,
-                       int n, int quality, int try_i4, std::vector<WebpEncodedFrame>* out, std::vector<uint8_t>* too_large,
-                       cudaStream_t st) {
-    out->assign((size_t)n, WebpEncodedFrame());
-    too_large->assign((size_t)n, 0);
-    if (n <= 0) return LP_OK;
-    if (width > 16383 || height > 16383 || (channels != 3 && channels != 4)) return LP_ERR_INVALID_IMAGE;
-    Vp8EncBatch b;
+// The one scratch allocation of a batch: frame regions, output slots, then the length and alpha arrays
+struct LossyLayout {
+    size_t lens_b, aplane_b, hist_b, tables_b, aout_b, alph_words, total;
+};
+
+// Geometry, per-frame scratch layout and output slot of a batch of n frames (b->P's size fields, the offsets, stride,
+// out_cap), and the sizes of the allocation lossy_batch makes for them
+static LossyLayout lossy_layout(int width, int height, int channels, int n, Vp8EncBatch* out) {
+    Vp8EncBatch& b = *out;
     b.P.width = width;
     b.P.height = height;
     b.P.mb_w = (width + 15) >> 4;
     b.P.mb_h = (height + 15) >> 4;
-    b.P.q = vp8enc::quality_to_q(quality);
-    b.P.filter_level = -1;
-    b.P.try_i4 = try_i4;
     b.n = n;
     const int ys = b.P.mb_w * 16, yh = b.P.mb_h * 16;
     const size_t ypl = (size_t)ys * yh, nmb = (size_t)b.P.mb_w * b.P.mb_h;
@@ -793,14 +790,41 @@ static int lossy_batch(const uint8_t* d_frames, size_t img_stride, size_t row_st
     b.out_cap = round_up((size_t)16 + b.part0_cap + b.tokens_cap, (size_t)256);
     const bool alpha = channels == 4;
     const size_t npix = (size_t)width * height;
-    const size_t alph_words = (npix * 2 + 4096 + 3) / 4;  // one <=15-bit green code per pixel + the head
+    LossyLayout L;
+    L.alph_words = (npix * 2 + 4096 + 3) / 4;  // one <=15-bit green code per pixel + the head
+    L.lens_b = round_up((size_t)n * 4, (size_t)256);
+    L.aplane_b = alpha ? round_up((size_t)n * npix, (size_t)256) : 0;
+    L.hist_b = alpha ? round_up((size_t)n * 1024 * 4, (size_t)256) : 0;
+    L.tables_b = alpha ? round_up((size_t)n * sizeof(vp8lenc::CodeTable), (size_t)256) : 0;
+    L.aout_b = alpha ? round_up((size_t)n * L.alph_words * 4, (size_t)256) : 0;
+    L.total = (size_t)n * b.stride + (size_t)n * b.out_cap + 4 * L.lens_b + L.aplane_b + L.hist_b + L.tables_b + L.aout_b;
+    return L;
+}
+
+size_t webp_encode_lossy_scratch_bytes(int width, int height, int channels, int n) {
+    Vp8EncBatch b{};
+    return lossy_layout(width, height, channels, n, &b).total;
+}
+
+// `too_large[i]` = 1 when frame i failed only because its first partition outgrew the format's limit
+static int lossy_batch(const uint8_t* d_frames, size_t img_stride, size_t row_step, int width, int height, int channels,
+                       int n, int quality, int try_i4, std::vector<WebpEncodedFrame>* out, std::vector<uint8_t>* too_large,
+                       cudaStream_t st) {
+    out->assign((size_t)n, WebpEncodedFrame());
+    too_large->assign((size_t)n, 0);
+    if (n <= 0) return LP_OK;
+    if (width > 16383 || height > 16383 || (channels != 3 && channels != 4)) return LP_ERR_INVALID_IMAGE;
+    Vp8EncBatch b;
+    const LossyLayout lay = lossy_layout(width, height, channels, n, &b);
+    b.P.q = vp8enc::quality_to_q(quality);
+    b.P.filter_level = -1;
+    b.P.try_i4 = try_i4;
+    const int ys = b.P.mb_w * 16, yh = b.P.mb_h * 16;
+    const bool alpha = channels == 4;
+    const size_t npix = (size_t)width * height;
+    const size_t alph_words = lay.alph_words, lens_b = lay.lens_b, aplane_b = lay.aplane_b, hist_b = lay.hist_b,
+                 tables_b = lay.tables_b, total = lay.total;
     uint8_t* scratch = nullptr;
-    const size_t lens_b = round_up((size_t)n * 4, (size_t)256);
-    const size_t aplane_b = alpha ? round_up((size_t)n * npix, (size_t)256) : 0;
-    const size_t hist_b = alpha ? round_up((size_t)n * 1024 * 4, (size_t)256) : 0;
-    const size_t tables_b = alpha ? round_up((size_t)n * sizeof(vp8lenc::CodeTable), (size_t)256) : 0;
-    const size_t aout_b = alpha ? round_up((size_t)n * alph_words * 4, (size_t)256) : 0;
-    const size_t total = (size_t)n * b.stride + (size_t)n * b.out_cap + 4 * lens_b + aplane_b + hist_b + tables_b + aout_b;
     if (cudaMallocAsync(&scratch, total, st) != cudaSuccess) {
         fprintf(stderr, "[lilliput_b200] webp_encode_lossy_batch: cudaMallocAsync(%zu) failed\n", total);
         cudaGetLastError();

@@ -143,6 +143,11 @@ Error NewDecoder(const uint8_t* buf, size_t len, std::unique_ptr<Decoder>* out);
 Error NewEncoder(const std::string& ext, Decoder* decodedBy, uint8_t* dst, size_t dst_cap,
                  std::unique_ptr<Encoder>* out);
 
+// ICCHeaderIsSane (ref color_info.cpp:70-79): the WebP writer carries a profile only when it is at least a header
+// (128 B) long and its big-endian size field equals its length; any other profile is dropped and the output written
+// untagged (ref webp.go:190-197)
+bool iccHeaderIsSane(const uint8_t* icc, size_t len);
+
 // ref ops.go:243-255
 void calculateExpectedSize(int origW, int origH, int reqW, int reqH, int* w, int* h);
 // ref opencv.go:331-363 (the crop rectangle Fit hands to opencv_mat_crop)
