@@ -208,6 +208,8 @@ const uint8_t* lp_batch_resized_dev(const lp_batch* b, size_t* image_stride);
 
 /* ---- heterogeneous batch: any supported formats and sizes, one set of options ----------------
  * (BASELINE configs 3, 4, 5: PNG -> WebP, animated GIF -> animated WebP, mixed JPEG / PNG / WebP -> JPEG.)
+ * Sinks with a grid path: ".jpeg", lossy ".webp", ".gif" (from GIF sources) and ".png" (from JPEG, PNG and WebP
+ * stills; RGBA sources keep their alpha).
  * Per-item semantics, status and bytes are those of lp_transform(in[i], ..., opt, out[i], out_cap, ...).
  * Items are grouped by decoder and source geometry and every stage of a group is one grid launch
  * (csrc/xbatch.cu); whatever the grid path does not cover runs through lp_transform inside the call. */
@@ -262,6 +264,16 @@ int lp_resize_area_dev(const uint8_t* src, size_t src_image_stride, size_t src_r
 int lp_jpeg_encode_dev(const uint8_t* frames, size_t frame_img_stride, size_t frame_row_stride,
                        int width, int height, int channels, int quality, int n, uint8_t* out,
                        size_t out_cap, uint32_t* out_len, void* stream);
+
+/* Batched PNG encode of `n` packed device frames of one geometry (BGR / BGRA / Gray) into device memory, as lp_xbatch's
+ * ".png" sink runs it: file i, complete (signature to IEND), at d_files + i*slot; d_len[i] = 0 when it did not fit.
+ * level: zlib level 0..9; adaptive != 0: libpng's adaptive filter choice, else Sub on every row. */
+int lp_png_encode_batch_dev(const uint8_t* d_frames, size_t img_stride, size_t row_stride, int width, int height,
+                            int channels, int n, int level, int adaptive, uint8_t* d_files, size_t slot,
+                            uint32_t* d_len);
+/* CRC-32 and Adler-32 of `n` bytes of device memory by the PNG encoder's device arithmetic (a warp per 32 KB piece,
+ * pieces folded by the rules of csrc/crc32_core.h): for tests against zlib. */
+int lp_png_checksums_dev(const uint8_t* d_data, size_t n, uint32_t* crc32, uint32_t* adler32);
 
 /* Library-owned device/pinned memory helpers so tests and bench need no torch. */
 void* lp_dev_alloc(size_t bytes);

@@ -806,15 +806,9 @@ bool opencv_encoder_write(opencv_encoder e, const opencv_mat src, const int* opt
     Mat* s = static_cast<Mat*>(src);
     if (!enc || !s) return false;
     if (enc->ext == ".png") {
-        // OpenCV: IMWRITE_PNG_COMPRESSION given -> that zlib level with libpng's adaptive filters;
-        // absent -> Z_BEST_SPEED + FILTER_SUB (grfmt_png.cpp)
-        int level = 1;
-        bool adaptive = false;
-        for (size_t i = 0; i + 1 < opt_len; i += 2)
-            if (opt[i] == CV_IMWRITE_PNG_COMPRESSION) {
-                level = std::min(std::max(opt[i + 1], 0), 9);
-                adaptive = true;
-            }
+        int level;
+        bool adaptive;
+        png_encode_policy(opt, opt_len, &level, &adaptive);
         if (ensure_dev(s)) return false;
         std::vector<uint8_t> file;
         if (png_encode_frame(s->dptr(), s->dev_step, s->cols, s->rows, s->channels(), level, adaptive, &file,

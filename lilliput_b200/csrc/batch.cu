@@ -44,7 +44,8 @@ struct lp_batch {
     lp_batch_config cfg;
     bool progressive = false;        // JPEG output is progressive (lp_xbatch with JpegProgressive)
     bool multiscan = true;           // takes multi-scan sources (lp_xbatch groups of single-scan files do not)
-    bool resize_only = false;        // lp_xbatch's WebP sink: the chunk ends with the resized frames (no JPEG encode)
+    bool resize_only = false;        // lp_xbatch's WebP and PNG sinks: the chunk ends with the resized frames (no JPEG encode)
+    size_t arena_dev_used = 0, arena_host_used = 0;  // bytes carved from the caller's arenas (batch_create_in)
     cudaStream_t st = nullptr;       // kernels
     cudaStream_t st_h2d = nullptr;   // input copies (pipelined transform)
     cudaStream_t st_d2h = nullptr;   // output copies (pipelined transform)
@@ -146,6 +147,7 @@ lp_batch* batch_create_in(const lp_batch_config* cfg, uint8_t* dev_arena, size_t
                           size_t host_bytes, bool progressive_jpeg = false, bool multiscan_sources = true,
                           bool resize_only = false);
 int batch_resized_status(lp_batch* b, int* status);
+void batch_arena_used(const lp_batch* b, size_t* dev_bytes, size_t* host_bytes);
 }
 extern "C" lp_batch* lp_batch_create(const lp_batch_config* cfg) { return lp::batch_create_in(cfg, nullptr, 0, nullptr, 0); }
 
@@ -271,7 +273,15 @@ lp_batch* lp::batch_create_in(const lp_batch_config* cfg, uint8_t* dev_arena, si
     b->items.resize(N);
     b->parse_status.resize(N);
     b->file_dev_off.resize(N);
+    b->arena_dev_used = dev_used;
+    b->arena_host_used = host_used;
     return b;
+}
+
+// What a context made by batch_create_in took from the front of the caller's arenas: the rest is the caller's.
+void lp::batch_arena_used(const lp_batch* b, size_t* dev_bytes, size_t* host_bytes) {
+    *dev_bytes = b->arena_dev_used;
+    *host_bytes = b->arena_host_used;
 }
 
 extern "C" void lp_batch_destroy(lp_batch* b) {

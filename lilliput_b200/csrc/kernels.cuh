@@ -190,7 +190,20 @@ int png_inflate_launch(const PngDecodeBatch& b, cudaStream_t st);
 int png_unfilter_launch(const PngDecodeBatch& b, int first, int count, cudaStream_t st);
 
 // ---- png_encode.cu ---------------------------------------------------------------------------
-// One packed device frame -> a complete PNG file in host memory (filter + deflate on the device).
+// zlib level and filter policy of a PNG file from OpenCV's flat encode options (key, value, ...): PngCompression given ->
+// that level clamped to 0..9 with libpng's adaptive filters; absent -> level 1, Sub on every row (grfmt_png.cpp).
+void png_encode_policy(const int* opt, size_t opt_len, int* level, bool* adaptive_filters);
+// The largest file a frame can become (every DEFLATE chunk stored): a slot of this size always fits.
+size_t png_encode_max_file_bytes(int width, int height, int channels);
+// n packed device frames of one geometry (frame i at d_frames + i * img_stride) -> n complete PNG files on the device:
+// file i at d_files + i * slot, d_len[i] its length, 0 when it does not fit `slot`.  Filter, DEFLATE, Adler-32, the
+// chunk CRCs and the container are all written by the three kernels; `scratch` (device, png_encode_batch_scratch_bytes)
+// is the caller's, so nothing is allocated here.
+size_t png_encode_batch_scratch_bytes(int width, int height, int channels, int n, int level);
+int png_encode_batch(const uint8_t* d_frames, size_t img_stride, size_t row_stride, int width, int height, int channels,
+                     int n, int level, bool adaptive_filters, uint8_t* d_files, size_t slot, uint32_t* d_len, void* scratch,
+                     cudaStream_t st);
+// One packed device frame -> a complete PNG file in host memory: png_encode_batch with n = 1.
 int png_encode_frame(const uint8_t* frame, size_t row_stride, int width, int height, int channels, int level,
                      bool adaptive_filters, std::vector<uint8_t>* out, cudaStream_t st);
 

@@ -9,8 +9,8 @@
 //      (ref ops.go:243-255, opencv.go:331-363), so every stage of a group is ONE launch over all its images:
 //        JPEG  -> the lp_batch pipeline (batch.cu): parallel Huffman, IDCT, colour, resize, encode; multi-scan
 //                 (progressive) files form groups of their own, so a chunk of baseline files never waits for the
-//                 serial decode of a large progressive one.  To WebP the pipeline stops after the resize and the
-//                 group's frames go to the lossy WebP encoder
+//                 serial decode of a large progressive one.  To WebP or PNG the pipeline stops after the resize and the
+//                 group's frames go to that sink's encoder
 //        PNG   -> IDAT gather + warp-parallel inflate + defilter + convert (png_decode.cu), resize
 //        WebP  -> stills and animations: VP8 frames one per warp, VP8L / ALPH streams one per warp in arena-sized waves,
 //                 a per-pixel compositor over every file's frame sequence (webp_decode.cu), resize of every canvas
@@ -18,9 +18,10 @@
 //                 frame sequence (gif_decode.cu), resize of every composited canvas
 //      and the sinks: JPEG (jpeg_encode.cu), lossy WebP still / animation (webp_encode.cu) carrying the ICC profile of
 //      a JPEG, PNG or WebP source as WebpEncoder does, GIF from GIF sources (palette mapping + LZW of every frame of the
-//      task, gif_decode.cu; the container assembled on the host);
+//      task, gif_decode.cu; the container assembled on the host), PNG from JPEG, PNG and WebP stills (filter, DEFLATE,
+//      checksums and container of every frame of a run in three launches, png_encode.cu);
 //   3. anything the grid path does not cover (gray or over-budget multi-scan JPEGs, EXIF-rotated sources, lossless WebP
-//      output, PNG output, GIF output from other formats ...) and any item whose grid stage fails goes through
+//      output, PNG output of animations, GIF output from other formats ...) and any item whose grid stage fails goes through
 //      lp_transform on a worker thread -- still this library's device kernels, one image per call -- so the
 //      status and bytes of EVERY item are what lp_transform would have returned.
 // Two worker lanes, each with half of the device arena and its own stream, process chunks of groups
@@ -50,12 +51,13 @@ lp_batch* batch_create_in(const lp_batch_config* cfg, uint8_t* dev_arena, size_t
                           size_t host_bytes, bool progressive_jpeg, bool multiscan_sources, bool resize_only);
 int batch_resized_status(lp_batch* b, int* status);
 size_t batch_multiscan_pool_bytes(size_t n);
+void batch_arena_used(const lp_batch* b, size_t* dev_bytes, size_t* host_bytes);
 }  // namespace lp
 
 namespace {
 
 enum Kind { K_FALLBACK = 0, K_JPEG = 1, K_PNG = 2, K_WEBP = 3, K_GIF = 4 };
-enum Sink { S_NONE = 0, S_JPEG = 1, S_WEBP = 2, S_GIF = 3 };
+enum Sink { S_NONE = 0, S_JPEG = 1, S_WEBP = 2, S_GIF = 3, S_PNG = 4 };
 
 struct XItem {
     Kind kind = K_FALLBACK;
@@ -125,6 +127,8 @@ struct lp_xbatch {
     Sink sink = S_NONE;
     int quality = 0;
     bool progressive = false;  // S_JPEG: progressive files (JpegProgressive)
+    int png_level = 1;         // S_PNG: zlib level and filter policy (png_encode_policy)
+    bool png_adaptive = false;
     std::vector<XItem> items;
     std::vector<int> fallback;
     std::mutex fb_mu;
@@ -178,11 +182,15 @@ static void parse_item(lp_xbatch* X, int i) {
     it.kind = K_FALLBACK;
     it.icc.clear();
     if (!d || n < 16 || X->sink == S_NONE) return;
+    // To PNG every still is one frame in, the file out of the first Encode call: MaxEncodeFrames, DisableAnimatedOutput
+    // and the deadline are never consulted.  A negative MaxEncodeDuration is exceeded before the frame is encoded, and
+    // Transform then asks the decoder to skip to the end, which no still decoder can (ErrSkipNotSupported): per image.
+    if (X->sink == S_PNG && X->opt.max_encode_duration_ns < 0) return;
     const int max_side = X->cfg.max_size > 0 ? X->cfg.max_size : 8192;
     static const uint8_t png_sig[8] = {0x89, 0x50, 0x4E, 0x47, 0x0D, 0x0A, 0x1A, 0x0A};
     thread_local std::vector<uint8_t> icc_buf(32768);
     if (d[0] == 0xFF && d[1] == 0xD8) {
-        if (X->sink != S_JPEG && X->sink != S_WEBP) return;
+        if (X->sink != S_JPEG && X->sink != S_WEBP && X->sink != S_PNG) return;
         // A still to WebP: after its frame Transform checks its deadline (a zero budget fails with ErrEncodeTimeout),
         // MaxEncodeFrames == 1 asks the decoder to skip to the end (a JPEG cannot: ErrSkipNotSupported), and a negative
         // MaxEncodeDuration is exceeded at once (the same skip).  Those go per image.
@@ -258,6 +266,9 @@ static void parse_item(lp_xbatch* X, int i) {
             // simple lossy stills the grid has always taken keep going there; the others stay with lp_transform
             const bool simple = !f0.lossless && !f0.has_alph && !p->icc_len && !p->animated && p->channels == 3;
             if (X->sink == S_WEBP && X->opt.encode_timeout_ns <= 0 && !simple) return;
+            // to PNG under MaxEncodeDuration: a WebP still's frame carries a duration, which Transform holds against the
+            // limit before it encodes the frame; lp_transform decides
+            if (X->sink == S_PNG && X->opt.max_encode_duration_ns != 0) return;
             f0.blend = 1;  // copied onto a canvas of its own size, never disposed
             f0.dispose = 0;
         } else {
@@ -304,10 +315,101 @@ static void parse_item(lp_xbatch* X, int i) {
 
 // ------------------------------------------------------------------ sinks
 
-// resized frames (n x ow x oh x ch, `stride` apart) -> encoded files in the callers' buffers
-static void sink_encode(lp_xbatch* X, Lane& L, Bump& bump, const std::vector<int>& idx, const uint8_t* d_frames,
-                        size_t stride, int ow, int oh, int ch, std::vector<int>* failed) {
+// The PNG sink's file slot for a frame of ow x oh x ch: the largest file it can become, capped by the callers' buffers
+// (a longer file is lp_transform's to refuse).
+static size_t png_sink_slot(const lp_xbatch* X, int ow, int oh, int ch) {
+    return round_up(std::min(X->out_cap, png_encode_max_file_bytes(ow, oh, ch)), (size_t)256);
+}
+// Device bytes the PNG sink takes from a lane's arena per frame: encoder scratch, the slot, its place in the packed copy.
+static size_t png_sink_item_bytes(const lp_xbatch* X, int ow, int oh, int ch) {
+    return round_up(png_encode_batch_scratch_bytes(ow, oh, ch, 1, X->png_level), (size_t)256) + 2 * png_sink_slot(X, ow, oh, ch) + 64;
+}
+
+// n encoded files in device slots (`slot` apart, d_len[k] = 0: did not fit) -> packed back to back, one D2H of lengths
+// and offsets, one D2H of the packed files into the pinned staging area
+static int slots_to_host(Lane& L, uint8_t* h_stage, size_t h_stage_bytes, const uint8_t* d_out, size_t slot, const uint32_t* d_len,
+                         int n, uint8_t* d_packed, unsigned long long* d_off, std::vector<unsigned long long>* off,
+                         std::vector<uint32_t>* len) {
+    int rc = compact_launch(d_out, slot, d_len, (uint32_t)slot, n, d_packed, d_off, L.st);
+    off->assign((size_t)n + 1, 0);
+    len->assign((size_t)n, 0);
+    if (!rc && (cudaMemcpyAsync(off->data(), d_off, (size_t)(n + 1) * 8, cudaMemcpyDeviceToHost, L.st) != cudaSuccess ||
+                cudaMemcpyAsync(len->data(), d_len, (size_t)n * 4, cudaMemcpyDeviceToHost, L.st) != cudaSuccess ||
+                cudaStreamSynchronize(L.st) != cudaSuccess))
+        rc = LP_ERR_CUDA;
+    const size_t total = rc ? 0 : (size_t)(*off)[n];
+    if (!rc && total > h_stage_bytes) rc = LP_ERR_CUDA;
+    if (!rc && total &&
+        (cudaMemcpyAsync(h_stage, d_packed, total, cudaMemcpyDeviceToHost, L.st) != cudaSuccess ||
+         cudaStreamSynchronize(L.st) != cudaSuccess))
+        rc = LP_ERR_CUDA;
+    if (!rc) L.d2h += total + (size_t)n * 12;
+    return rc;
+}
+
+// the staged files into the callers' buffers; one that did not fit its slot or the caller's buffer: let Transform decide
+static void deliver_staged(lp_xbatch* X, const uint8_t* h_stage, const int* idx, int n, const std::vector<unsigned long long>& off,
+                           const std::vector<uint32_t>& len, size_t slot, std::vector<int>* failed) {
+    for (int k = 0; k < n; k++) {
+        const int i = idx[k];
+        if (len[k] == 0 || len[k] > slot || len[k] > X->out_cap) {
+            failed->push_back(i);
+            continue;
+        }
+        memcpy(X->out[i], h_stage + off[k], len[k]);
+        X->out_len[i] = len[k];
+        X->status[i] = LP_OK;
+    }
+}
+
+// PNG sink: every frame of the run through png_encode_batch (whole files in device slots), packed and copied home.  A
+// run whose slots and scratch do not fit what is left of the arena, or whose files may not fit the staging area, is
+// encoded in parts.
+static void png_sink(lp_xbatch* X, Lane& L, Bump& bump, uint8_t* h_stage, size_t h_stage_bytes, const std::vector<int>& idx,
+                     const uint8_t* d_frames, size_t stride, int ow, int oh, int ch, std::vector<int>* failed) {
     const int n = (int)idx.size();
+    const size_t slot = png_sink_slot(X, ow, oh, ch), per = png_sink_item_bytes(X, ow, oh, ch);
+    const size_t mark = bump.used, room = bump.cap - bump.used;
+    const size_t fixed = 4096;  // lengths, offsets and the arena's alignment
+    const int part = (int)std::min<size_t>((size_t)n, std::min(room > fixed ? (room - fixed) / (per + 16) : 0, h_stage_bytes / (slot + 16)));
+    if (part < 1) {
+        failed->insert(failed->end(), idx.begin(), idx.end());
+        return;
+    }
+    std::vector<unsigned long long> off;
+    std::vector<uint32_t> len;
+    for (int k0 = 0; k0 < n; k0 += part) {
+        const int m = std::min(part, n - k0);
+        bump.used = mark;  // (the part before this one has been copied home)
+        uint8_t* d_out = bump.take<uint8_t>((size_t)m * slot);
+        uint32_t* d_len = bump.take<uint32_t>((size_t)m * 4);
+        uint8_t* d_packed = bump.take<uint8_t>((size_t)m * slot + 16);
+        auto* d_off = bump.take<unsigned long long>((size_t)(m + 1) * 8);
+        void* scratch = bump.take<uint8_t>(png_encode_batch_scratch_bytes(ow, oh, ch, m, X->png_level));
+        int rc = d_out && d_len && d_packed && d_off && scratch ? LP_OK : LP_ERR_BUF_TOO_SMALL;
+        if (!rc)
+            rc = png_encode_batch(d_frames + (size_t)k0 * stride, stride, (size_t)ow * ch, ow, oh, ch, m, X->png_level, X->png_adaptive,
+                                  d_out, slot, d_len, scratch, L.st);
+        if (!rc) rc = slots_to_host(L, h_stage, h_stage_bytes, d_out, slot, d_len, m, d_packed, d_off, &off, &len);
+        if (rc) {
+            cudaGetLastError();
+            failed->insert(failed->end(), idx.begin() + k0, idx.end());
+            break;
+        }
+        deliver_staged(X, h_stage, idx.data() + k0, m, off, len, slot, failed);
+    }
+    bump.used = mark;
+}
+
+// resized frames (n x ow x oh x ch, `stride` apart) -> encoded files in the callers' buffers.  h_stage: the pinned
+// staging area the JPEG and PNG sinks copy their files through.
+static void sink_encode(lp_xbatch* X, Lane& L, Bump& bump, uint8_t* h_stage, size_t h_stage_bytes, const std::vector<int>& idx,
+                        const uint8_t* d_frames, size_t stride, int ow, int oh, int ch, std::vector<int>* failed) {
+    const int n = (int)idx.size();
+    if (X->sink == S_PNG) {
+        png_sink(X, L, bump, h_stage, h_stage_bytes, idx, d_frames, stride, ow, oh, ch, failed);
+        return;
+    }
     if (X->sink == S_JPEG) {
         const size_t slot = round_up(std::min(X->out_cap, std::max((size_t)65536, (size_t)ow * oh * ch)), (size_t)256);
         uint8_t* d_out = bump.take<uint8_t>((size_t)n * slot);
@@ -336,39 +438,19 @@ static void sink_encode(lp_xbatch* X, Lane& L, Bump& bump, const std::vector<int
         e.scratch = scratch;
         e.progressive = X->progressive;
         int rc = jpeg_encode_launch(e, L.st, nullptr);
-        if (!rc) rc = compact_launch(d_out, slot, d_len, (uint32_t)slot, n, d_packed, d_off, L.st);
-        std::vector<unsigned long long> off((size_t)n + 1);
-        std::vector<uint32_t> len((size_t)n);
-        if (!rc && (cudaMemcpyAsync(off.data(), d_off, (size_t)(n + 1) * 8, cudaMemcpyDeviceToHost, L.st) != cudaSuccess ||
-                    cudaMemcpyAsync(len.data(), d_len, (size_t)n * 4, cudaMemcpyDeviceToHost, L.st) != cudaSuccess ||
-                    cudaStreamSynchronize(L.st) != cudaSuccess))
-            rc = LP_ERR_CUDA;
-        const size_t total = rc ? 0 : (size_t)off[n];
-        if (!rc && total > L.host_bytes) rc = LP_ERR_CUDA;
-        if (!rc && total &&
-            (cudaMemcpyAsync(L.host, d_packed, total, cudaMemcpyDeviceToHost, L.st) != cudaSuccess ||
-             cudaStreamSynchronize(L.st) != cudaSuccess))
-            rc = LP_ERR_CUDA;
+        std::vector<unsigned long long> off;
+        std::vector<uint32_t> len;
+        if (!rc) rc = slots_to_host(L, h_stage, h_stage_bytes, d_out, slot, d_len, n, d_packed, d_off, &off, &len);
         if (rc) {
             cudaGetLastError();
             failed->insert(failed->end(), idx.begin(), idx.end());
             return;
         }
-        L.d2h += total + (size_t)n * 12;
         const auto tq1 = std::chrono::steady_clock::now();
         if (dbg)
             fprintf(stderr, "[lilliput_b200] jpeg sink: n=%d %dx%dx%d slot=%zu total=%zu: launches + D2H %.2f ms\n", n, ow, oh, ch, slot,
-                    total, std::chrono::duration<double, std::milli>(tq1 - tq0).count());
-        for (int k = 0; k < n; k++) {
-            const int i = idx[k];
-            if (len[k] == 0 || len[k] > slot || len[k] > X->out_cap) {  // did not fit the slot: let Transform decide
-                failed->push_back(i);
-                continue;
-            }
-            memcpy(X->out[i], L.host + off[k], len[k]);
-            X->out_len[i] = len[k];
-            X->status[i] = LP_OK;
-        }
+                    (size_t)off[n], std::chrono::duration<double, std::milli>(tq1 - tq0).count());
+        deliver_staged(X, h_stage, idx.data(), n, off, len, slot, failed);
         return;
     }
     // lossy WebP stills, each with its source's ICC profile
@@ -465,7 +547,8 @@ static void encode_runs(lp_xbatch* X, Lane& L, Bump& bump, const std::vector<int
             failed->insert(failed->end(), sub.begin(), sub.end());
             continue;
         }
-        sink_encode(X, L, bump, sub, d_out + out_off[r.k0], round_up((size_t)g.ow * g.oh * g.ch, (size_t)256), g.ow, g.oh, g.ch, failed);
+        sink_encode(X, L, bump, L.host, L.host_bytes, sub, d_out + out_off[r.k0], round_up((size_t)g.ow * g.oh * g.ch, (size_t)256),
+                    g.ow, g.oh, g.ch, failed);
     }
     cudaEventRecord(L.ev[3], L.st);
     cudaEventSynchronize(L.ev[3]);
@@ -599,7 +682,7 @@ static void run_png(lp_xbatch* X, Lane& L, const std::vector<int>& idx) {
 // WebP task: stills and animations of any canvas size, every frame of every file.  Decode + composite is one set of
 // launches over the task (webp_decode_batch: VP8 frames, VP8L / ALPH waves, the per-pixel compositor); a still is one
 // frame copied onto its canvas.  Then one resize per run of equal canvas geometry (its files' canvases lie back to back)
-// and the sinks: JPEG as for every still, WebP as one lossy encode of all the run's frames + the container per file with
+// and the sinks: JPEG and PNG as for every still, WebP as one lossy encode of all the run's frames + the container per file with
 // the source's ICC profile, background, loop count and frame durations (what WebpEncoder::Create / Encode pass on).
 static void run_webp(lp_xbatch* X, Lane& L, const std::vector<int>& idx) {
     const int n = (int)idx.size();
@@ -660,9 +743,9 @@ static void run_webp(lp_xbatch* X, Lane& L, const std::vector<int>& idx) {
     for (const Run& r : runs) {
         const XItem& g = X->items[idx[r.k0]];
         const size_t os = round_up((size_t)g.ow * g.oh * g.ch, (size_t)256);
-        if (X->sink == S_JPEG) {  // stills only; a file whose frame failed is encoded with its run, then handed over
-            sink_encode(X, L, bump, std::vector<int>(idx.begin() + r.k0, idx.begin() + r.k1), d_out + out_off[r.k0], os, g.ow,
-                        g.oh, g.ch, &failed);
+        if (X->sink != S_WEBP) {  // JPEG, PNG: stills only; a file whose frame failed is encoded with its run, then handed over
+            sink_encode(X, L, bump, L.host, L.host_bytes, std::vector<int>(idx.begin() + r.k0, idx.begin() + r.k1),
+                        d_out + out_off[r.k0], os, g.ow, g.oh, g.ch, &failed);
             for (int k = r.k0; k < r.k1; k++)
                 if (st[k]) failed.push_back(idx[k]);
             continue;
@@ -834,15 +917,18 @@ static void run_gif(lp_xbatch* X, Lane& L, const std::vector<int>& idx) {
 
 // ------------------------------------------------------------------ JPEG groups (the lp_batch pipeline)
 
-// Device bytes one encode of a JPEG group's frames may allocate (webp_encode_lossy_batch's scratch lives outside the
+// Device bytes one WebP encode of a JPEG group's frames may allocate (webp_encode_lossy_batch's scratch lives outside the
 // lane's arena): 1 GiB holds 717 frames of 256x256 (1.43 MiB each, webp_encode_lossy_scratch_bytes), and stays below
 // what one encode of a PNG task of bench.py's config 3 takes (6.4 MiB per 512x512 RGBA frame, hundreds of frames).
 static constexpr size_t kJpegWebpScratch = (size_t)1 << 30;
+// Frames of a JPEG group the PNG sink is sure to have arena for (run_jpeg keeps that much out of the decode chunks' reach)
+static constexpr size_t kJpegPngFrames = 512;
 
-// WebP sink: the group through a resize-only lp_batch context (decode + resize of every image, one chunk after
-// another), then the lossy encoder over its resized frames in sub-batches of at most the decode chunk's image count
-// and kJpegWebpScratch of encoder scratch.  Items the decode refused go to the per-image path without being encoded.
-static void jpeg_to_webp(lp_xbatch* X, Lane& L, lp_batch* b, const std::vector<int>& idx, const uint8_t* const* in,
+// WebP and PNG sinks: the group through a resize-only lp_batch context (decode + resize of every image, one chunk after
+// another), then the sink's encoder over its resized frames.  WebP: in sub-batches of at most the decode chunk's image
+// count and kJpegWebpScratch of encoder scratch.  PNG: out of what the context left of the lane's arena and pinned
+// staging.  Items the decode refused go to the per-image path without being encoded.
+static void jpeg_to_sink(lp_xbatch* X, Lane& L, lp_batch* b, const std::vector<int>& idx, const uint8_t* const* in,
                          const size_t* len) {
     const int n = (int)idx.size();
     const XItem& g = X->items[idx[0]];
@@ -858,10 +944,15 @@ static void jpeg_to_webp(lp_xbatch* X, Lane& L, lp_batch* b, const std::vector<i
     L.ms_resize += stage[LP_STAGE_RESIZE];
     size_t stride = 0;
     const uint8_t* d_resized = lp_batch_resized_dev(b, &stride);
-    const size_t per_frame = webp_encode_lossy_scratch_bytes(g.ow, g.oh, 3, 1);
-    const int sub = (int)std::max<size_t>(1, std::min<size_t>((size_t)lp_batch_chunk(b), kJpegWebpScratch / per_frame));
+    int sub = n;
+    if (X->sink == S_WEBP) {
+        const size_t per_frame = webp_encode_lossy_scratch_bytes(g.ow, g.oh, 3, 1);
+        sub = (int)std::max<size_t>(1, std::min<size_t>((size_t)lp_batch_chunk(b), kJpegWebpScratch / per_frame));
+    }
     std::vector<int> failed;
-    Bump unused{nullptr, 0};  // (the WebP branch of sink_encode takes nothing from the lane's arena)
+    size_t dev_used = 0, host_used = 0;
+    batch_arena_used(b, &dev_used, &host_used);
+    Bump bump{L.dev + dev_used, L.dev_bytes - dev_used};  // (the WebP branch of sink_encode takes nothing from it)
     cudaEventRecord(L.ev[2], L.st);
     // runs of decoded items (their frames back to back), at most `sub` long; a refused item goes to the per-image path
     for (int k0 = 0; k0 < n;) {
@@ -871,8 +962,8 @@ static void jpeg_to_webp(lp_xbatch* X, Lane& L, lp_batch* b, const std::vector<i
         }
         int k1 = k0 + 1;
         while (k1 < n && k1 - k0 < sub && st[k1] == LP_OK) k1++;
-        sink_encode(X, L, unused, std::vector<int>(idx.begin() + k0, idx.begin() + k1), d_resized + (size_t)k0 * stride, stride,
-                    g.ow, g.oh, 3, &failed);
+        sink_encode(X, L, bump, L.host + host_used, L.host_bytes - host_used, std::vector<int>(idx.begin() + k0, idx.begin() + k1),
+                    d_resized + (size_t)k0 * stride, stride, g.ow, g.oh, 3, &failed);
         k0 = k1;
     }
     cudaEventRecord(L.ev[3], L.st);
@@ -884,7 +975,7 @@ static void jpeg_to_webp(lp_xbatch* X, Lane& L, lp_batch* b, const std::vector<i
 static void run_jpeg(lp_xbatch* X, Lane& L, const std::vector<int>& idx) {
     const int n = (int)idx.size();
     const XItem& g = X->items[idx[0]];
-    const bool to_webp = X->sink == S_WEBP;
+    const bool resize_only = X->sink != S_JPEG;  // WebP, PNG: the frames go to that sink's encoder
     size_t in_bytes = 0;
     for (int i : idx) in_bytes += X->in_len[i];
     lp_batch_config c;
@@ -906,7 +997,9 @@ static void run_jpeg(lp_xbatch* X, Lane& L, const std::vector<int>& idx) {
     // multi-scan groups: + the nonzero masks per block, + the scan and table-set pools (batch.cu)
     const size_t per_img = (mcus * 3 + 64) * (128 + 64 + 2 + (g.jpeg_multiscan ? 8 : 0)) + (size_t)g.w * g.h * 3 + 65536;
     const size_t pools = g.jpeg_multiscan ? batch_multiscan_pool_bytes((size_t)n) : 0;
-    const size_t fixed = 2 * in_bytes + (size_t)n * ((to_webp ? 0 : c.out_cap) + (size_t)g.ow * g.oh * 3 + 4096) + (64u << 20) + pools;
+    const size_t png_room =
+        X->sink == S_PNG ? std::min(L.dev_bytes / 4, std::min((size_t)n, kJpegPngFrames) * png_sink_item_bytes(X, g.ow, g.oh, 3)) : 0;
+    const size_t fixed = 2 * in_bytes + (size_t)n * ((resize_only ? 0 : c.out_cap) + (size_t)g.ow * g.oh * 3 + 4096) + (64u << 20) + pools + png_room;
     const int slots = jpeg_huff_parallel_slots();
     long fit = L.dev_bytes > fixed ? (long)((L.dev_bytes - fixed) / per_img) : 0;
     if (fit < 1) {
@@ -916,7 +1009,7 @@ static void run_jpeg(lp_xbatch* X, Lane& L, const std::vector<int>& idx) {
     int chunk = (int)std::min<long>(fit, 3L * std::max(slots, 1));
     if (slots > 0 && chunk > slots) chunk = chunk / slots * slots;
     c.chunk = std::max(1, std::min(chunk, n));
-    lp_batch* b = batch_create_in(&c, L.dev, L.dev_bytes, L.host, L.host_bytes, X->progressive, g.jpeg_multiscan, to_webp);
+    lp_batch* b = batch_create_in(&c, L.dev, L.dev_bytes, L.host, L.host_bytes, X->progressive, g.jpeg_multiscan, resize_only);
     if (!b) {
         for (int i : idx) push_fallback(X, i);
         return;
@@ -931,8 +1024,8 @@ static void run_jpeg(lp_xbatch* X, Lane& L, const std::vector<int>& idx) {
         out[k] = X->out[idx[k]];
     }
     L.h2d += in_bytes;
-    if (to_webp) {
-        jpeg_to_webp(X, L, b, idx, in.data(), len.data());
+    if (resize_only) {
+        jpeg_to_sink(X, L, b, idx, in.data(), len.data());
         lp_batch_destroy(b);
         return;
     }
@@ -1036,7 +1129,7 @@ static void parallel_for(int n, int threads, F&& fn) {
 
 // device bytes one item of a group needs inside a lane's arena (upper bound, sinks included)
 static size_t item_device_bytes(const lp_xbatch* X, const XItem& it, int i) {
-    const size_t outb = (size_t)it.ow * it.oh * 4 * 3 + (256u << 10);
+    const size_t outb = (size_t)it.ow * it.oh * 4 * 3 + (256u << 10) + (X->sink == S_PNG ? png_sink_item_bytes(X, it.ow, it.oh, it.ch) : 0);
     switch (it.kind) {
         case K_PNG: {
             // compressed span (+ its gathered copy) + inflated scanlines + resized output; the packed frames live in a
@@ -1098,6 +1191,9 @@ extern "C" int lp_xbatch_transform(lp_xbatch* X, const uint8_t* const* in, const
         X->sink = q > 100 ? S_NONE : S_WEBP;  // lossless output: per image
     } else if (ext == ".gif") {
         X->sink = S_GIF;
+    } else if (ext == ".png") {
+        X->sink = S_PNG;
+        png_encode_policy(opt->encode_options, opt->encode_options_len, &X->png_level, &X->png_adaptive);
     }
     parallel_for(n, X->threads, [&](int i) { parse_item(X, i); });
     const auto t1 = std::chrono::steady_clock::now();
