@@ -153,6 +153,9 @@ typedef struct lp_batch_config {
     size_t max_in_bytes; /* capacity for the sum of compressed input sizes */
     size_t out_cap;      /* per-image output capacity in bytes */
     int chunk;           /* images per pipelined chunk (0 = default) */
+    int normalize_orientation; /* ImageOptions.NormalizeOrientation (0 = false): the size requested of an
+                                  image whose EXIF orientation swaps its axes (5..8) is that of the
+                                  header's size turned, as Transform computes it */
 } lp_batch_config;
 
 lp_batch* lp_batch_create(const lp_batch_config* cfg);
@@ -162,12 +165,15 @@ void lp_batch_destroy(lp_batch* b);
  * (pinned or not); H2D of the compressed bytes and D2H of the encoded bytes are
  * inside the call.  status[i] is an lp_status per image.
  *
- * Sources taken: 8-bit Huffman-coded 3-component JPEGs of the configured size whose
- * EXIF orientation is top-left -- baseline or extended sequential (with or without
- * restart markers and optimised tables), progressive, or sequential with one scan per
- * component.  Each item gets the status and bytes lp_transform gives it, except that
- * gray and EXIF-rotated files, and multi-scan files that overflow the context's scan
- * or Huffman-table pools (sized by max_images, see batch.cu), get LP_ERR_UNSUPPORTED. */
+ * Sources taken: 8-bit Huffman-coded 3-component JPEGs of the configured size, with any
+ * EXIF orientation -- baseline or extended sequential (with or without restart markers
+ * and optimised tables), progressive, or sequential with one scan per component.  The
+ * orientation is applied on the device, per item, as Transform applies it (whether or
+ * not normalize_orientation is set); an orientation that swaps the axes may give an item
+ * another output size than the top-left ones (Fit above the source size, Width != Height).
+ * Each item gets the status and bytes lp_transform gives it, except that gray files, and
+ * multi-scan files that overflow the context's scan or Huffman-table pools (sized by
+ * max_images, see batch.cu), get LP_ERR_UNSUPPORTED. */
 int lp_batch_transform(lp_batch* b, const uint8_t* const* in, const size_t* in_len, int n,
                        uint8_t* const* out, size_t* out_len, int* status);
 
@@ -202,7 +208,8 @@ void lp_batch_sync_rounds(const lp_batch* b, double* mean, int* max);
  * its CTAs -- out8[0] table set-up, [1] guess pass, [2] synchronisation rounds, [3] prefix sum + write pass, [4] DC pass,
  * [5] number of CTAs (= images).  reset != 0 clears the counters after reading.  Returns an lp_status. */
 int lp_huff_phase_clocks(unsigned long long* out8, int reset);
-/* Device pointer to the decoded frames / resized frames of the last run (tests). */
+/* Device pointer to the decoded frames / resized frames of the last run (tests).  Resized frame i is at
+ * i * image_stride, rows packed, in its own output size; decoded windows are slot-strided within the last chunk. */
 const uint8_t* lp_batch_decoded_dev(const lp_batch* b, size_t* image_stride);
 const uint8_t* lp_batch_resized_dev(const lp_batch* b, size_t* image_stride);
 

@@ -63,7 +63,7 @@ class _BatchConfig(C.Structure):
         ("device", C.c_int), ("max_images", C.c_int), ("src_width", C.c_int),
         ("src_height", C.c_int), ("dst_width", C.c_int), ("dst_height", C.c_int),
         ("resize_method", C.c_int), ("jpeg_quality", C.c_int), ("max_in_bytes", C.c_size_t),
-        ("out_cap", C.c_size_t), ("chunk", C.c_int),
+        ("out_cap", C.c_size_t), ("chunk", C.c_int), ("normalize_orientation", C.c_int),
     ]
 
 
@@ -321,7 +321,7 @@ class Batch:
 
     def __init__(self, lib: Lib, device: int, max_images: int, src_w: int, src_h: int, dst_w: int,
                  dst_h: int, quality: int, max_in_bytes: int, out_cap: int = 65536,
-                 resize_method: int = ImageOpsFit, chunk: int = 0):
+                 resize_method: int = ImageOpsFit, chunk: int = 0, normalize_orientation: bool = False):
         self.lib = lib
         l = lib.l
         l.lp_batch_create.restype = C.c_void_p
@@ -347,7 +347,7 @@ class Batch:
         l.lp_memcpy_d2h.restype = C.c_int
         l.lp_memcpy_d2h.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t]
         cfg = _BatchConfig(device, max_images, src_w, src_h, dst_w, dst_h, resize_method, quality,
-                           max_in_bytes, out_cap, chunk)
+                           max_in_bytes, out_cap, chunk, int(normalize_orientation))
         self.h = l.lp_batch_create(C.byref(cfg))
         if not self.h:
             raise RuntimeError("lp_batch_create failed (no CUDA device / out of memory)")

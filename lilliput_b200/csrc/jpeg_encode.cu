@@ -240,7 +240,7 @@ struct EncGeom {
 // and their DC resolved by the entropy kernel (jccoefct.c dummy-block rule).
 __global__ void __launch_bounds__(128)
     jpeg_fdct_quant_kernel(const uint8_t* frames, size_t img_stride, size_t row_stride, EncGeom g,
-                           const EncConst* ec, int16_t* coef, int n) {
+                           const EncConst* ec, int16_t* coef, int n, const int* index) {
     __shared__ uint16_t sq[2][64];
     __shared__ float sqr[2][64];  // 1 / (8 * Q)
     if (threadIdx.x < 64) {
@@ -278,7 +278,7 @@ __global__ void __launch_bounds__(128)
         }
     }
     const int mx = mcu % g.mcus_x, my = mcu / g.mcus_x;
-    const uint8_t* f = frames + (size_t)img * img_stride;
+    const uint8_t* f = frames + (size_t)(index ? __ldg(index + img) : img) * img_stride;
     int16_t* out = coef + (((size_t)img * nmcu + mcu) * g.blocks_per_mcu + k) * 64;
     int d[64];
     int qsel = 0;
@@ -533,7 +533,7 @@ __device__ __forceinline__ long long stuff_bytes(const uint32_t* words, uint32_t
 __global__ void __launch_bounds__(kEntThreads)
     jpeg_entropy_kernel(const int16_t* coef_all, EncGeom g, const EncConst* ec, uint32_t* mcu_bits_all,
                         uint32_t* words_all, size_t words_per_img, uint8_t* out_all, size_t out_cap,
-                        uint32_t* out_len, int header_len) {
+                        uint32_t* out_len, int header_len, const int* index) {
     __shared__ uint32_t huff[4][256];
     __shared__ uint32_t warp_sums[kEntThreads / 32];
     __shared__ uint32_t s_carry;
@@ -543,7 +543,8 @@ __global__ void __launch_bounds__(kEntThreads)
     const int16_t* coef = coef_all + (size_t)img * nmcu * g.blocks_per_mcu * 64;
     uint32_t* mcu_bits = mcu_bits_all + (size_t)img * nmcu;
     uint32_t* words = words_all + (size_t)img * words_per_img;
-    uint8_t* out = out_all + (size_t)img * out_cap;
+    const int slot = index ? __ldg(index + img) : img;
+    uint8_t* out = out_all + (size_t)slot * out_cap;
     for (int i = tid; i < 1024; i += kEntThreads) huff[i >> 8][i & 255] = ec->huff[i >> 8][i & 255];
     if (tid == 0) s_carry = 0;
     __syncthreads();
@@ -565,7 +566,7 @@ __global__ void __launch_bounds__(kEntThreads)
     const uint32_t nwords = (nbytes + 3) >> 2;
     const size_t room = out_cap > (size_t)header_len + 2 ? out_cap - header_len - 2 : 0;
     if ((size_t)nbytes > room || nwords + 1 > words_per_img) {  // cannot fit even unstuffed
-        if (tid == 0) out_len[img] = 0;
+        if (tid == 0) out_len[slot] = 0;
         return;
     }
     // phase 3: zero the word buffer, then every MCU writes its bits (big-endian bit order)
@@ -637,7 +638,7 @@ __global__ void __launch_bounds__(kEntThreads)
     }
     const int any_overflow = __syncthreads_or(overflow);
     if (any_overflow) {
-        if (tid == 0) out_len[img] = 0;
+        if (tid == 0) out_len[slot] = 0;
         return;
     }
     for (int i = tid; i < header_len; i += kEntThreads) out[i] = ec->header[i];
@@ -645,7 +646,7 @@ __global__ void __launch_bounds__(kEntThreads)
         const size_t end = (size_t)header_len + nbytes + s_carry;
         out[end] = 0xFF;
         out[end + 1] = 0xD9;
-        out_len[img] = (uint32_t)(end + 2);
+        out_len[slot] = (uint32_t)(end + 2);
     }
 }
 
@@ -681,7 +682,7 @@ struct AtomicOrWord {
 __global__ void __launch_bounds__(kEntThreads)
     jpeg_prog_entropy_kernel(const int16_t* coef_all, EncGeom g, const EncConst* ec, uint32_t* summ_all,
                              uint32_t* runs_all, uint32_t* words_all, size_t words_per_img, uint8_t* out_all,
-                             size_t out_cap, uint32_t* out_len) {
+                             size_t out_cap, uint32_t* out_len, const int* index) {
     __shared__ uint32_t hist[2][257];
     __shared__ uint32_t huff[2][256];
     __shared__ int tbl_work[2][257];
@@ -698,10 +699,11 @@ __global__ void __launch_bounds__(kEntThreads)
     uint32_t* summ = summ_all + (size_t)img * nblk;
     uint32_t* runs = runs_all + (size_t)img * nblk;
     uint32_t* words = words_all + (size_t)img * words_per_img;
-    uint8_t* out = out_all + (size_t)img * out_cap;
+    const int slot = index ? __ldg(index + img) : img;
+    uint8_t* out = out_all + (size_t)slot * out_cap;
     const int flen = jprog::frame_len(gray);
     if (out_cap < (size_t)flen + 2) {
-        if (tid == 0) out_len[img] = 0;
+        if (tid == 0) out_len[slot] = 0;
         return;
     }
     const int sof = jprog::sof_type_at(gray);
@@ -748,7 +750,7 @@ __global__ void __launch_bounds__(kEntThreads)
         }
         __syncthreads();
         if (s_fail) {
-            if (tid == 0) out_len[img] = 0;
+            if (tid == 0) out_len[slot] = 0;
             return;
         }
         pos += s_carry;
@@ -772,7 +774,7 @@ __global__ void __launch_bounds__(kEntThreads)
         const uint32_t nwords = (nbytes + 3) >> 2;
         const size_t room = out_cap - pos - 2;
         if ((size_t)nbytes > room || nwords + 1 > words_per_img) {  // cannot fit even unstuffed
-            if (tid == 0) out_len[img] = 0;
+            if (tid == 0) out_len[slot] = 0;
             return;
         }
         for (uint32_t i = tid; i <= nwords; i += kEntThreads) words[i] = 0;
@@ -793,7 +795,7 @@ __global__ void __launch_bounds__(kEntThreads)
         __syncthreads();
         const long long stuffed = stuff_bytes(words, nbytes, out + pos, room, warp_sums, s_carry);
         if (stuffed < 0) {
-            if (tid == 0) out_len[img] = 0;
+            if (tid == 0) out_len[slot] = 0;
             return;
         }
         pos += (size_t)stuffed;
@@ -802,7 +804,7 @@ __global__ void __launch_bounds__(kEntThreads)
     if (tid == 0) {
         out[pos] = 0xFF;
         out[pos + 1] = 0xD9;
-        out_len[img] = (uint32_t)(pos + 2);
+        out_len[slot] = (uint32_t)(pos + 2);
     }
 }
 
@@ -870,7 +872,7 @@ int jpeg_encode_launch(const JpegEncodeBatch& b, cudaStream_t st, cudaEvent_t ev
     // NOTE: coef is laid out densely ([n][nmcu*bpm][64]); coef_bytes padding only sizes the region
     const long total_blocks = (long)nmcu * g.blocks_per_mcu * b.n;
     jpeg_fdct_quant_kernel<<<(unsigned)ceil_div(total_blocks, 128L), 128, 0, st>>>(
-        b.frames, b.frame_img_stride, b.frame_row_stride, g, ec, coef, b.n);
+        b.frames, b.frame_img_stride, b.frame_row_stride, g, ec, coef, b.n, b.index);
     g_launches++;
     LP_CUDA_OK(cudaGetLastError());
     if (ev_after_transform) LP_CUDA_OK(cudaEventRecord(ev_after_transform, st));
@@ -879,10 +881,10 @@ int jpeg_encode_launch(const JpegEncodeBatch& b, cudaStream_t st, cudaEvent_t ev
         uint32_t* summ = reinterpret_cast<uint32_t*>(s + (size_t)b.n * (coef_bytes + bits_bytes + words_bytes));
         uint32_t* runs = summ + (size_t)b.n * prog_block_bytes(g) / sizeof(uint32_t);
         jpeg_prog_entropy_kernel<<<b.n, kEntThreads, 0, st>>>(coef, g, ec, summ, runs, words, wpi, b.out, b.out_cap,
-                                                             b.out_len);
+                                                             b.out_len, b.index);
     } else {
         jpeg_entropy_kernel<<<b.n, kEntThreads, 0, st>>>(coef, g, ec, mcu_bits, words, wpi, b.out, b.out_cap,
-                                                        b.out_len, header_len);
+                                                        b.out_len, header_len, b.index);
     }
     g_launches++;
     LP_CUDA_OK(cudaGetLastError());

@@ -22,6 +22,9 @@ struct ResizeArgs {
     int dst_w, dst_h;
     int n;
     int interpolation;  // 1 = INTER_LINEAR, 2 = INTER_CUBIC, 3 = INTER_AREA
+    // device, n entries, or nullptr: image j of the launch reads src image index[j] and writes dst image index[j]
+    // (INTER_AREA and INTER_LINEAR only)
+    const int* index = nullptr;
 };
 int resize_launch(const ResizeArgs& a, cudaStream_t st);
 
@@ -221,6 +224,8 @@ struct JpegEncodeBatch {
     void* scratch;
     // progressive output (libjpeg-turbo's jpeg_simple_progression script, optimal tables per scan)
     bool progressive = false;
+    // device, n entries, or nullptr: image j of the launch reads frame index[j] and writes out slot / out_len index[j]
+    const int* index = nullptr;
 };
 size_t jpeg_encode_scratch_bytes(int width, int height, int channels, int n, size_t out_cap, bool progressive = false);
 int jpeg_encode_launch(const JpegEncodeBatch& b, cudaStream_t st, cudaEvent_t ev_after_transform);
@@ -296,6 +301,32 @@ int gif_encode_batch(GifAnimPlan* const* plans, int n, const uint8_t* d_frames, 
 // ---- pixel_ops.cu --------------------------------------------------------------------------
 int orient_launch(const uint8_t* src, int w, int h, int channels, int orientation, uint8_t* dst,
                   cudaStream_t st);
+// EXIF orientation o of a w x h frame (golden table SURVEY.md 8a R4; values outside 2..8 are the identity): the source
+// pixel that lands at (x, y) of the oriented frame.
+__host__ __device__ inline void orient_source_pixel(int o, int w, int h, int x, int y, int* sx, int* sy) {
+    switch (o) {
+        case 2: *sx = w - 1 - x; *sy = y; break;
+        case 3: *sx = w - 1 - x; *sy = h - 1 - y; break;
+        case 4: *sx = x; *sy = h - 1 - y; break;
+        case 5: *sx = y; *sy = x; break;
+        case 6: *sx = y; *sy = h - 1 - x; break;
+        case 7: *sx = w - 1 - y; *sy = h - 1 - x; break;
+        case 8: *sx = w - 1 - y; *sy = x; break;
+        default: *sx = x; *sy = y; break;
+    }
+}
+// One item of orient_crop_launch: the crop [cx, cx+cw) x [cy, cy+ch) of the oriented frame, read from a decoded window
+// of the w x h source (window origin win_x0, win_y0; rows src_stride bytes apart, starting at src_off) and written
+// packed BGR (rows cw * 3 bytes apart) at dst_off.
+struct OrientJob {
+    uint64_t src_off, dst_off;
+    uint32_t src_stride;
+    int32_t o, cx, cy, cw, ch, win_x0, win_y0;
+};
+// n jobs on 3-channel frames of one w x h source; max_cw / max_ch bound every job's crop.  32 x 32 tiles staged in
+// shared memory, so the transposing orientations read and write whole rows too.
+int orient_crop_launch(const OrientJob* d_jobs, int n, const uint8_t* src, uint8_t* dst, int w, int h, int max_cw,
+                       int max_ch, cudaStream_t st);
 int copy_region_launch(const uint8_t* src, size_t src_step, int src_ch, uint8_t* dst,
                        size_t dst_step, int dst_ch, int w, int h, cudaStream_t st);
 // ---- tonemap.cu ----------------------------------------------------------------------------

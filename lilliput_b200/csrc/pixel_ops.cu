@@ -18,16 +18,7 @@ __global__ void orient_kernel(const uint8_t* __restrict__ src, int w, int h, int
     const int y = blockIdx.y;
     if (x >= W || y >= H) return;
     int sx, sy;
-    switch (o) {
-        case 2: sx = w - 1 - x; sy = y; break;
-        case 3: sx = w - 1 - x; sy = h - 1 - y; break;
-        case 4: sx = x; sy = h - 1 - y; break;
-        case 5: sx = y; sy = x; break;
-        case 6: sx = y; sy = h - 1 - x; break;
-        case 7: sx = w - 1 - y; sy = h - 1 - x; break;
-        case 8: sx = w - 1 - y; sy = x; break;
-        default: sx = x; sy = y; break;
-    }
+    orient_source_pixel(o, w, h, x, y, &sx, &sy);
     const uint8_t* s = src + ((size_t)sy * w + sx) * C;
     uint8_t* d = dst + ((size_t)y * W + x) * C;
     for (int c = 0; c < C; c++) d[c] = s[c];
@@ -40,6 +31,56 @@ int orient_launch(const uint8_t* src, int w, int h, int C, int o, uint8_t* dst, 
     orient_kernel<<<grid, 128, 0, st>>>(src, w, h, C, o, dst, W, H);
     g_launches++;
     LP_CUDA_OK(cudaGetLastError());
+    return LP_OK;
+}
+
+// Oriented crops of decoded windows (batch.cu): one CTA per 32 x 32 tile of a job's crop.  Under every orientation the
+// tile's source pixels form a rectangle of the window of at most 32 x 32; it is read row by row into shared memory (a
+// BGR pixel per 32-bit word, rows padded to 33 words so that a column is conflict-free) and the tile is written row by
+// row of the crop, so both sides move runs of consecutive pixels even when the orientation transposes.
+__global__ void __launch_bounds__(256)
+    orient_crop_kernel(const OrientJob* __restrict__ jobs, const uint8_t* __restrict__ src, uint8_t* __restrict__ dst,
+                       int w, int h) {
+    __shared__ uint32_t tile[32][33];
+    const OrientJob j = jobs[blockIdx.z];
+    const int x0 = blockIdx.x * 32, y0 = blockIdx.y * 32;
+    if (x0 >= j.cw || y0 >= j.ch) return;  // (uniform over the CTA)
+    const int x1 = min(x0 + 32, j.cw) - 1, y1 = min(y0 + 32, j.ch) - 1;
+    int ax, ay, bx, by;  // pre-images of the tile's first and last pixel: opposite corners of its source rectangle
+    orient_source_pixel(j.o, w, h, j.cx + x0, j.cy + y0, &ax, &ay);
+    orient_source_pixel(j.o, w, h, j.cx + x1, j.cy + y1, &bx, &by);
+    const int sx0 = min(ax, bx), sy0 = min(ay, by);
+    const int sw = abs(bx - ax) + 1, sh = abs(by - ay) + 1;
+    const uint8_t* s = src + j.src_off + (size_t)(sy0 - j.win_y0) * j.src_stride + (size_t)(sx0 - j.win_x0) * 3;
+    for (int r = threadIdx.y; r < sh; r += blockDim.y) {
+        if ((int)threadIdx.x < sw) {
+            const uint8_t* p = s + (size_t)r * j.src_stride + threadIdx.x * 3;
+            tile[r][threadIdx.x] = (uint32_t)p[0] | ((uint32_t)p[1] << 8) | ((uint32_t)p[2] << 16);
+        }
+    }
+    __syncthreads();
+    const int x = x0 + (int)threadIdx.x;
+    if (x > x1) return;
+    for (int y = y0 + (int)threadIdx.y; y <= y1; y += blockDim.y) {
+        int sx, sy;
+        orient_source_pixel(j.o, w, h, j.cx + x, j.cy + y, &sx, &sy);
+        const uint32_t v = tile[sy - sy0][sx - sx0];
+        uint8_t* q = dst + j.dst_off + ((size_t)y * j.cw + x) * 3;
+        q[0] = (uint8_t)v;
+        q[1] = (uint8_t)(v >> 8);
+        q[2] = (uint8_t)(v >> 16);
+    }
+}
+
+int orient_crop_launch(const OrientJob* d_jobs, int n, const uint8_t* src, uint8_t* dst, int w, int h, int max_cw,
+                       int max_ch, cudaStream_t st) {
+    constexpr int kMaxJobsPerLaunch = 65535;  // gridDim.z
+    for (int j0 = 0; j0 < n; j0 += kMaxJobsPerLaunch) {
+        dim3 grid(ceil_div(max_cw, 32), ceil_div(max_ch, 32), std::min(kMaxJobsPerLaunch, n - j0));
+        orient_crop_kernel<<<grid, dim3(32, 8), 0, st>>>(d_jobs + j0, src, dst, w, h);
+        g_launches++;
+        LP_CUDA_OK(cudaGetLastError());
+    }
     return LP_OK;
 }
 

@@ -242,6 +242,7 @@ struct AreaParams {
     int ypad;
     int rows_per_band;
     int slot_bytes;
+    const int* index = nullptr;  // ResizeArgs::index
 };
 
 constexpr int kAreaTile = 256;    // destination pixels per CTA
@@ -299,7 +300,7 @@ __global__ void __launch_bounds__(kAreaTile / PPT + 32)
     uint8_t* ring = smem + 256 + kAreaMaxBand * kAreaMaxYTaps * 4;
 
     const int tid = threadIdx.x;
-    const int img = blockIdx.z;
+    const int img = p.index ? __ldg(p.index + blockIdx.z) : blockIdx.z;
     const int dx0 = blockIdx.x * kAreaTile;
     const int dx1 = min(dx0 + kAreaTile, p.dw);
     const int dy0 = blockIdx.y * p.rows_per_band;
@@ -445,7 +446,7 @@ __global__ void __launch_bounds__(kAreaTile / PPT + 32)
 // runtime loops, direct global loads.  One thread per destination sample.
 __global__ void resize_area_generic_kernel(const AreaParams p, int C, int xpad) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    const int img = blockIdx.z;
+    const int img = p.index ? __ldg(p.index + blockIdx.z) : blockIdx.z;
     if (i >= p.dw * C) return;
     const int dx = i / C, c = i % C;
     const int dy = blockIdx.y;
@@ -472,12 +473,13 @@ struct BoxParams {
     uint8_t* dst;
     size_t dst_img_stride, dst_row_stride;
     int crop_x, crop_y, dw, dh, kx, ky, C;
+    const int* index = nullptr;  // ResizeArgs::index
 };
 
 __global__ void resize_box_kernel(const BoxParams p) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;  // sample index within the dst row
     if (i >= p.dw * p.C) return;
-    const int dy = blockIdx.y, img = blockIdx.z;
+    const int dy = blockIdx.y, img = p.index ? __ldg(p.index + blockIdx.z) : blockIdx.z;
     const int dx = i / p.C, c = i % p.C;
     const uint8_t* s = p.src + (size_t)img * p.src_img_stride +
                        (size_t)(p.crop_y + dy * p.ky) * p.src_row_stride +
@@ -505,12 +507,13 @@ struct LinearParams {
     const short* xa;  // [dw][2]
     const int* yofs;
     const short* yb;  // [dh][2]
+    const int* index = nullptr;  // ResizeArgs::index
 };
 
 __global__ void resize_linear_kernel(const LinearParams p) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= p.dw * p.C) return;
-    const int dy = blockIdx.y, img = blockIdx.z;
+    const int dy = blockIdx.y, img = p.index ? __ldg(p.index + blockIdx.z) : blockIdx.z;
     const int dx = i / p.C, c = i % p.C;
     const int sx = p.xofs[dx], a0 = p.xa[2 * dx], a1 = p.xa[2 * dx + 1];
     const int sx1 = min(sx + 1, p.sw - 1);
@@ -772,14 +775,19 @@ int resize_launch(const ResizeArgs& a, cudaStream_t st) {
     if (a.crop_w < 1 || a.crop_h < 1 || a.dst_w < 1 || a.dst_h < 1) return LP_ERR_BAD_ARGUMENT;
     if (a.channels != 1 && a.channels != 3 && a.channels != 4) return LP_ERR_BAD_ARGUMENT;
     if (a.interpolation != 1 && a.interpolation != 2 && a.interpolation != 3) return LP_ERR_UNSUPPORTED;
+    if (a.index && a.interpolation == 2) return LP_ERR_UNSUPPORTED;  // (no caller maps images through INTER_CUBIC)
     // Every kernel below takes the image from blockIdx.z, and gridDim.z is at most 65535: a larger batch (the frames of
     // a GIF task in lp_xbatch can exceed it) goes in slices of that many images.
     constexpr int kMaxImagesPerLaunch = 65535;
     if (a.n > kMaxImagesPerLaunch) {
         for (int i0 = 0; i0 < a.n; i0 += kMaxImagesPerLaunch) {
             ResizeArgs s = a;
-            s.src += (size_t)i0 * a.src_img_stride;
-            s.dst += (size_t)i0 * a.dst_img_stride;
+            if (a.index) {
+                s.index += i0;
+            } else {
+                s.src += (size_t)i0 * a.src_img_stride;
+                s.dst += (size_t)i0 * a.dst_img_stride;
+            }
             s.n = std::min(kMaxImagesPerLaunch, a.n - i0);
             const int rc = resize_launch(s, st);
             if (rc) return rc;
@@ -787,6 +795,16 @@ int resize_launch(const ResizeArgs& a, cudaStream_t st) {
         return LP_OK;
     }
     const int C = a.channels;
+    if (a.crop_w == a.dst_w && a.crop_h == a.dst_h && a.index) {
+        // cv::resize: same size is a copy; with an image map that is the box kernel with 1 x 1 boxes (exact)
+        BoxParams p{a.src, a.src_img_stride, a.src_row_stride, a.dst, a.dst_img_stride,
+                    a.dst_row_stride, a.crop_x, a.crop_y, a.dst_w, a.dst_h, 1, 1, C, a.index};
+        dim3 grid(ceil_div(a.dst_w * C, 256), a.dst_h, a.n);
+        resize_box_kernel<<<grid, 256, 0, st>>>(p);
+        g_launches++;
+        LP_CUDA_OK(cudaGetLastError());
+        return LP_OK;
+    }
     if (a.crop_w == a.dst_w && a.crop_h == a.dst_h) {  // cv::resize: same size is a copy
         LP_CUDA_OK(cudaMemcpy2DAsync(a.dst, a.dst_row_stride,
                                      a.src + (size_t)a.crop_y * a.src_row_stride + (size_t)a.crop_x * C,
@@ -809,7 +827,7 @@ int resize_launch(const ResizeArgs& a, cudaStream_t st) {
     if (interp == 3 && scale_x >= 1 && scale_y >= 1) {
         if (is_area_fast) {
             BoxParams p{a.src, a.src_img_stride, a.src_row_stride, a.dst, a.dst_img_stride,
-                        a.dst_row_stride, a.crop_x, a.crop_y, a.dst_w, a.dst_h, ix, iy, C};
+                        a.dst_row_stride, a.crop_x, a.crop_y, a.dst_w, a.dst_h, ix, iy, C, a.index};
             dim3 grid(ceil_div(a.dst_w * C, 256), a.dst_h, a.n);
             resize_box_kernel<<<grid, 256, 0, st>>>(p);
             g_launches++;
@@ -840,6 +858,7 @@ int resize_launch(const ResizeArgs& a, cudaStream_t st) {
         p.crop_x = a.crop_x; p.crop_y = a.crop_y; p.dw = a.dst_w; p.dh = a.dst_h;
         p.xfirst = tx.first; p.xcount = tx.count; p.xperm = tx.perm; p.xw = tx.w;
         p.yfirst = ty.first; p.ycount = ty.count; p.yw = ty.w; p.ypad = ty.padt;
+        p.index = a.index;
         if (tx.padt > 16) {
             dim3 grid(ceil_div(a.dst_w * C, 128), a.dst_h, a.n);
             resize_area_generic_kernel<<<grid, 128, 0, st>>>(p, C, tx.padt);
@@ -893,7 +912,7 @@ int resize_launch(const ResizeArgs& a, cudaStream_t st) {
     LP_CUDA_OK(cudaStreamSynchronize(st));  // host vectors go out of scope below
     LinearParams p{a.src, a.src_img_stride, a.src_row_stride, a.dst, a.dst_img_stride,
                    a.dst_row_stride, a.crop_x, a.crop_y, a.crop_w, a.crop_h, a.dst_w, a.dst_h, C,
-                   dxo, dxa, dyo, dyb};
+                   dxo, dxa, dyo, dyb, a.index};
     dim3 grid(ceil_div(a.dst_w * C, 256), a.dst_h, a.n);
     resize_linear_kernel<<<grid, 256, 0, st>>>(p);
     g_launches++;

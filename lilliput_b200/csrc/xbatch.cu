@@ -48,7 +48,8 @@ using namespace lp;
 
 namespace lp {
 lp_batch* batch_create_in(const lp_batch_config* cfg, uint8_t* dev_arena, size_t dev_bytes, uint8_t* host_arena,
-                          size_t host_bytes, bool progressive_jpeg, bool multiscan_sources, bool resize_only);
+                          size_t host_bytes, bool progressive_jpeg, bool multiscan_sources, bool resize_only,
+                          bool oriented_sources = false);  // (rotated JPEGs are handed to lp_transform before grouping)
 int batch_resized_status(lp_batch* b, int* status);
 size_t batch_multiscan_pool_bytes(size_t n);
 void batch_arena_used(const lp_batch* b, size_t* dev_bytes, size_t* host_bytes);
