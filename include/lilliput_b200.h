@@ -165,15 +165,17 @@ void lp_batch_destroy(lp_batch* b);
  * (pinned or not); H2D of the compressed bytes and D2H of the encoded bytes are
  * inside the call.  status[i] is an lp_status per image.
  *
- * Sources taken: 8-bit Huffman-coded 3-component JPEGs of the configured size, with any
- * EXIF orientation -- baseline or extended sequential (with or without restart markers
+ * Sources taken: 8-bit Huffman-coded 3-component (YCbCr) and 1-component (gray) JPEGs of
+ * the configured size, in any order in one batch, with any EXIF orientation -- baseline or extended sequential (with or without restart markers
  * and optimised tables), progressive, or sequential with one scan per component.  The
  * orientation is applied on the device, per item, as Transform applies it (whether or
  * not normalize_orientation is set); an orientation that swaps the axes may give an item
  * another output size than the top-left ones (Fit above the source size, Width != Height).
- * Each item gets the status and bytes lp_transform gives it, except that gray files, and
- * multi-scan files that overflow the context's scan or Huffman-table pools (sized by
- * max_images, see batch.cu), get LP_ERR_UNSUPPORTED. */
+ * A gray item is decoded, oriented and resized on one channel and comes back as a
+ * one-component JPEG, as Transform writes it.
+ * Each item gets the status and bytes lp_transform gives it, except that multi-scan files
+ * that overflow the context's scan or Huffman-table pools (sized by max_images, see
+ * batch.cu) get LP_ERR_UNSUPPORTED. */
 int lp_batch_transform(lp_batch* b, const uint8_t* const* in, const size_t* in_len, int n,
                        uint8_t* const* out, size_t* out_len, int* status);
 
@@ -201,6 +203,9 @@ int lp_batch_last_launches(const lp_batch* b);
 size_t lp_batch_d2h_overhead_per_image(void);
 /* Images per pipelined chunk actually used by this context. */
 int lp_batch_chunk(const lp_batch* b);
+/* Channels of item i's decoded and resized frames in the staged batch: 3 (BGR), 1 (a gray source), 0 when its
+ * header was refused. */
+int lp_batch_item_channels(const lp_batch* b, int i);
 /* Diagnostics (valid after lp_batch_fetch / lp_batch_transform): rounds the parallel Huffman
  * synchronisation needed per image. */
 void lp_batch_sync_rounds(const lp_batch* b, double* mean, int* max);
@@ -209,7 +214,9 @@ void lp_batch_sync_rounds(const lp_batch* b, double* mean, int* max);
  * [5] number of CTAs (= images).  reset != 0 clears the counters after reading.  Returns an lp_status. */
 int lp_huff_phase_clocks(unsigned long long* out8, int reset);
 /* Device pointer to the decoded frames / resized frames of the last run (tests).  Resized frame i is at
- * i * image_stride, rows packed, in its own output size; decoded windows are slot-strided within the last chunk. */
+ * i * image_stride, rows packed, in its own output size; decoded windows are slot-strided within the last chunk.
+ * Slots are spaced for 3 channels; a gray item's frame is 1 channel (lp_batch_item_channels), its rows packed (resized)
+ * or a 16-byte multiple apart (decoded window) from the start of its own slot. */
 const uint8_t* lp_batch_decoded_dev(const lp_batch* b, size_t* image_stride);
 const uint8_t* lp_batch_resized_dev(const lp_batch* b, size_t* image_stride);
 

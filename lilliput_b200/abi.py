@@ -317,7 +317,7 @@ STAGE_NAMES = ["huff_decode", "idct_color", "resize", "enc_transform", "enc_entr
 
 
 class Batch:
-    """lp_batch_*: N independent JPEGs -> Fit/area resize -> JPEG on one GPU."""
+    """lp_batch_*: N independent JPEGs (colour and gray, any EXIF orientation) -> Fit/area resize -> JPEG on one GPU."""
 
     def __init__(self, lib: Lib, device: int, max_images: int, src_w: int, src_h: int, dst_w: int,
                  dst_h: int, quality: int, max_in_bytes: int, out_cap: int = 65536,
@@ -341,6 +341,8 @@ class Batch:
         l.lp_batch_last_launches.argtypes = [C.c_void_p]
         l.lp_batch_chunk.restype = C.c_int
         l.lp_batch_chunk.argtypes = [C.c_void_p]
+        l.lp_batch_item_channels.restype = C.c_int
+        l.lp_batch_item_channels.argtypes = [C.c_void_p, C.c_int]
         for name in ("lp_batch_decoded_dev", "lp_batch_resized_dev"):
             getattr(l, name).restype = C.c_void_p
             getattr(l, name).argtypes = [C.c_void_p, C.POINTER(C.c_size_t)]
@@ -418,6 +420,10 @@ class Batch:
     def last_launches(self):
         return self.lib.l.lp_batch_last_launches(self.h)
 
+    def item_channels(self, i: int) -> int:
+        """Channels of staged item i's frames: 3, 1 for a gray source, 0 when its header was refused."""
+        return self.lib.l.lp_batch_item_channels(self.h, i)
+
     def _copy_back(self, getter, n):
         stride = C.c_size_t(0)
         ptr = getter(self.h, C.byref(stride))
@@ -443,6 +449,13 @@ class Batch:
         if buf.shape[1] != w * h * 3:
             raise ValueError(f"resized frames are {buf.shape[1]} bytes, not {w}x{h}x3")
         return buf.reshape(n, h, w, 3)
+
+    def frame_slots(self, n: int, resized: bool) -> np.ndarray:
+        """The raw slots of the last `run()`, (n, slot bytes): the resized frames, or the decoded windows of a batch
+        that fits one chunk.  Item i's frame starts its slot with `item_channels(i)` bytes per pixel."""
+        if not resized and n > self.lib.l.lp_batch_chunk(self.h):
+            raise ValueError("the decoded frames of a multi-chunk batch are not kept")
+        return self._copy_back(self.lib.l.lp_batch_resized_dev if resized else self.lib.l.lp_batch_decoded_dev, n)
 
 
 # ----------------------------------------------------------------------------------------------

@@ -23,6 +23,17 @@
 // one launch turns the rotated items' windows into their oriented crops, packed, and each class present is resized
 // (and class 2, when its size differs, encoded) through an image map, so results stay at the caller's item index.
 // A chunk without rotated items launches exactly what it did before orientation was taken.
+//
+// Gray sources (contexts made by lp_batch_create).  A one-component file is decoded into a 1-channel window, oriented,
+// resized and encoded on one channel, as Transform does, next to the colour items of its chunk.  The channel count
+// is a per-item property beside the orientation class, so a chunk has up to six sub-classes, in the order of its image
+// map: colour classes 0, 1, 2, then gray classes 0, 1, 2.  Each sub-class present gets one resize launch, each channel
+// count with rotated items one orientation launch, each (channel count, output size) present one encode.  Slots (decoded
+// window, oriented crop, resized frame) stay sized and spaced for three channels: a gray item's rows are packed at the
+// start of its slot and take a third of it, and the encoder scratch is the colour geometry's (the larger), so taking
+// gray files allocates nothing.  A chunk with no gray item launches exactly what it launched before gray was taken, with
+// the same strides and slot layout; a chunk of unrotated gray items only launches without an image map, like a chunk of
+// unrotated colour items.
 #include <algorithm>
 #include <cstring>
 #include <map>
@@ -55,6 +66,7 @@ struct lp_batch {
     bool multiscan = true;           // takes multi-scan sources (lp_xbatch groups of single-scan files do not)
     bool resize_only = false;        // lp_xbatch's WebP and PNG sinks: the chunk ends with the resized frames (no JPEG encode)
     bool orient = false;             // takes EXIF-rotated sources (lp_batch_create; lp_xbatch hands them to lp_transform)
+    bool gray = false;               // takes one-component sources (lp_batch_create; lp_xbatch hands them to lp_transform)
     size_t arena_dev_used = 0, arena_host_used = 0;  // bytes carved from the caller's arenas (batch_create_in)
     cudaStream_t st = nullptr;       // kernels
     cudaStream_t st_h2d = nullptr;   // input copies (pipelined transform)
@@ -79,6 +91,7 @@ struct lp_batch {
     uint32_t blocks = 0;
     size_t max_blocks_alloc = 0;
     size_t frame_bytes = 0, resized_bytes = 0;
+    uint32_t gray_row_bytes = 0;  // row stride of an unrotated gray item's decoded window
     // device
     uint8_t* d_scan = nullptr;
     JpegDecodeItem* d_items = nullptr;
@@ -100,7 +113,7 @@ struct lp_batch {
     uint32_t* d_out_len = nullptr;
     uint8_t* d_oriented = nullptr;  // per chunk slot: a rotated item's oriented crop
     OrientJob* d_jobs = nullptr;    // per image: the rotated items of each chunk, from the chunk's first image
-    int* d_index = nullptr;         // per image: each chunk's slots ordered by class (the resize / encode image maps)
+    int* d_index = nullptr;         // per image: each chunk's slots ordered by sub-class (the resize / encode image maps)
     // host
     std::vector<JpegDecodeItem> items;
     std::vector<JpegHuffSet> tables;
@@ -122,7 +135,12 @@ struct lp_batch {
         int ordinal = 0;
         int n_multiscan = 0;
         size_t frame_stride = 0;        // decoded-window slot stride
-        int n_class[3] = {0, 0, 0};     // items per orientation class (the classes at the top of the file)
+        // items per sub-class (top of the file): colour orientation classes 0, 1, 2, then gray 0, 1, 2
+        int n_class[6] = {0, 0, 0, 0, 0, 0};
+        // whether the chunk launches through the image map: not when all of it is unrotated items of one channel count
+        bool mapped(int cnt) const {
+            return n_class[1] + n_class[2] + n_class[3] + n_class[4] + n_class[5] > 0 && n_class[3] != cnt;
+        }
         std::vector<uint2> rst_work;  // (image in chunk, restart interval) of the chunk's DRI images
         uint2* d_rst_work = nullptr;  // stream-ordered allocation, freed after the chunk's launches
     };
@@ -167,12 +185,12 @@ static void batch_free(lp_batch* b) {
 namespace lp {
 lp_batch* batch_create_in(const lp_batch_config* cfg, uint8_t* dev_arena, size_t dev_bytes, uint8_t* host_arena,
                           size_t host_bytes, bool progressive_jpeg = false, bool multiscan_sources = true,
-                          bool resize_only = false, bool oriented_sources = false);
+                          bool resize_only = false, bool oriented_sources = false, bool gray_sources = false);
 int batch_resized_status(lp_batch* b, int* status);
 void batch_arena_used(const lp_batch* b, size_t* dev_bytes, size_t* host_bytes);
 }
 extern "C" lp_batch* lp_batch_create(const lp_batch_config* cfg) {
-    return lp::batch_create_in(cfg, nullptr, 0, nullptr, 0, false, true, false, true);
+    return lp::batch_create_in(cfg, nullptr, 0, nullptr, 0, false, true, false, true, true);
 }
 
 // dev_arena / host_arena non-null: every device / pinned buffer is carved from them (nothing is allocated or
@@ -181,10 +199,12 @@ extern "C" lp_batch* lp_batch_create(const lp_batch_config* cfg) {
 // LP_ERR_UNSUPPORTED.  resize_only: every chunk stops after the resize, so the context has no JPEG encoder scratch and
 // no output slots; it is driven by lp_batch_stage + lp_batch_run, then batch_resized_status (lp_batch_transform and
 // lp_batch_fetch refuse it), and the caller encodes the frames at lp_batch_resized_dev.  oriented_sources: take
-// EXIF-rotated files (and allocate the oriented-crop buffers); otherwise they get LP_ERR_UNSUPPORTED.
+// EXIF-rotated files (and allocate the oriented-crop buffers); otherwise they get LP_ERR_UNSUPPORTED.  gray_sources: take
+// one-component files (they fit the colour slots: only the image map is allocated for them); otherwise they get
+// LP_ERR_UNSUPPORTED.
 lp_batch* lp::batch_create_in(const lp_batch_config* cfg, uint8_t* dev_arena, size_t dev_bytes, uint8_t* host_arena,
                               size_t host_bytes, bool progressive_jpeg, bool multiscan_sources, bool resize_only,
-                              bool oriented_sources) {
+                              bool oriented_sources, bool gray_sources) {
     if (!cfg || cfg->max_images < 1 || cfg->src_width < 1 || cfg->src_height < 1) return nullptr;
     if (ensure_device()) return nullptr;
     DeviceGuard dev_guard(cfg->device);
@@ -195,6 +215,7 @@ lp_batch* lp::batch_create_in(const lp_batch_config* cfg, uint8_t* dev_arena, si
     b->multiscan = multiscan_sources;
     b->resize_only = resize_only;
     b->orient = oriented_sources;
+    b->gray = gray_sources;
     b->owns_mem = dev_arena == nullptr;
     size_t dev_used = 0, host_used = 0;
     b->W = cfg->src_width;
@@ -290,11 +311,16 @@ lp_batch* lp::batch_create_in(const lp_batch_config* cfg, uint8_t* dev_arena, si
         size_t enc = jpeg_encode_scratch_bytes(b->out_w, b->out_h, 3, b->chunk, cfg->out_cap, b->progressive);
         if (b->orient)
             enc = std::max(enc, jpeg_encode_scratch_bytes(b->out_w2, b->out_h2, 3, b->chunk, cfg->out_cap, b->progressive));
+        for (int c = 0; c < (b->gray ? 2 : 0); c++)  // (colour is the larger but for rounding: six blocks per 16 x 16 pixels against four)
+            enc = std::max(enc, jpeg_encode_scratch_bytes(c ? b->out_w2 : b->out_w, c ? b->out_h2 : b->out_h, 1, b->chunk,
+                                                          cfg->out_cap, b->progressive));
         BALLOC(b->d_enc_scratch, enc);
     }
     if (b->orient) {
         BALLOC(b->d_oriented, (size_t)b->chunk * b->oriented_bytes);
         BALLOC(b->d_jobs, N * sizeof(OrientJob));
+    }
+    if (b->orient || b->gray) {
         BALLOC(b->d_index, N * sizeof(int));
     }
     BALLOC(b->d_clean, cfg->max_in_bytes + 64 * N + 4096);
@@ -330,8 +356,8 @@ lp_batch* lp::batch_create_in(const lp_batch_config* cfg, uint8_t* dev_arena, si
     b->file_dev_off.resize(N);
     if (b->orient) {
         b->jobs.resize(N);
-        b->index.resize(N);
     }
+    if (b->orient || b->gray) b->index.resize(N);
     b->arena_dev_used = dev_used;
     b->arena_host_used = host_used;
     return b;
@@ -426,7 +452,7 @@ static int batch_layout_chunk(lp_batch* b, const uint8_t* const* in, const size_
 static int batch_parse_chunk(lp_batch* b, const uint8_t* const* in, const size_t* in_len, int i0, int cnt, int ordinal) {
     std::vector<JpegHeader> hdr((size_t)cnt);
     std::vector<uint32_t> blocks_of((size_t)cnt, 0), tiles_of((size_t)cnt, 0), total_of((size_t)cnt, 0);
-    std::vector<uint8_t> class_of((size_t)cnt, 0);  // orientation class (top of the file)
+    std::vector<uint8_t> class_of((size_t)cnt, 0);  // sub-class (top of the file): orientation class, + 3 for gray
     // multi-scan files: their scans (table_set numbering the file's own sets) and the Huffman tables of each set
     std::vector<std::vector<JpegScanDesc>> ms_scans((size_t)cnt);
     std::vector<std::vector<JpegHeader>> ms_sets((size_t)cnt);
@@ -442,8 +468,8 @@ static int batch_parse_chunk(lp_batch* b, const uint8_t* const* in, const size_t
             const int o = h.orientation;
             const int cls = o >= 2 && o <= 8 ? (o >= 5 ? 2 : 1) : 0;
             if (!rc && cls && !b->orient) rc = LP_ERR_UNSUPPORTED;
-            class_of[k - i0] = (uint8_t)cls;
-            if (!rc && h.ncomp != 3) rc = LP_ERR_UNSUPPORTED;
+            if (!rc && h.ncomp != 3 && !(h.ncomp == 1 && b->gray)) rc = LP_ERR_UNSUPPORTED;
+            class_of[k - i0] = (uint8_t)(cls + (h.ncomp == 1 ? 3 : 0));
             if (!rc && ms) {
                 // what the per-image decoder refuses when it reads the scans (damage, over the work budget), lp_transform
                 // reports as a failed decode
@@ -472,7 +498,7 @@ static int batch_parse_chunk(lp_batch* b, const uint8_t* const* in, const size_t
                     memcpy(it.qt[c], h.qt[h.comp[c].tq], sizeof(it.qt[c]));
                     it.td[c] = h.comp[c].td; it.ta[c] = h.comp[c].ta;
                 }
-                it.frame_channels = 3;
+                it.frame_channels = h.ncomp == 1 ? 1 : 3;
                 // decode only what Fit will read: the crop window (+ the chroma-upsampling margin); a rotated item's
                 // crop is in its oriented frame, and the window is that crop's pre-image in the source
                 int x0 = b->crop_x, y0 = b->crop_y, x1 = b->crop_x + b->crop_w, y1 = b->crop_y + b->crop_h;
@@ -517,14 +543,15 @@ static int batch_parse_chunk(lp_batch* b, const uint8_t* const* in, const size_t
         lay.blocks = std::max(lay.blocks, blocks_of[k - i0]);
         lay.tiles = std::max(lay.tiles, tiles_of[k - i0]);
         lay.total_blocks = std::max(lay.total_blocks, total_of[k - i0]);
-        if (class_of[k - i0]) rotated_window_bytes = std::max(rotated_window_bytes, (size_t)it.win_stride * it.win_h);
+        if (class_of[k - i0] % 3) rotated_window_bytes = std::max(rotated_window_bytes, (size_t)it.win_stride * it.win_h);
         if (!b->layout_known) {  // class 0's decoded window depends on the geometry only, which the context fixes
             JpegDecodeItem a = it;
             jpeg_item_set_window(&a, b->crop_x, b->crop_y, b->crop_x + b->crop_w, b->crop_y + b->crop_h, true, nullptr);
             b->win_w = a.win_w;
             b->win_h = a.win_h;
             b->win_x0 = a.win_x0;
-            b->frame_bytes = (size_t)a.win_stride * a.win_h;
+            b->frame_bytes = (size_t)jpeg_window_row_bytes(a.win_x0, a.win_w, a.width, 3) * a.win_h;
+            b->gray_row_bytes = jpeg_window_row_bytes(a.win_x0, a.win_w, a.width, 1);
             b->layout_known = true;
         }
     }
@@ -594,22 +621,22 @@ static int batch_parse_chunk(lp_batch* b, const uint8_t* const* in, const size_t
         b->clean_off += huff_clean_bytes(it.scan_len);
         b->state_off += state_need;
     }
-    if (b->orient) {
-        // the chunk's slots by class (the resize / encode image maps), and the oriented crops of classes 1 and 2 in
-        // that order; an item refused above is class 0 whatever its orientation
+    if (!b->index.empty()) {
+        // the chunk's slots by sub-class (the resize / encode image maps), and the oriented crops of the rotated items in
+        // that order; an item refused above is a colour item of class 0 whatever it is
         lp_batch::ChunkLayout& cl = b->chunk_layout[i0];
         int* idx = b->index.data() + i0;
-        OrientJob* job = b->jobs.data() + i0;
-        int at = 0;
-        for (int c = 0; c < 3; c++) {
+        int at = 0, rotated = 0;
+        for (int s = 0; s < 6; s++) {
+            const int c = s % 3;
             for (int k = i0; k < i0 + cnt; k++) {
                 const int cls = b->parse_status[k] ? 0 : class_of[k - i0];
-                if (cls != c) continue;
+                if (cls != s) continue;
                 idx[at++] = k - i0;
-                cl.n_class[c]++;
+                cl.n_class[s]++;
                 if (!c) continue;
                 const JpegDecodeItem& it = b->items[k];
-                OrientJob& j = job[at - 1 - cl.n_class[0]];
+                OrientJob& j = b->jobs[i0 + rotated++];
                 j.src_off = it.frame_off;
                 j.dst_off = (uint64_t)(k - i0) * b->oriented_bytes;
                 j.src_stride = it.win_stride;
@@ -645,11 +672,14 @@ static int batch_upload_items(lp_batch* b, int i0, int cnt, cudaStream_t st) {
     LP_CUDA_OK(cudaMemcpyAsync(b->d_items + i0, b->items.data() + i0, (size_t)cnt * sizeof(JpegDecodeItem),
                                cudaMemcpyHostToDevice, st));
     const auto lay = b->chunk_layout.find(i0);
-    const int rotated = lay == b->chunk_layout.end() ? 0 : lay->second.n_class[1] + lay->second.n_class[2];
-    if (rotated) {  // (a chunk without rotated items launches without image maps)
-        LP_CUDA_OK(cudaMemcpyAsync(b->d_index + i0, b->index.data() + i0, (size_t)cnt * sizeof(int), cudaMemcpyHostToDevice, st));
-        LP_CUDA_OK(cudaMemcpyAsync(b->d_jobs + i0, b->jobs.data() + i0, (size_t)rotated * sizeof(OrientJob),
-                                   cudaMemcpyHostToDevice, st));
+    if (lay != b->chunk_layout.end()) {
+        const int* nc = lay->second.n_class;
+        const int rotated = nc[1] + nc[2] + nc[4] + nc[5];
+        if (lay->second.mapped(cnt))
+            LP_CUDA_OK(cudaMemcpyAsync(b->d_index + i0, b->index.data() + i0, (size_t)cnt * sizeof(int), cudaMemcpyHostToDevice, st));
+        if (rotated)
+            LP_CUDA_OK(cudaMemcpyAsync(b->d_jobs + i0, b->jobs.data() + i0, (size_t)rotated * sizeof(OrientJob),
+                                       cudaMemcpyHostToDevice, st));
     }
     if (b->tables.size() > b->tables_uploaded) {
         LP_CUDA_OK(cudaMemcpyAsync(b->d_tables + b->tables_uploaded, b->tables.data() + b->tables_uploaded,
@@ -705,44 +735,51 @@ static int batch_launch_chunk(lp_batch* b, int i0, int cnt, cudaStream_t st, cud
     int rc = jpeg_decode_launch(d, st, ev ? ev[1] : nullptr);
     if (rc) return rc;
     if (ev) LP_CUDA_OK(cudaEventRecord(ev[2], st));
-    const int n0 = lay.n_class[0], n1 = lay.n_class[1], n2 = lay.n_class[2];
+    // items per sub-class as launched: a chunk that needs no image map is one sub-class in slot order
+    const bool mapped = lay.mapped(cnt);
+    int count[6];
+    for (int s = 0; s < 6; s++) count[s] = mapped ? lay.n_class[s] : 0;
+    if (!mapped) count[lay.n_class[3] == cnt ? 3 : 0] = cnt;
     const int* index = b->d_index + i0;
-    if (n1 + n2) {
-        rc = orient_crop_launch(b->d_jobs + i0, n1 + n2, b->d_frames, b->d_oriented, b->W, b->H,
-                                std::max(n1 ? b->crop_w : 0, n2 ? b->crop2_w : 0),
-                                std::max(n1 ? b->crop_h : 0, n2 ? b->crop2_h : 0), st);
-        if (rc) return rc;
+    for (int g = 0, job0 = 0; g < 2; g++) {  // the rotated items' oriented crops: colour, then gray
+        const int n1 = lay.n_class[3 * g + 1], n2 = lay.n_class[3 * g + 2];
+        if (n1 + n2) {
+            rc = orient_crop_launch(b->d_jobs + i0 + job0, n1 + n2, b->d_frames, b->d_oriented, b->W, b->H, g ? 1 : 3,
+                                    std::max(n1 ? b->crop_w : 0, n2 ? b->crop2_w : 0),
+                                    std::max(n1 ? b->crop_h : 0, n2 ? b->crop2_h : 0), st);
+            if (rc) return rc;
+        }
+        job0 += n1 + n2;
     }
-    ResizeArgs r;
-    r.src = b->d_frames;
-    r.src_img_stride = lay.frame_stride;
-    r.src_row_stride = b->frame_bytes / (size_t)b->win_h;  // window rows (16-byte multiple)
-    r.channels = 3;
-    r.crop_x = b->crop_x - b->win_x0; r.crop_y = 0; r.crop_w = b->crop_w; r.crop_h = b->crop_h;
-    r.dst = b->d_resized + (size_t)i0 * b->resized_bytes;
-    r.dst_img_stride = b->resized_bytes;
-    r.dst_row_stride = (size_t)b->out_w * 3;
-    r.dst_w = b->out_w; r.dst_h = b->out_h;
-    r.n = n1 + n2 ? n0 : cnt;
-    r.interpolation = 3;
-    r.index = n1 + n2 ? index : nullptr;
-    rc = resize_launch(r, st);
-    if (rc) return rc;
-    for (int c = 1; c <= 2; c++) {  // the rotated classes, from their packed oriented crops
-        ResizeArgs q = r;
-        q.n = c == 1 ? n1 : n2;
-        if (!q.n) continue;
-        q.index = index + (c == 1 ? n0 : n0 + n1);
-        q.src = b->d_oriented;
-        q.src_img_stride = b->oriented_bytes;
-        q.crop_x = 0;
-        q.crop_w = c == 1 ? b->crop_w : b->crop2_w;
-        q.crop_h = c == 1 ? b->crop_h : b->crop2_h;
-        q.src_row_stride = (size_t)q.crop_w * 3;
-        q.dst_w = c == 1 ? b->out_w : b->out_w2;
-        q.dst_h = c == 1 ? b->out_h : b->out_h2;
-        q.dst_row_stride = (size_t)q.dst_w * 3;
-        rc = resize_launch(q, st);
+    uint8_t* const resized = b->d_resized + (size_t)i0 * b->resized_bytes;
+    for (int s = 0, at = 0; s < 6; at += count[s++]) {
+        if (!count[s]) continue;
+        const int c = s % 3, ch = s < 3 ? 3 : 1;
+        ResizeArgs r;
+        r.channels = ch;
+        if (c == 0) {  // from the decoded windows (rows a 16-byte multiple)
+            r.src = b->d_frames;
+            r.src_img_stride = lay.frame_stride;
+            r.src_row_stride = ch == 3 ? b->frame_bytes / (size_t)b->win_h : b->gray_row_bytes;
+            r.crop_x = b->crop_x - b->win_x0;
+        } else {  // the rotated classes, from their packed oriented crops
+            r.src = b->d_oriented;
+            r.src_img_stride = b->oriented_bytes;
+            r.src_row_stride = (size_t)(c == 1 ? b->crop_w : b->crop2_w) * ch;
+            r.crop_x = 0;
+        }
+        r.crop_y = 0;
+        r.crop_w = c == 2 ? b->crop2_w : b->crop_w;
+        r.crop_h = c == 2 ? b->crop2_h : b->crop_h;
+        r.dst = resized;
+        r.dst_img_stride = b->resized_bytes;
+        r.dst_w = c == 2 ? b->out_w2 : b->out_w;
+        r.dst_h = c == 2 ? b->out_h2 : b->out_h;
+        r.dst_row_stride = (size_t)r.dst_w * ch;
+        r.n = count[s];
+        r.interpolation = 3;
+        r.index = mapped ? index + at : nullptr;
+        rc = resize_launch(r, st);
         if (rc) return rc;
     }
     if (ev) LP_CUDA_OK(cudaEventRecord(ev[3], st));
@@ -754,30 +791,37 @@ static int batch_launch_chunk(lp_batch* b, int i0, int cnt, cudaStream_t st, cud
         return LP_OK;
     }
     JpegEncodeBatch e;
-    e.frames = r.dst;
+    e.frames = resized;
     e.frame_img_stride = b->resized_bytes;
-    e.frame_row_stride = (size_t)b->out_w * 3;
-    e.width = b->out_w; e.height = b->out_h; e.channels = 3;
     e.quality = b->cfg.jpeg_quality;
-    e.n = cnt;
     e.out = b->d_out + (size_t)i0 * b->cfg.out_cap;
     e.out_cap = b->cfg.out_cap;
     e.out_len = b->d_out_len + i0;
     e.scratch = b->d_enc_scratch;
     e.progressive = b->progressive;
-    if (n2 && (b->out_w2 != b->out_w || b->out_h2 != b->out_h)) {
-        // class 2 has its own output size: classes 0 and 1, then class 2, each through the image map
-        e.n = n0 + n1;
-        e.index = index;
-        rc = jpeg_encode_launch(e, st, nullptr);
-        if (rc) return rc;
-        e.n = n2;
-        e.index = index + n0 + n1;
-        e.width = b->out_w2; e.height = b->out_h2;
-        e.frame_row_stride = (size_t)b->out_w2 * 3;
+    // one encode per (channel count, output size) present: class 2 has its own launch when its size differs.  A chunk
+    // of one channel count and one size is encoded in slot order, without the image map.
+    const bool two_sizes = b->out_w2 != b->out_w || b->out_h2 != b->out_h;
+    std::vector<JpegEncodeBatch> enc;
+    for (int g = 0, at = 0; g < 2; g++) {
+        const int n01 = count[3 * g] + count[3 * g + 1], n2 = count[3 * g + 2];
+        const bool split = n2 && two_sizes;
+        const bool whole_chunk = n01 + n2 == cnt && !split;
+        e.channels = g ? 1 : 3;
+        for (int part = 0; part < 2; part++) {
+            e.n = split ? (part ? n2 : n01) : (part ? 0 : n01 + n2);
+            e.index = whole_chunk ? nullptr : index + at;
+            at += e.n;
+            e.width = split && part ? b->out_w2 : b->out_w;
+            e.height = split && part ? b->out_h2 : b->out_h;
+            e.frame_row_stride = (size_t)e.width * e.channels;
+            if (e.n) enc.push_back(e);
+        }
     }
-    rc = jpeg_encode_launch(e, st, ev ? ev[4] : nullptr);
-    if (rc) return rc;
+    for (size_t k = 0; k < enc.size(); k++) {
+        rc = jpeg_encode_launch(enc[k], st, ev && k + 1 == enc.size() ? ev[4] : nullptr);
+        if (rc) return rc;
+    }
     // the encoded bytes leave packed: slots are out_cap (64 KB) apart but hold a few KB each, so a compaction
     // kernel writes them back to back straight into the pinned, device-mapped host buffer (no D2H of the slots)
     rc = compact_launch(e.out, b->cfg.out_cap, e.out_len, (uint32_t)b->cfg.out_cap, cnt, b->h_out + (size_t)i0 * b->cfg.out_cap,
@@ -976,6 +1020,10 @@ extern "C" int lp_batch_last_launches(const lp_batch* b) { return b ? b->last_la
 // bytes per image that come back besides the encoded file: length, packed offset, the item mirror (status, diagnostics)
 extern "C" size_t lp_batch_d2h_overhead_per_image(void) { return 4 + 8 + sizeof(JpegDecodeItem); }
 extern "C" int lp_batch_chunk(const lp_batch* b) { return b ? b->chunk : 0; }
+extern "C" int lp_batch_item_channels(const lp_batch* b, int i) {
+    if (!b || i < 0 || i >= b->n || b->parse_status[i]) return 0;
+    return b->items[i].frame_channels;
+}
 // Diagnostics after lp_batch_fetch / lp_batch_transform: Huffman synchronisation rounds per image.
 extern "C" void lp_batch_sync_rounds(const lp_batch* b, double* mean, int* max) {
     double sum = 0;

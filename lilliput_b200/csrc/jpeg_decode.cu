@@ -85,9 +85,7 @@ uint32_t jpeg_item_set_window(JpegDecodeItem* it, int x0, int y0, int x1, int y1
     it->win_y0 = y0;
     it->win_w = x1 - x0;
     it->win_h = y1 - y0;
-    const int fc = it->ncomp == 1 ? 1 : 3;
-    it->win_stride = (uint32_t)(((size_t)it->win_w * fc + 15) / 16 * 16);
-    if (x0 == 0 && x1 == it->width) it->win_stride = (uint32_t)it->win_w * fc;  // whole rows: packed
+    it->win_stride = jpeg_window_row_bytes(x0, it->win_w, it->width, it->ncomp == 1 ? 1 : 3);
     // fancy upsampling reads one chroma sample beyond the window on every side = 2 luma pixels at 2x
     const int mw = 8 * maxh, mh = 8 * maxv;
     int px0 = x0 - 2 * maxh, px1 = x1 - 1 + 2 * maxh, py0 = y0 - 2 * maxv, py1 = y1 - 1 + 2 * maxv;
@@ -630,25 +628,51 @@ __device__ __forceinline__ void color16_420(const JpegDecodeItem& it, const Tile
     dst[2] = make_uint4(ow[8], ow[9], ow[10], ow[11]);
 }
 
+// Grayscale: the window pixels [xa, xb) x [ya, yb) of an MCU row are a copy of the tile.  One thread moves one
+// 16-pixel segment of a row; segments are cut at multiples of 16 from the window's left edge, whatever MCU column the
+// span starts at.  When the window's rows are 16-byte aligned in the frame (`aligned`; the windows of batch.cu are) a
+// whole segment is one 16-byte store, fed by two 8-byte shared-memory loads: the halo column of a one-block MCU is 8
+// pixels, so tile columns are 8-byte aligned only.  Ragged segments and unaligned frames go byte by byte.
+__device__ __forceinline__ void gray_phase(const JpegDecodeItem& it, const TileCtx& t, const uint8_t* tile, uint8_t* frames,
+                                        int xa, int xb, int ya, int yb, bool aligned) {
+    const int base = aligned ? it.win_x0 + ((xa - it.win_x0) & ~15) : xa;
+    const int segs = (xb - base + 15) >> 4;
+    const int n = (yb - ya) * segs;
+    for (int j = threadIdx.x; j < n; j += blockDim.x) {
+        const int r = j / segs;
+        const int y = ya + r, x0 = base + (j - r * segs) * 16;
+        uint8_t* out = frames + it.frame_off + (size_t)(y - it.win_y0) * it.win_stride - it.win_x0;
+        const uint8_t* in = tile + tile_row(t, 0, y);
+        if (aligned && x0 >= xa && x0 + 16 <= xb) {
+            const uint2 lo = *reinterpret_cast<const uint2*>(in + x0), hi = *reinterpret_cast<const uint2*>(in + x0 + 8);
+            *reinterpret_cast<uint4*>(out + x0) = make_uint4(lo.x, lo.y, hi.x, hi.y);
+        } else {
+            for (int x = max(x0, xa); x < min(x0 + 16, xb); x++) out[x] = in[x];
+        }
+    }
+}
+
 // Upsample + colour the window pixels of ROI MCU row m inside the span [c0, c1), one thread per 16 consecutive
 // pixels of a row.  4:2:0 frames whose rows are 16-byte aligned take color16_420; everything else (other
-// samplings, odd widths) goes pixel by pixel through upsampled(); grayscale is a copy.
+// samplings, odd widths) goes pixel by pixel through upsampled(); grayscale is a copy (gray_phase).
 __device__ __forceinline__ void color_phase(const JpegDecodeItem& it, const TileCtx& t, const uint8_t* tile,
                                             uint8_t* frames, int m, int c0, int c1, int maxh, int maxv, bool fast) {
     const int mh = 8 * maxv, mw = 8 * maxh;
     const int ya = max(it.win_y0, (it.roi_my0 + m) * mh), yb = min(it.win_y0 + it.win_h, (it.roi_my0 + m + 1) * mh);
     const int xa = max(it.win_x0, (it.roi_mx0 + c0) * mw), xb = min(it.win_x0 + it.win_w, (it.roi_mx0 + c1) * mw);
     if (ya >= yb || xa >= xb) return;
+    if (it.ncomp == 1) {
+        gray_phase(it, t, tile, frames, xa, xb, ya, yb,
+                   (it.win_x0 & 15) == 0 && (it.win_stride & 15) == 0 && (it.frame_off & 15) == 0);
+        return;
+    }
     const int segs = (xb - xa + 15) >> 4;
     const int n = (yb - ya) * segs;
     for (int j = threadIdx.x; j < n; j += blockDim.x) {
         const int r = j / segs;
         const int y = ya + r, x0 = xa + (j - r * segs) * 16;
         uint8_t* out = frames + it.frame_off + (size_t)(y - it.win_y0) * it.win_stride;
-        if (it.ncomp == 1) {
-            const int o = tile_row(t, 0, y);
-            for (int x = x0; x < min(x0 + 16, xb); x++) out[x - it.win_x0] = tile[o + x];
-        } else if (fast) {
+        if (fast) {
             color16_420(it, t, tile, out, x0, y);
         } else {
             for (int x = x0; x < min(x0 + 16, xb); x++) {

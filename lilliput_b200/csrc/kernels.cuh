@@ -62,6 +62,12 @@ int jpeg_parse_header(const uint8_t* data, size_t len, JpegHeader* out);
 // jpeg_idct_color_kernel runs for the image.
 uint32_t jpeg_item_set_window(JpegDecodeItem* it, int x0, int y0, int x1, int y1, bool align16,
                               uint32_t* tiles);
+// Row stride of a decoded window [win_x0, win_x0 + win_w) of a `width`-pixel frame with `channels` bytes per pixel: a
+// 16-byte multiple, except that whole rows are packed.
+inline uint32_t jpeg_window_row_bytes(int win_x0, int win_w, int width, int channels) {
+    if (win_x0 == 0 && win_w == width) return (uint32_t)win_w * channels;
+    return (uint32_t)(((size_t)win_w * channels + 15) / 16 * 16);
+}
 
 void jpeg_build_huff_set(const JpegHeader& h, JpegHuffSet* out);
 // Walks every SOS of a multi-scan file, snapshotting the Huffman tables / restart interval in force.
@@ -317,16 +323,16 @@ __host__ __device__ inline void orient_source_pixel(int o, int w, int h, int x, 
 }
 // One item of orient_crop_launch: the crop [cx, cx+cw) x [cy, cy+ch) of the oriented frame, read from a decoded window
 // of the w x h source (window origin win_x0, win_y0; rows src_stride bytes apart, starting at src_off) and written
-// packed BGR (rows cw * 3 bytes apart) at dst_off.
+// packed (rows cw * channels bytes apart) at dst_off.
 struct OrientJob {
     uint64_t src_off, dst_off;
     uint32_t src_stride;
     int32_t o, cx, cy, cw, ch, win_x0, win_y0;
 };
-// n jobs on 3-channel frames of one w x h source; max_cw / max_ch bound every job's crop.  32 x 32 tiles staged in
-// shared memory, so the transposing orientations read and write whole rows too.
-int orient_crop_launch(const OrientJob* d_jobs, int n, const uint8_t* src, uint8_t* dst, int w, int h, int max_cw,
-                       int max_ch, cudaStream_t st);
+// n jobs on frames of `channels` (3: BGR, 1: gray) of one w x h source; max_cw / max_ch bound every job's crop.
+// 32 x 32 tiles staged in shared memory, so the transposing orientations read and write whole rows too.
+int orient_crop_launch(const OrientJob* d_jobs, int n, const uint8_t* src, uint8_t* dst, int w, int h, int channels,
+                       int max_cw, int max_ch, cudaStream_t st);
 int copy_region_launch(const uint8_t* src, size_t src_step, int src_ch, uint8_t* dst,
                        size_t dst_step, int dst_ch, int w, int h, cudaStream_t st);
 // ---- tonemap.cu ----------------------------------------------------------------------------

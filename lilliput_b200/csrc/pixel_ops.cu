@@ -36,8 +36,10 @@ int orient_launch(const uint8_t* src, int w, int h, int C, int o, uint8_t* dst, 
 
 // Oriented crops of decoded windows (batch.cu): one CTA per 32 x 32 tile of a job's crop.  Under every orientation the
 // tile's source pixels form a rectangle of the window of at most 32 x 32; it is read row by row into shared memory (a
-// BGR pixel per 32-bit word, rows padded to 33 words so that a column is conflict-free) and the tile is written row by
-// row of the crop, so both sides move runs of consecutive pixels even when the orientation transposes.
+// pixel of C = 3 (BGR) or 1 (gray) bytes per 32-bit word, rows padded to 33 words so that a column is conflict-free) and
+// the tile is written row by row of the crop, so both sides move runs of consecutive pixels even when the orientation
+// transposes.
+template <int C>
 __global__ void __launch_bounds__(256)
     orient_crop_kernel(const OrientJob* __restrict__ jobs, const uint8_t* __restrict__ src, uint8_t* __restrict__ dst,
                        int w, int h) {
@@ -51,11 +53,11 @@ __global__ void __launch_bounds__(256)
     orient_source_pixel(j.o, w, h, j.cx + x1, j.cy + y1, &bx, &by);
     const int sx0 = min(ax, bx), sy0 = min(ay, by);
     const int sw = abs(bx - ax) + 1, sh = abs(by - ay) + 1;
-    const uint8_t* s = src + j.src_off + (size_t)(sy0 - j.win_y0) * j.src_stride + (size_t)(sx0 - j.win_x0) * 3;
+    const uint8_t* s = src + j.src_off + (size_t)(sy0 - j.win_y0) * j.src_stride + (size_t)(sx0 - j.win_x0) * C;
     for (int r = threadIdx.y; r < sh; r += blockDim.y) {
         if ((int)threadIdx.x < sw) {
-            const uint8_t* p = s + (size_t)r * j.src_stride + threadIdx.x * 3;
-            tile[r][threadIdx.x] = (uint32_t)p[0] | ((uint32_t)p[1] << 8) | ((uint32_t)p[2] << 16);
+            const uint8_t* p = s + (size_t)r * j.src_stride + threadIdx.x * C;
+            tile[r][threadIdx.x] = C == 1 ? (uint32_t)p[0] : (uint32_t)p[0] | ((uint32_t)p[1] << 8) | ((uint32_t)p[2] << 16);
         }
     }
     __syncthreads();
@@ -65,19 +67,25 @@ __global__ void __launch_bounds__(256)
         int sx, sy;
         orient_source_pixel(j.o, w, h, j.cx + x, j.cy + y, &sx, &sy);
         const uint32_t v = tile[sy - sy0][sx - sx0];
-        uint8_t* q = dst + j.dst_off + ((size_t)y * j.cw + x) * 3;
+        uint8_t* q = dst + j.dst_off + ((size_t)y * j.cw + x) * C;
         q[0] = (uint8_t)v;
-        q[1] = (uint8_t)(v >> 8);
-        q[2] = (uint8_t)(v >> 16);
+        if (C == 3) {
+            q[1] = (uint8_t)(v >> 8);
+            q[2] = (uint8_t)(v >> 16);
+        }
     }
 }
 
-int orient_crop_launch(const OrientJob* d_jobs, int n, const uint8_t* src, uint8_t* dst, int w, int h, int max_cw,
-                       int max_ch, cudaStream_t st) {
+int orient_crop_launch(const OrientJob* d_jobs, int n, const uint8_t* src, uint8_t* dst, int w, int h, int channels,
+                       int max_cw, int max_ch, cudaStream_t st) {
+    if (channels != 1 && channels != 3) return LP_ERR_BAD_ARGUMENT;
     constexpr int kMaxJobsPerLaunch = 65535;  // gridDim.z
     for (int j0 = 0; j0 < n; j0 += kMaxJobsPerLaunch) {
         dim3 grid(ceil_div(max_cw, 32), ceil_div(max_ch, 32), std::min(kMaxJobsPerLaunch, n - j0));
-        orient_crop_kernel<<<grid, dim3(32, 8), 0, st>>>(d_jobs + j0, src, dst, w, h);
+        if (channels == 1)
+            orient_crop_kernel<1><<<grid, dim3(32, 8), 0, st>>>(d_jobs + j0, src, dst, w, h);
+        else
+            orient_crop_kernel<3><<<grid, dim3(32, 8), 0, st>>>(d_jobs + j0, src, dst, w, h);
         g_launches++;
         LP_CUDA_OK(cudaGetLastError());
     }

@@ -49,7 +49,8 @@ using namespace lp;
 namespace lp {
 lp_batch* batch_create_in(const lp_batch_config* cfg, uint8_t* dev_arena, size_t dev_bytes, uint8_t* host_arena,
                           size_t host_bytes, bool progressive_jpeg, bool multiscan_sources, bool resize_only,
-                          bool oriented_sources = false);  // (rotated JPEGs are handed to lp_transform before grouping)
+                          bool oriented_sources = false,  // (rotated and gray JPEGs are handed to lp_transform before
+                          bool gray_sources = false);     // grouping, so these contexts take neither)
 int batch_resized_status(lp_batch* b, int* status);
 size_t batch_multiscan_pool_bytes(size_t n);
 void batch_arena_used(const lp_batch* b, size_t* dev_bytes, size_t* host_bytes);
