@@ -391,7 +391,8 @@ LP_VP8_INL uint8_t clip8(int v) { return (uint8_t)(v < 0 ? 0 : v > 255 ? 255 : v
 LP_VP8_INL int mul1(int a) { return ((a * 20091) >> 16) + a; }
 LP_VP8_INL int mul2(int a) { return (a * 35468) >> 16; }
 
-// dst += IDCT(in), clipped; dst is a stride-`bps` pixel block.
+// dst += IDCT(in), clipped; dst is a stride-`bps` pixel block.  Evaluated in int: libwebp's TransformAC3 /
+// TransformDC (blocks whose tokens stop before zigzag position 3) and its C transform.
 LP_VP8_FN void inverse_dct_add(const int16_t* in, uint8_t* dst, int bps) {
     int tmp[16];
     for (int i = 0; i < 4; i++) {  // vertical pass
@@ -416,6 +417,54 @@ LP_VP8_FN void inverse_dct_add(const int16_t* in, uint8_t* dst, int bps) {
         r[2] = clip8(r[2] + ((b - c) >> 3));
         r[3] = clip8(r[3] + ((a - d) >> 3));
     }
+}
+
+// The same transform as libwebp's x86 build runs it on blocks with a token past zigzag position 2
+// (Transform_SSE2): 16-bit lanes throughout, wrapping adds, mulhi by 20091 and 35468 - 65536 plus the
+// input, an arithmetic >> 3.  Equal to inverse_dct_add while no intermediate leaves int16, which holds for
+// every coefficient within +-2048; crafted streams reach the whole int16 range.
+LP_VP8_INL int wrap16(int v) { return (int16_t)v; }
+LP_VP8_INL int mulhi16(int a, int k) { return (a * k) >> 16; }
+LP_VP8_FN void inverse_dct_add16(const int16_t* in, uint8_t* dst, int bps) {
+    const int k1 = 20091, k2 = 35468 - 65536;
+    int tmp[16];
+    for (int i = 0; i < 4; i++) {  // vertical pass
+        const int i0 = in[i], i1 = in[4 + i], i2 = in[8 + i], i3 = in[12 + i];
+        const int a = i0 + i2;
+        const int b = i0 - i2;
+        const int c = i1 - i3 + mulhi16(i1, k2) - mulhi16(i3, k1);
+        const int d = i1 + i3 + mulhi16(i1, k1) + mulhi16(i3, k2);
+        tmp[4 * i + 0] = wrap16(a + d);
+        tmp[4 * i + 1] = wrap16(b + c);
+        tmp[4 * i + 2] = wrap16(b - c);
+        tmp[4 * i + 3] = wrap16(a - d);
+    }
+    for (int i = 0; i < 4; i++) {  // horizontal pass
+        const int t0 = tmp[i], t1 = tmp[4 + i], t2 = tmp[8 + i], t3 = tmp[12 + i];
+        const int a = t0 + 4 + t2;
+        const int b = t0 + 4 - t2;
+        const int c = t1 - t3 + mulhi16(t1, k2) - mulhi16(t3, k1);
+        const int d = t1 + t3 + mulhi16(t1, k1) + mulhi16(t3, k2);
+        uint8_t* r = dst + i * bps;
+        r[0] = clip8(r[0] + (wrap16(a + d) >> 3));
+        r[1] = clip8(r[1] + (wrap16(b + c) >> 3));
+        r[2] = clip8(r[2] + (wrap16(b - c) >> 3));
+        r[3] = clip8(r[3] + (wrap16(a - d) >> 3));
+    }
+}
+
+// Per-block inverse transform classes (libwebp's NzCodeBits / DoTransform): 2 bits per block.
+enum { TR_NONE = 0, TR_DC = 1, TR_AC3 = 2, TR_FULL = 3 };
+LP_VP8_FN void transform_add(int cls, const int16_t* in, uint8_t* dst, int bps) {
+    if (cls == TR_FULL) inverse_dct_add16(in, dst, bps);
+    else if (cls != TR_NONE) inverse_dct_add(in, dst, bps);
+}
+// Chroma block n (0..3 U, 4..7 V) of `tr_uv`: when any block of its plane has AC (class AC3 or FULL), all four
+// take the full transform (libwebp's DoUVTransform / TransformUV), else each its DC.
+LP_VP8_INL int uv_transform(uint32_t tr_uv, int n) {
+    const uint32_t plane = (tr_uv >> (n & 4 ? 8 : 0)) & 0xff;
+    if (!((tr_uv >> 2 * n) & 3)) return TR_NONE;
+    return (plane & 0xaa) ? TR_FULL : TR_DC;
 }
 
 // ---- intra prediction (RFC 6386 s.12) ------------------------------------------------------
@@ -602,7 +651,8 @@ LP_VP8_HD void work_carve(uint8_t* base, int mb_w, int mb_h, Work& w) {
 struct MbInfo {
     uint8_t is_i4x4, ymode, uvmode, segment;
     uint8_t modes[16];   // sub-block modes when is_i4x4
-    uint32_t nz_blocks;  // bit b set: block b (0..15 Y, 16..19 U, 20..23 V) has a non-zero coefficient
+    uint32_t tr_y;       // bits 2n..2n+1: TR_* class of luma block n
+    uint32_t tr_uv;      // bits 2n..2n+1: TR_* class of chroma block n (0..3 U, 4..7 V), before uv_transform
     uint32_t finfo;      // loop-filter parameters, packed as in Work::finfo
 };
 struct RowCtx {  // state carried from the macroblock on the left
@@ -648,11 +698,11 @@ LP_VP8_FN int parse_mb_modes(const FrameHdr& h, BoolDec& br, uint8_t* tm, RowCtx
 
 // Coefficient tokens of one macroblock (its row's token partition) into `coeffs` (25 blocks of
 // 16, zeroed by the caller; block 24 is scratch for Y2).  `tnz` = the 9 non-zero flags above.
-// Fills mb.nz_blocks and mb.finfo.
+// Fills mb.tr_y, mb.tr_uv and mb.finfo.
 LP_VP8_FN void parse_mb_residuals(const FrameHdr& h, BoolDec& tbr, const uint8_t* proba, uint8_t* tnz, RowCtx& rc,
                                   int skip, MbInfo& mb, int16_t* coeffs) {
     const QuantMat& q = h.q[mb.segment];
-    uint32_t nzb = 0;
+    uint32_t tr_y = 0, tr_uv = 0;
     if (!skip) {
         const int has_y2 = !mb.is_i4x4;
         // one loop over Y2?, 16 Y, 4 U, 4 V so the token reader is instantiated once
@@ -675,15 +725,19 @@ LP_VP8_FN void parse_mb_residuals(const FrameHdr& h, BoolDec& tbr, const uint8_t
             if (k < 0) {
                 inverse_wht(out, coeffs);
             } else {
-                nzb |= (uint32_t)((nz > 1) | (out[0] != 0)) << k;  // the DC may come from the Y2 transform
+                // the DC may come from the Y2 transform
+                const uint32_t cls = nz > 3 ? TR_FULL : nz > 1 ? TR_AC3 : out[0] != 0 ? TR_DC : TR_NONE;
+                if (k < 16) tr_y |= cls << 2 * k;
+                else tr_uv |= cls << 2 * (k - 16);
             }
         }
-        skip = nzb == 0;
+        skip = (tr_y | tr_uv) == 0;
     } else {
         for (int i = 0; i < 8; i++) tnz[i] = rc.left_nz[i] = 0;
         if (!mb.is_i4x4) tnz[8] = rc.left_nz[8] = 0;
     }
-    mb.nz_blocks = nzb;
+    mb.tr_y = tr_y;
+    mb.tr_uv = tr_uv;
     const FilterStrength& f = h.fs[mb.segment][mb.is_i4x4];
     const uint32_t inner = f.inner | (uint32_t)(!skip);
     mb.finfo = f.limit | ((uint32_t)f.ilevel << 8) | ((uint32_t)f.hev << 16) | (inner << 24);
@@ -743,18 +797,18 @@ LP_VP8_FN void reconstruct_mb(const FrameHdr& h, Work& w, int mb_x, int mb_y, co
         for (int n = 0; n < 16; n++) {
             uint8_t* d = yd + (n >> 2) * 4 * BPS + (n & 3) * 4;
             pred_4x4(d, BPS, mb.modes[n]);
-            if ((mb.nz_blocks >> n) & 1) inverse_dct_add(coeffs + n * 16, d, BPS);
+            transform_add((mb.tr_y >> 2 * n) & 3, coeffs + n * 16, d, BPS);
         }
     } else {
         pred_block(yd, BPS, 16, mb.ymode, mb_y > 0, mb_x > 0);
         for (int n = 0; n < 16; n++)
-            if ((mb.nz_blocks >> n) & 1) inverse_dct_add(coeffs + n * 16, yd + (n >> 2) * 4 * BPS + (n & 3) * 4, BPS);
+            transform_add((mb.tr_y >> 2 * n) & 3, coeffs + n * 16, yd + (n >> 2) * 4 * BPS + (n & 3) * 4, BPS);
     }
     pred_block(ud, BPS, 8, mb.uvmode, mb_y > 0, mb_x > 0);
     pred_block(vd, BPS, 8, mb.uvmode, mb_y > 0, mb_x > 0);
     for (int n = 0; n < 4; n++) {
-        if ((mb.nz_blocks >> (16 + n)) & 1) inverse_dct_add(coeffs + (16 + n) * 16, ud + (n >> 1) * 4 * BPS + (n & 1) * 4, BPS);
-        if ((mb.nz_blocks >> (20 + n)) & 1) inverse_dct_add(coeffs + (20 + n) * 16, vd + (n >> 1) * 4 * BPS + (n & 1) * 4, BPS);
+        transform_add(uv_transform(mb.tr_uv, n), coeffs + (16 + n) * 16, ud + (n >> 1) * 4 * BPS + (n & 1) * 4, BPS);
+        transform_add(uv_transform(mb.tr_uv, 4 + n), coeffs + (20 + n) * 16, vd + (n >> 1) * 4 * BPS + (n & 1) * 4, BPS);
     }
     for (int j = 0; j < 16; j++)
         for (int i = 0; i < 16; i++) py[j * ys + i] = yd[j * BPS + i];

@@ -199,7 +199,7 @@ __device__ void reconstruct_mb_warp(Vp8WarpSmem& sm, vp8::Work& w, int mb_x, int
         for (int n = 0; n < 16; n++) {
             uint8_t* d = yd + (n >> 2) * 4 * BPS + (n & 3) * 4;
             pred_4x4(d, BPS, mb.modes[n]);
-            if ((mb.nz_blocks >> n) & 1) inverse_dct_add(sm.coeffs + n * 16, d, BPS);
+            transform_add((mb.tr_y >> 2 * n) & 3, sm.coeffs + n * 16, d, BPS);
         }
     }
     // ---- chroma prediction: U on lanes 0..15, V on 16..31, 4 pixels each ----
@@ -219,14 +219,15 @@ __device__ void reconstruct_mb_warp(Vp8WarpSmem& sm, vp8::Work& w, int mb_x, int
     }
     __syncwarp();
     // ---- residuals: one 4x4 block per lane (i4x4 luma was added in order above) ----
-    if (lane < 24 && ((mb.nz_blocks >> lane) & 1) && !(mb.is_i4x4 && lane < 16)) {
+    if (lane < 24 && !(mb.is_i4x4 && lane < 16)) {
+        const int cls = lane < 16 ? (mb.tr_y >> 2 * lane) & 3 : uv_transform(mb.tr_uv, lane - 16);
         uint8_t* d;
         if (lane < 16) d = yd + (lane >> 2) * 4 * BPS + (lane & 3) * 4;
         else {
             const int n = lane & 3;
             d = (lane < 20 ? ud : vd) + (n >> 1) * 4 * BPS + (n & 1) * 4;
         }
-        inverse_dct_add(sm.coeffs + lane * 16, d, BPS);
+        transform_add(cls, sm.coeffs + lane * 16, d, BPS);
     }
     __syncwarp();
     // ---- store: luma row per lane 0..15, chroma row per lane 16..31 ----
