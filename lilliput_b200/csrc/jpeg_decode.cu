@@ -210,18 +210,33 @@ __global__ void __launch_bounds__(256) jpeg_rst_scan_kernel(JpegDecodeItem* item
     uint32_t* out = rst_all + it.state_off;  // (state_off doubles as the interval table offset of DRI images)
     const uint32_t cap = it.clean_len;       // intervals expected (set by the host); out has cap + 1 slots
     const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
+    __shared__ uint32_t s_end;
     if (tid == 0) {
         s_carry = 1;
         out[0] = 0;
+        s_end = len;
     }
     __syncthreads();
+    // The entropy-coded segment ends at the first marker that is not RSTn (EOI): bytes after it -- an appended preview
+    // or second frame with restart markers of its own -- are not part of this scan, as libjpeg-turbo reads it.  The
+    // tile that holds that marker drops the RSTn behind it and is the last one.
     for (uint32_t base = 0; base < len; base += 256 * 16) {
-        // 16 consecutive bytes per thread; marker = FF followed by D0..D7
+        // 16 consecutive bytes per thread; marker = FF followed by D0..D7, end = FF followed by anything but 00, FF, RSTn
         const uint32_t b0 = base + (uint32_t)tid * 16;
-        uint32_t found = 0;
+        uint32_t found = 0, my_end = 0xFFFFFFFFu;
         for (uint32_t k = 0; k < 16; k++) {
             const uint32_t i = b0 + k;
-            if (i + 1 < len && s[i] == 0xFF && (s[i + 1] & 0xF8) == 0xD0) found |= 1u << k;
+            if (i + 1 < len && s[i] == 0xFF) {
+                const uint32_t m = s[i + 1];
+                if ((m & 0xF8) == 0xD0) found |= 1u << k;
+                else if (m != 0x00 && m != 0xFF) my_end = min(my_end, i);
+            }
+        }
+        if (__syncthreads_or(my_end != 0xFFFFFFFFu)) {
+            if (my_end != 0xFFFFFFFFu) atomicMin(&s_end, my_end);
+            __syncthreads();
+            const uint32_t e = s_end;
+            found &= e <= b0 ? 0u : (e - b0 >= 16 ? 0xFFFFu : (1u << (e - b0)) - 1u);
         }
         const uint32_t cnt = __popc(found);
         uint32_t inc = cnt;
@@ -243,6 +258,7 @@ __global__ void __launch_bounds__(256) jpeg_rst_scan_kernel(JpegDecodeItem* item
         __syncthreads();
         if (tid == 255) s_carry = before + inc;
         __syncthreads();
+        if (s_end < len) break;  // (uniform: s_end last changed before the barriers above)
     }
     if (tid == 0) it.pad_ = s_carry;  // intervals found (markers + 1)
 }
