@@ -28,7 +28,8 @@ namespace lp {
 
 // Diagnostics: SM cycles (clock64, thread 0 of every CTA) spent in the phases of the sync kernels, summed over the
 // CTAs since the last reset: [0] table set-up, [1] guess pass, [2] synchronisation rounds, [3] prefix sum + write
-// pass, [4] DC pass, [5] CTAs.  Four clock reads and five atomics per CTA.
+// pass, [4] DC pass, [5] CTAs.  Four clock reads and five atomics per CTA.  Not cycles: [6] bits decoded in the
+// synchronisation rounds, [7] bits decoded in the guess pass (a shared-memory atomic per decode, two atomics per CTA).
 __device__ unsigned long long g_huff_phase[8];
 #define LP_PHASE_MARK(k)                                             \
     do {                                                             \
@@ -43,12 +44,16 @@ constexpr uint32_t kMinSubBits = 1024;  // shortest subsequence (bits); scratch 
 // Subsequences per thread and pass.  Synchronising the position inside the MCU (not just the
 // codeword boundary) takes several hundred symbols, so short subsequences need ~10 re-decode rounds;
 // sizing them so that one pass is exactly kSubPerThread full rounds of the CTA cuts that to ~2
-// (measured: 10.9 rounds at 1024 bits, 1.9 at one subsequence per thread).
+// (measured: 10.9 rounds at 1024 bits, 1.9 at one subsequence per thread of 512).
 constexpr uint32_t kSubPerThread = 1;
+// Threads (= subsequences per pass) of the sync kernel.  384 threads at 4 CTAs/SM keep as many threads per SM as 512
+// at 3 within the same 40 registers, and the longer subsequences (~9.3 kbit at 1080p) need fewer rounds (1.2 instead
+// of 1.9 at BASELINE config 2): measured 5 % less entropy-stage time on the H100 (DESIGN.md §5).
 #ifndef LP_HUFF_THREADS
-#define LP_HUFF_THREADS 512
+#define LP_HUFF_THREADS 384
 #endif
 constexpr int kHuffThreads = LP_HUFF_THREADS;
+constexpr int kUnstuffThreads = 512;  // the unstuff kernel: 8 KB tiles of 16-byte vectors
 
 __constant__ uint8_t c_zigzag_p[64] = {0,  1,  8,  16, 9,  2,  3,  10, 17, 24, 32, 25, 18, 11, 4,  5,
                                        12, 19, 26, 33, 40, 48, 41, 34, 27, 20, 13, 6,  7,  14, 21, 28,
@@ -93,11 +98,11 @@ __device__ __forceinline__ uint32_t block_excl_scan(uint32_t v, uint32_t* total,
 // tile, and the tile leaves as 4-byte words (stuffed bytes are ~0.4 % of the stream, so this is a
 // copy that occasionally closes a gap).  The marker search rides along: only the tile that holds
 // the marker pays for the second look.
-__global__ void __launch_bounds__(kHuffThreads)
+__global__ void __launch_bounds__(kUnstuffThreads)
     jpeg_unstuff_kernel(JpegDecodeItem* items, const uint8_t* scan, uint8_t* clean) {
-    __shared__ uint32_t warp_sums[kHuffThreads / 32];
+    __shared__ uint32_t warp_sums[kUnstuffThreads / 32];
     __shared__ uint32_t s_end;
-    __shared__ __align__(16) uint8_t stage[kHuffThreads * 16 + 16];
+    __shared__ __align__(16) uint8_t stage[kUnstuffThreads * 16 + 16];
     JpegDecodeItem& it = items[blockIdx.x];
     const uint8_t* src = scan + it.scan_off;
     const uint32_t len = it.scan_len;
@@ -116,7 +121,7 @@ __global__ void __launch_bounds__(kHuffThreads)
     const uint8_t* abase = src - mis;  // 16-byte aligned; the bytes before src belong to the same upload
     uint32_t carry = 0;
     uint32_t end = len;
-    constexpr uint32_t kTile = kHuffThreads * 16;
+    constexpr uint32_t kTile = kUnstuffThreads * 16;
     for (uint32_t t0 = 0; t0 < mis + end; t0 += kTile) {
         const uint32_t aoff = t0 + (uint32_t)tid * 16;      // offset from abase
         const int64_t i0 = (int64_t)aoff - (int64_t)mis;    // stream index of this thread's first byte
@@ -175,7 +180,7 @@ __global__ void __launch_bounds__(kHuffThreads)
         for (int k = 0; k < 16; k++) bsrc[k] = (uint8_t)(ws[k >> 2] >> (8 * (k & 3)));
         const uint32_t cnt = __popc(keep);
         uint32_t total;
-        const uint32_t ex = block_excl_scan<kHuffThreads>(cnt, &total, warp_sums);
+        const uint32_t ex = block_excl_scan<kUnstuffThreads>(cnt, &total, warp_sums);
         {
             uint32_t o = ex;
 #pragma unroll
@@ -189,7 +194,7 @@ __global__ void __launch_bounds__(kHuffThreads)
         const uint32_t nwords = (total - head) >> 2;
         const uint32_t tail0 = head + (nwords << 2);
         if ((uint32_t)tid < head) d[tid] = stage[tid];
-        for (uint32_t j = tid; j < nwords; j += kHuffThreads) {
+        for (uint32_t j = tid; j < nwords; j += kUnstuffThreads) {
             const uint8_t* q = stage + head + 4 * j;
             *reinterpret_cast<uint32_t*>(d + head + 4 * j) = (uint32_t)q[0] | ((uint32_t)q[1] << 8) | ((uint32_t)q[2] << 16) | ((uint32_t)q[3] << 24);
         }
@@ -199,7 +204,7 @@ __global__ void __launch_bounds__(kHuffThreads)
     }
     if (tid == 0) it.clean_len = carry;
     // zero padding so the 8-byte window loads past the end read defined data
-    for (uint32_t k = tid; k < 32; k += kHuffThreads) dst[carry + k] = 0;
+    for (uint32_t k = tid; k < 32; k += kUnstuffThreads) dst[carry + k] = 0;
 }
 
 // ------------------------------------------------------------------ 2. sync + write
@@ -493,9 +498,10 @@ __device__ __forceinline__ void dc_prefix_pass(const JpegDecodeItem& it, int16_t
     }
 }
 
-// 3 CTAs/SM (40 registers) measured faster than 4 at 32 registers (spills in the write pass) or 2 at 62
+// At 512 threads, 3 CTAs/SM (40 registers) measured faster than 4 at 32 registers (spills in the write pass) or 2 at
+// 62; at 384 threads, 4 CTAs/SM (40 registers) measured faster than 256 threads at 4 (62) or 5 (48) (DESIGN.md §5)
 #ifndef LP_HUFF_MIN_CTAS
-#define LP_HUFF_MIN_CTAS 3
+#define LP_HUFF_MIN_CTAS 4
 #endif
 __global__ void __launch_bounds__(kHuffThreads, LP_HUFF_MIN_CTAS)
     jpeg_huff_sync_kernel(JpegDecodeItem* items, const JpegHuffSet* tables, const uint8_t* clean,
@@ -509,6 +515,7 @@ __global__ void __launch_bounds__(kHuffThreads, LP_HUFF_MIN_CTAS)
     const int tid = threadIdx.x;
     if (it.status != 0 || it.restart_interval != 0 || it.nscans != 0) return;  // (DRI images: one thread per restart interval instead)
     __shared__ long long s_tphase;  // (shared, not a register pair every thread would carry through the loops)
+    __shared__ unsigned long long s_bits[2];  // diagnostics: bits decoded in the synchronisation rounds, in the guess pass
     if (tid == 0) s_tphase = clock64();
     // ---- build the per-CTA tables
     {
@@ -544,6 +551,7 @@ __global__ void __launch_bounds__(kHuffThreads, LP_HUFF_MIN_CTAS)
             hs.acb_rest = (uint32_t)__cvta_generic_to_shared(&hs.ac_look[hs.blk_ac[rest]][0]);
             s_status = 0;
             s_carry = 0;
+            s_bits[0] = s_bits[1] = 0;
         }
     }
     __syncthreads();
@@ -595,6 +603,7 @@ __global__ void __launch_bounds__(kHuffThreads, LP_HUFF_MIN_CTAS)
         uint32_t p = i * kSubBits, phase = 0, n = 0;
         const uint32_t limit = min((i + 1) * kSubBits, total_bits);
         decode_span<false>(hs, s, p, limit, total_bits, phase, n, nb, 0, 0, nullptr, nullptr, nullptr, nullptr);
+        atomicAdd(&s_bits[1], (unsigned long long)(p - i * kSubBits));
         st[i] = SubState{p, phase};
         ns[i] = n;
     }
@@ -621,7 +630,10 @@ __global__ void __launch_bounds__(kHuffThreads, LP_HUFF_MIN_CTAS)
             const SubState old = st[i];
             uint32_t p = in.p, phase = in.phase, n = 0;
             const uint32_t limit = min((i + 1) * kSubBits, total_bits);
-            if (p < limit) decode_span<false>(hs, s, p, limit, total_bits, phase, n, nb, 0, 0, nullptr, nullptr, nullptr, nullptr);
+            if (p < limit) {
+                decode_span<false>(hs, s, p, limit, total_bits, phase, n, nb, 0, 0, nullptr, nullptr, nullptr, nullptr);
+                atomicAdd(&s_bits[0], (unsigned long long)(p - in.p));
+            }
             ns[i] = n;  // slots consumed depend on the entry state even when the exit state does not
             if (p != old.p || phase != old.phase) {
                 // only an exit-state change can affect the right neighbour
@@ -637,7 +649,11 @@ __global__ void __launch_bounds__(kHuffThreads, LP_HUFF_MIN_CTAS)
         nxt_list = t;
         first_round = false;
     }
-    if (tid == 0) it.pad_ = rounds;  // diagnostics: synchronisation rounds this image needed
+    if (tid == 0) {
+        it.pad_ = rounds;  // diagnostics: synchronisation rounds this image needed
+        atomicAdd(&g_huff_phase[6], s_bits[0]);
+        atomicAdd(&g_huff_phase[7], s_bits[1]);
+    }
     LP_PHASE_MARK(2);
     SubState* cur = st;
     // ---- prefix sum of slot counts, then the writing decode.  Every thread learns each tile's total
@@ -702,7 +718,7 @@ int jpeg_huff_parallel_slots() {
 int jpeg_huff_parallel_launch(const JpegHuffParallelArgs& a, cudaStream_t st) {
     if (a.n <= 0) return LP_OK;
     static const uint32_t spt = getenv("LP_HUFF_SPT") ? (uint32_t)atoi(getenv("LP_HUFF_SPT")) : kSubPerThread;
-    jpeg_unstuff_kernel<<<a.n, kHuffThreads, 0, st>>>(a.items, a.scan, a.clean);
+    jpeg_unstuff_kernel<<<a.n, kUnstuffThreads, 0, st>>>(a.items, a.scan, a.clean);
     g_launches++;
     LP_CUDA_OK(cudaGetLastError());
     jpeg_huff_sync_kernel<<<a.n, kHuffThreads, 0, st>>>(a.items, a.tables, a.clean,
