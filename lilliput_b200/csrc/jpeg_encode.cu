@@ -5,7 +5,7 @@
 // Replaces: opencv_encoder_write for ".jpeg"/".jpg" (ref opencv.cpp:185-194), i.e. what
 // cv::ImageEncoder::write asks of libjpeg-turbo 3.1.0 defaults.  Arithmetic and bitstream
 // contract: SURVEY.md Appendix E.3; output is BYTE-IDENTICAL to the reference's
-// (tests/test_jpeg_encode_gpu.py).
+// (tests/test_gpu_jpeg_encode.py, against libjpeg-turbo through cv2).
 //
 // Kernels:
 //   jpeg_fdct_quant_kernel   one thread per 8x8 block (4 Y + Cb + Cr per MCU): colour convert

@@ -9,7 +9,7 @@
  * optimisation.  Restated from ITU-T T.81 and libjpeg-turbo's published
  * jccolor.c / jcsample.c / jfdctint.c / jcdctmgr.c / jccoefct.c / jchuff.c /
  * jcmarker.c as summarised in SURVEY.md Appendix E.3.
- * Pinned byte-for-byte against oracle/_ref in tests/test_oracle_jpeg.py.
+ * Pinned byte-for-byte against libjpeg-turbo (through cv2) in tests/test_oracle_jpeg_encode.py.
  */
 #include <stdlib.h>
 #include <string.h>
