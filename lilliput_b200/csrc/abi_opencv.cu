@@ -176,10 +176,12 @@ static int decode_jpeg_into(const Decoder* d, Mat* m) {
         fprintf(stderr, "[lilliput_b200] JPEG variant not supported on the device path (sampling layout)\n");
         return LP_ERR_UNSUPPORTED;
     }
-    // multi-scan files (progressive, or one scan per component): the scans and the tables in force
+    // The Huffman tables in force and, for the files one thread walks scan by scan (jpeg_multiscan_kernel), the scans:
+    // multi-scan files (progressive, or one scan per component) and baseline files with restart markers.  Other
+    // baseline files go to the self-synchronising parallel decoder.
     std::vector<JpegScanDesc> scans;
-    std::vector<JpegHuffSet> sets;
-    int nscans = 0, nsets = 0;
+    std::vector<JpegHuffSet> sets(1);
+    int nscans = 0, nsets = 1;
     if (h.multiscan) {
         scans.resize(kMultiscanMaxScans);
         sets.resize(kMultiscanMaxSets);
@@ -192,7 +194,15 @@ static int decode_jpeg_into(const Decoder* d, Mat* m) {
                     visits, nscans);
             return LP_ERR_UNSUPPORTED;
         }
+    } else {
+        jpeg_build_huff_set(h, &sets[0]);
+        if (h.restart_interval) {  // one scan visits every block once, so no visit budget: any size decodes
+            scans.resize(1);
+            jpeg_baseline_scan(h, &scans[0]);
+            nscans = 1;
+        }
     }
+    const bool parallel = nscans == 0;
     cudaStream_t st = thread_stream();
     JpegDecodeItem it;
     memset(&it, 0, sizeof(it));
@@ -218,22 +228,19 @@ static int decode_jpeg_into(const Decoder* d, Mat* m) {
     }
     uint32_t tiles = 0;
     const uint32_t blocks = jpeg_item_set_window(&it, 0, 0, h.width, h.height, false, &tiles);  // whole image
-    if (h.multiscan) {  // its scans are [0, nscans) of d_scans; the whole frame is the window, so no masks
+    if (!parallel) {  // its scans are [0, nscans) of d_scans; the whole frame is the window, so no masks
         it.restart_interval = 0;
         it.table_set = 0;
         it.nscans = (uint32_t)nscans;
     }
     it.frame_channels = h.ncomp == 1 ? 1 : 3;
-    JpegHuffSet hs;
-    jpeg_build_huff_set(h, &hs);
 
     uint8_t* scratch = nullptr;
-    const size_t upload_len = h.multiscan ? d->len : h.scan_length;  // multi-scan: the whole file
+    const size_t upload_len = parallel ? h.scan_length : d->len;  // walked scan by scan: the whole file
     const size_t scan_bytes = round_up(upload_len + 16, (size_t)256);
-    const size_t sets_b = round_up(sizeof(JpegHuffSet) * (size_t)(h.multiscan ? nsets : 1), (size_t)256);
+    const size_t sets_b = round_up(sizeof(JpegHuffSet) * (size_t)nsets, (size_t)256);
     const size_t scans_b = round_up(sizeof(JpegScanDesc) * (size_t)nscans + 16, (size_t)256);
     const size_t coef_bytes = round_up((size_t)blocks * 64 * sizeof(int16_t), (size_t)256);
-    const bool parallel = h.restart_interval == 0 && !h.multiscan;
     const size_t clean_b = parallel ? round_up(huff_clean_bytes(h.scan_length), (size_t)256) : 0;
     const size_t states_b = parallel ? round_up(2 * huff_nsub(h.scan_length) * 8, (size_t)256) : 0;
     const size_t nslots_b = parallel ? round_up(2 * huff_nsub(h.scan_length) * 4, (size_t)256) : 0;
@@ -251,13 +258,12 @@ static int decode_jpeg_into(const Decoder* d, Mat* m) {
     uint8_t* d_dcdiff = d_nslots + nslots_b;
     JpegScanDesc* d_scans = reinterpret_cast<JpegScanDesc*>(d_dcdiff + dcdiff_b);
     LP_CUDA_OK(cudaMemcpyAsync(d_item, &it, sizeof(it), cudaMemcpyHostToDevice, st));
-    if (h.multiscan) {
-        LP_CUDA_OK(cudaMemcpyAsync(d_hs, sets.data(), sizeof(JpegHuffSet) * nsets, cudaMemcpyHostToDevice, st));
+    LP_CUDA_OK(cudaMemcpyAsync(d_hs, sets.data(), sizeof(JpegHuffSet) * nsets, cudaMemcpyHostToDevice, st));
+    if (parallel) {
+        LP_CUDA_OK(cudaMemcpyAsync(d_scan, d->data + h.scan_offset, h.scan_length, cudaMemcpyHostToDevice, st));
+    } else {
         LP_CUDA_OK(cudaMemcpyAsync(d_scans, scans.data(), sizeof(JpegScanDesc) * nscans, cudaMemcpyHostToDevice, st));
         LP_CUDA_OK(cudaMemcpyAsync(d_scan, d->data, d->len, cudaMemcpyHostToDevice, st));
-    } else {
-        LP_CUDA_OK(cudaMemcpyAsync(d_hs, &hs, sizeof(hs), cudaMemcpyHostToDevice, st));
-        LP_CUDA_OK(cudaMemcpyAsync(d_scan, d->data + h.scan_offset, h.scan_length, cudaMemcpyHostToDevice, st));
     }
     JpegDecodeBatch b;
     b.items = d_item;
@@ -266,14 +272,12 @@ static int decode_jpeg_into(const Decoder* d, Mat* m) {
     b.coef = d_coef;
     b.frames = m->dptr();
     b.n = 1;
-    b.coef_elems_total = (size_t)blocks * 64;
     b.max_tiles_per_image = (int)tiles;
-    b.use_parallel_huffman = parallel;
     b.clean = d_clean;
     b.states = d_states;
     b.nslots = reinterpret_cast<uint32_t*>(d_nslots);
     b.dcdiff = reinterpret_cast<int16_t*>(d_dcdiff);
-    if (h.multiscan) {
+    if (!parallel) {
         b.n_multiscan = 1;
         b.scans = d_scans;
     }

@@ -126,7 +126,6 @@ struct lp_batch {
     std::vector<OrientJob> jobs;
     std::vector<int> index;
     size_t dev_off = 0, clean_off = 0, state_off = 0;
-    bool parallel_huffman = true;
     uint8_t* h_out = nullptr;       // pinned + device-mapped: the compaction kernel writes the encoded bytes straight into it
     uint32_t* h_out_len = nullptr;  // pinned
     unsigned long long* h_off = nullptr;  // pinned + device-mapped: packed offsets, (cnt + 1) per chunk at [i0 + chunk ordinal]
@@ -422,7 +421,6 @@ static void batch_begin(lp_batch* b, int n) {
     b->scans.clear();
     b->scans_uploaded = 0;
     b->dev_off = b->clean_off = b->state_off = 0;
-    b->parallel_huffman = true;
     for (auto& kv : b->chunk_layout)
         if (kv.second.d_rst_work) cudaFreeAsync(kv.second.d_rst_work, b->st);
     b->chunk_layout.clear();
@@ -722,10 +720,8 @@ static int batch_launch_chunk(lp_batch* b, int i0, int cnt, cudaStream_t st, cud
     d.coef = b->d_coef;
     d.frames = b->d_frames;
     d.n = cnt;
-    d.coef_elems_total = (size_t)cnt * lay.blocks * 64;
     d.max_tiles_per_image = (int)lay.tiles;
     d.dcdiff = b->d_dcdiff;
-    d.use_parallel_huffman = b->parallel_huffman;
     d.clean = b->d_clean;
     d.states = b->d_states;
     d.nslots = b->d_nslots;

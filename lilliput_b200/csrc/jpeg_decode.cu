@@ -7,15 +7,16 @@
 // bit-identical to the reference on baseline streams (tests/test_jpeg_decode_gpu.py).
 //
 // Kernels (each one grid launch over the whole batch):
-//   jpeg_huff_decode_kernel   entropy-coded segment -> quantised coefficients (int16, natural
-//                             order, zero-initialised buffer).  Bit-serial by nature; this
-//                             first version runs one stream per thread.
-//   jpeg_multiscan_kernel     progressive / one-scan-per-component files: one warp per item clears its blocks, one
-//                             thread walks its scans (jpeg_scan_core.h); scan-order blocks like the parallel path.
+//   jpeg_rst_*_kernel         lp_batch's scans with restart markers: one thread per restart interval.
+//   jpeg_multiscan_kernel     progressive / one-scan-per-component files, and per image a baseline scan with restart
+//                             markers: one warp per item clears its blocks, one thread walks its scans
+//                             (jpeg_scan_core.h).
 //   jpeg_idct_color_kernel    one CTA per tile of MCU rows x columns: dequantise + IDCT (one thread
 //                             per 8x8 block, two 1-D passes in registers) into shared-memory
 //                             component rows, then triangle upsampling + fixed-point colour
 //                             conversion from there into the packed BGR frame.
+// Scans without restart markers go to the self-synchronising decoder (jpeg_huff_parallel.cu).  Every entropy decoder
+// writes quantised coefficients (int16, natural order) in scan order and clears the blocks it writes.
 #include "common.cuh"
 #include "kernels.cuh"
 #include "jpeg_scan_core.h"
@@ -98,12 +99,7 @@ uint32_t jpeg_item_set_window(JpegDecodeItem* it, int x0, int y0, int x1, int y1
     it->roi_mcx = px1 / mw - it->roi_mx0 + 1;
     it->roi_mcy = py1 / mh - it->roi_my0 + 1;
     uint32_t blocks = 0;
-    for (int c = 0; c < it->ncomp; c++) {
-        it->bw[c] = it->roi_mcx * it->h[c];
-        it->bh[c] = it->roi_mcy * it->v[c];
-        it->block_off[c] = blocks;
-        blocks += (uint32_t)it->bw[c] * it->bh[c];
-    }
+    for (int c = 0; c < it->ncomp; c++) blocks += (uint32_t)(it->roi_mcx * it->h[c]) * (uint32_t)(it->roi_mcy * it->v[c]);
     // Tiles: spans as wide as the shared-memory budget allows, evened out over the ROI width, and four bands of
     // MCU rows so that an image gives several CTAs.
     const int mcx = it->roi_mcx > 0 ? it->roi_mcx : 1, mcy = it->roi_mcy > 0 ? it->roi_mcy : 1;
@@ -114,81 +110,6 @@ uint32_t jpeg_item_set_window(JpegDecodeItem* it, int x0, int y0, int x1, int y1
     it->tile_mcy = (mcy + 3) / 4;
     if (tiles_out) *tiles_out = (uint32_t)(it->tiles_x * ((mcy + it->tile_mcy - 1) / it->tile_mcy));
     return blocks;
-}
-
-// Coefficient block of component c at full-image block position (X, Y); nullptr outside the ROI.
-__device__ __forceinline__ int16_t* roi_block(const JpegDecodeItem& it, int16_t* coef, int c, int X, int Y) {
-    const int rx = X - it.roi_mx0 * it.h[c], ry = Y - it.roi_my0 * it.v[c];
-    if (rx < 0 || ry < 0 || rx >= it.bw[c] || ry >= it.bh[c]) return nullptr;
-    return coef + it.coef_off + ((size_t)it.block_off[c] + (size_t)ry * it.bw[c] + rx) * 64;
-}
-
-// ------------------------------------------------------------------ entropy decode (serial)
-
-__global__ void jpeg_huff_decode_kernel(JpegDecodeItem* items, const JpegHuffSet* tables,
-                                        const uint8_t* scan, int16_t* coef, int n) {
-    __shared__ uint8_t zz[64];
-    for (int k = threadIdx.x; k < 64; k += blockDim.x) zz[k] = c_zigzag[k];
-    __syncthreads();
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    JpegDecodeItem& it = items[i];
-    const JpegHuffSet* hs = tables + it.table_set;
-    BitReader b{scan + it.scan_off, scan + it.scan_off + it.scan_len, 0, 0, false};
-    int pred[3] = {0, 0, 0};
-    int todo = it.restart_interval;
-    int status = 0;
-    const int nc = it.ncomp;
-    for (int my = 0; my < it.mcus_y && status == 0; my++) {
-        for (int mx = 0; mx < it.mcus_x && status == 0; mx++) {
-            if (it.restart_interval && todo == 0) {
-                // byte-align, skip to just past the next RSTn, reset predictors
-                b.acc = 0;
-                b.nbits = 0;
-                const uint8_t* q = b.p;
-                while (q + 1 < b.end && !(q[0] == 0xFF && q[1] >= 0xD0 && q[1] <= 0xD7)) q++;
-                if (q + 1 >= b.end) {
-                    status = -3;
-                    break;
-                }
-                b.p = q + 2;
-                b.marker = false;
-                pred[0] = pred[1] = pred[2] = 0;
-                todo = it.restart_interval;
-            }
-            for (int c = 0; c < nc && status == 0; c++) {
-                const int td = it.td[c], ta = 4 + it.ta[c];
-                for (int by = 0; by < it.v[c] && status == 0; by++) {
-                    for (int bx = 0; bx < it.h[c]; bx++) {
-                        const int X = mx * it.h[c] + bx, Y = my * it.v[c] + by;
-                        int16_t* blk = roi_block(it, coef, c, X, Y);  // nullptr: decode but do not store
-                        int s = huff_symbol(b, hs, td);
-                        if (s < 0 || s > 15) { status = -3; break; }
-                        if (s) pred[c] += receive_extend(b, s);
-                        if (blk) blk[0] = (int16_t)pred[c];
-                        for (int k = 1; k < 64;) {
-                            const int rs = huff_symbol(b, hs, ta);
-                            if (rs < 0) { status = -3; break; }
-                            const int r = rs >> 4, sz = rs & 15;
-                            if (sz == 0) {
-                                if (r != 15) break;
-                                k += 16;
-                                continue;
-                            }
-                            k += r;
-                            if (k > 63) { status = -3; break; }
-                            const int val = receive_extend(b, sz);
-                            if (blk) blk[zz[k]] = (int16_t)val;
-                            k++;
-                        }
-                        if (status) break;
-                    }
-                }
-            }
-            if (it.restart_interval) todo--;
-        }
-    }
-    it.status = status;
 }
 
 // ------------------------------------------------------------------ restart-interval-parallel decode
@@ -345,6 +266,8 @@ int jpeg_rst_launch(JpegDecodeItem* items, const JpegHuffSet* tables, const uint
 }
 
 // ------------------------------------------------------------------ multi-scan files (serial per image)
+// Per image, a baseline scan with restart markers runs here too, as one sequential scan: the walk takes the next RSTn
+// whatever its number, where jpeg_rst_decode_kernel refuses markers out of sequence.
 // One CTA of one warp per item; items that are not multi-scan return at once.  The warp clears the item's ROI
 // blocks (and, for a window smaller than the frame, its nonzero masks), then lane 0 walks every scan
 // (jpeg_scan_core.h).  Refinement scans carry no restart-free synchronisation point the way a baseline scan does
@@ -481,12 +404,10 @@ __device__ __forceinline__ int tile_row(const TileCtx& t, int c, int cy) {
 }
 
 // Dequantise + IDCT ROI MCU row m_ring of the ring components and m_flat of the others (-1: none) over the
-// tile's columns into shared memory, one thread per block.  The serial baseline decoder stores blocks per
-// component in raster order; the parallel and multi-scan decoders store them in scan order (jpeg_huff_parallel.cu):
-// block (X % h, Y % v) of component c inside ROI MCU (X / h, Y / v).
+// tile's columns into shared memory, one thread per block.  The entropy decoders store blocks in scan order
+// (jpeg_huff_parallel.cu): block (X % h, Y % v) of component c inside ROI MCU (X / h, Y / v).
 __device__ __forceinline__ void idct_phase(const JpegDecodeItem& it, const TileCtx& t, const int16_t* coef,
-                                           int mcu_order, const uint16_t (*qt)[64], uint8_t* tile, int m_flat,
-                                           int m_ring) {
+                                           const uint16_t (*qt)[64], uint8_t* tile, int m_flat, int m_ring) {
     int end[3];
     int total = 0;
 #pragma unroll
@@ -503,9 +424,7 @@ __device__ __forceinline__ void idct_phase(const JpegDecodeItem& it, const TileC
         const int per = t.nc[c] * h;  // blocks per block row
         const int by = k / per, bx = k - by * per;
         const int X = t.ca[c] * h + bx;  // ROI block column
-        const size_t sblk = mcu_order
-                                ? ((size_t)m * it.roi_mcx + X / h) * t.nb + t.kfirst[c] + by * h + X % h
-                                : (size_t)it.block_off[c] + (size_t)(m * vs + by) * it.bw[c] + X;
+        const size_t sblk = ((size_t)m * it.roi_mcx + X / h) * t.nb + t.kfirst[c] + by * h + X % h;
         const uint4* src = reinterpret_cast<const uint4*>(coef + it.coef_off + sblk * 64);
         const uint4* q4 = reinterpret_cast<const uint4*>(qt[c]);
         int v[64];
@@ -708,7 +627,7 @@ __device__ __forceinline__ void color_phase(const JpegDecodeItem& it, const Tile
 }
 
 __global__ void __launch_bounds__(kIdctColorThreads, 5)
-    jpeg_idct_color_kernel(const JpegDecodeItem* items, const int16_t* coef, uint8_t* frames, int mcu_order) {
+    jpeg_idct_color_kernel(const JpegDecodeItem* items, const int16_t* coef, uint8_t* frames) {
     const JpegDecodeItem& it = items[blockIdx.y];
     if (it.status != 0) return;
     const int band = (int)blockIdx.x / it.tiles_x, span = (int)blockIdx.x - band * it.tiles_x;
@@ -751,10 +670,10 @@ __global__ void __launch_bounds__(kIdctColorThreads, 5)
                       it.h[2] == 1 && it.v[2] == 1 && (it.width & 15) == 0 && (it.win_x0 & 15) == 0 &&
                       (it.win_w & 15) == 0 && (it.win_stride & 15) == 0 && (it.frame_off & 15) == 0;
     // the ring's rows above the band and the band's first row
-    if (m0 > 0) idct_phase(it, t, coef, mcu_order, s_qt, s_tile, -1, m0 - 1);
-    idct_phase(it, t, coef, mcu_order, s_qt, s_tile, -1, m0);
+    if (m0 > 0) idct_phase(it, t, coef, s_qt, s_tile, -1, m0 - 1);
+    idct_phase(it, t, coef, s_qt, s_tile, -1, m0);
     for (int m = m0; m < m1; m++) {
-        idct_phase(it, t, coef, mcu_order, s_qt, s_tile, m, m + 1 < it.roi_mcy ? m + 1 : -1);
+        idct_phase(it, t, coef, s_qt, s_tile, m, m + 1 < it.roi_mcy ? m + 1 : -1);
         __syncthreads();
         color_phase(it, t, s_tile, frames, m, c0, c1, maxh, maxv, fast);
         __syncthreads();
@@ -765,26 +684,17 @@ __global__ void __launch_bounds__(kIdctColorThreads, 5)
 
 int jpeg_decode_launch(const JpegDecodeBatch& b, cudaStream_t st, cudaEvent_t ev_after_huff) {
     if (b.n <= 0) return LP_OK;
-    if (b.use_parallel_huffman) {
-        // The parallel decoders (self-synchronising and restart-interval) clear every block of the region of
-        // interest themselves as they open it, so their array is not cleared: at 4096 1080p images a memset
-        // alone would write 15 GB per batch.  Blocks of an image that fails are not read.  Both skip multi-scan
-        // items.
+    // Every decoder clears the blocks of the region of interest itself as it opens them, so the coefficient array is
+    // not cleared: at 4096 1080p images a memset alone would write 15 GB per batch.  Blocks of an image that fails
+    // are not read.
+    if (b.n_multiscan < b.n) {  // the self-synchronising and restart-interval decoders skip multi-scan items
         JpegHuffParallelArgs a{b.items, b.tables, b.scan, b.clean, b.states, b.nslots, b.coef, b.dcdiff, b.n};
         int rc = jpeg_huff_parallel_launch(a, st);  // skips the images that carry restart markers
         if (rc) return rc;
         rc = jpeg_rst_launch(b.items, b.tables, b.scan, b.nslots, b.rst_work, b.n_rst_work, b.n, b.coef, st);
         if (rc) return rc;
-    } else if (b.n_multiscan < b.n) {
-        // the serial decoder stores only the nonzero coefficients of a zeroed array
-        LP_CUDA_OK(cudaMemsetAsync(b.coef, 0, b.coef_elems_total * sizeof(int16_t), st));
-        const int threads = 32;
-        jpeg_huff_decode_kernel<<<ceil_div(b.n, threads), threads, 0, st>>>(b.items, b.tables, b.scan,
-                                                                           b.coef, b.n);
-        g_launches++;
-        LP_CUDA_OK(cudaGetLastError());
     }
-    if (b.n_multiscan > 0) {  // clears its own blocks
+    if (b.n_multiscan > 0) {
         jpeg_multiscan_kernel<<<b.n, kMultiscanThreads, 0, st>>>(b.items, b.scans, b.tables, b.scan, b.coef, b.masks);
         g_launches++;
         LP_CUDA_OK(cudaGetLastError());
@@ -792,8 +702,7 @@ int jpeg_decode_launch(const JpegDecodeBatch& b, cudaStream_t st, cudaEvent_t ev
     if (ev_after_huff) LP_CUDA_OK(cudaEventRecord(ev_after_huff, st));
     if (b.max_tiles_per_image > 0) {
         const dim3 grid((unsigned)b.max_tiles_per_image, b.n);
-        const int mcu_order = b.use_parallel_huffman || b.n_multiscan > 0;
-        jpeg_idct_color_kernel<<<grid, kIdctColorThreads, kTileSmemBytes, st>>>(b.items, b.coef, b.frames, mcu_order);
+        jpeg_idct_color_kernel<<<grid, kIdctColorThreads, kTileSmemBytes, st>>>(b.items, b.coef, b.frames);
         g_launches++;
         LP_CUDA_OK(cudaGetLastError());
     }

@@ -392,6 +392,20 @@ int jpeg_parse_scans(const uint8_t* in, size_t len, const JpegHeader& h, JpegSca
     return rc;
 }
 
+void jpeg_baseline_scan(const JpegHeader& h, JpegScanDesc* out) {
+    memset(out, 0, sizeof(*out));
+    out->data_off = (uint32_t)h.scan_offset;
+    out->data_len = (uint32_t)h.scan_length;
+    out->ns = h.ncomp;
+    for (int i = 0; i < h.ncomp; i++) {
+        out->ci[i] = i;
+        out->td[i] = h.comp[i].td;
+        out->ta[i] = h.comp[i].ta;
+    }
+    out->Se = 63;
+    out->restart_interval = h.restart_interval;
+}
+
 size_t jpeg_multiscan_visits(const JpegHeader& h, const JpegScanDesc* scans, int nscans) {
     size_t visits = 0;
     for (int k = 0; k < nscans; k++)

@@ -5,10 +5,11 @@
 // progressive (T.81 Annex G; libjpeg-turbo's jdphuff.c is what the reference runs) or sequential with one scan per
 // component -- by walking its scans in order: every scan refines the same coefficients, and inside a scan the
 // end-of-band runs chain across blocks, so one thread walks one image.  Restated in oracle/oracle_jpeg_dec.c
-// (prog_*), which is pinned on the reference.
+// (prog_*), which is pinned on the reference.  The per-image decode also walks a baseline file with restart markers
+// here, as one sequential scan (jpeg_baseline_scan).
 //
-// Coefficients go to the scan order of the parallel decoders ([roi MCU][block in MCU], jpeg_huff_parallel.cu), so
-// jpeg_idct_color_kernel reads every kind of file with mcu_order = 1.  Only blocks inside the region of interest
+// Coefficients go to the scan order of the parallel decoders ([roi MCU][block in MCU], jpeg_huff_parallel.cu), which
+// jpeg_idct_color_kernel reads for every kind of file.  Only blocks inside the region of interest
 // keep coefficients.  An AC refinement scan reads one correction bit for every coefficient of its band that is
 // already nonzero, and its zero runs skip those coefficients, so a block outside the region keeps a 64-bit mask of
 // its nonzero coefficients (bit k = zigzag position k) instead: 8 bytes where the coefficients would take 128.  DC

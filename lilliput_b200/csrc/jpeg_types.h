@@ -28,9 +28,7 @@ struct JpegDecodeItem {
     int32_t width, height, ncomp;
     int32_t mcus_x, mcus_y, restart_interval;
     int32_t h[3], v[3];   // sampling factors
-    int32_t bw[3], bh[3]; // blocks per component plane (padded to the MCU grid)
     int32_t dw[3], dh[3]; // true downsampled component size in samples
-    uint32_t block_off[3];  // first block of component c inside the image's coef area
     // tiles of jpeg_idct_color_kernel (one CTA each): tiles_x spans of tile_mcx ROI MCU columns, bands of tile_mcy
     // ROI MCU rows
     int32_t tile_mcx, tile_mcy, tiles_x;
@@ -46,14 +44,15 @@ struct JpegDecodeItem {
     uint32_t clean_len;     // written by jpeg_unstuff_kernel
     uint32_t pad_;
     // Region of interest.  Only MCUs [roi_mx0, roi_mx0+roi_mcx) x [roi_my0, roi_my0+roi_mcy) get
-    // coefficients (bw, bh, block_off describe THAT grid); the packed frame holds
+    // coefficients, in scan order ([roi MCU][block in MCU]); the packed frame holds
     // the pixel window [win_x0, win_x0+win_w) x [win_y0, win_y0+win_h) with rows win_stride apart.
     // A full decode has roi = every MCU and win = the whole image.
     int32_t roi_mx0, roi_my0, roi_mcx, roi_mcy;
     int32_t win_x0, win_y0, win_w, win_h;
     uint32_t win_stride;
-    uint32_t nscans;        // 0: one interleaved scan.  > 0: multi-scan file, decoded by jpeg_multiscan_kernel from
-                            // its scans [table_set, table_set + nscans); the parallel and serial passes skip it
+    uint32_t nscans;        // 0: one interleaved scan.  > 0: decoded by jpeg_multiscan_kernel from its scans
+                            // [table_set, table_set + nscans), which the parallel passes skip: a multi-scan file, or
+                            // per image a baseline file with restart markers (one scan)
 };
 
 // Huffman decode tables for one image (or many images sharing them), device format.

@@ -79,6 +79,10 @@ int jpeg_parse_scans(const uint8_t* data, size_t len, const JpegHeader& h, JpegS
 // The same, with the sets built into device-format tables.
 int jpeg_parse_scans(const uint8_t* data, size_t len, const JpegHeader& h, JpegScanDesc* scans, int max_scans,
                      int* nscans, JpegHuffSet* sets, int max_sets, int* nsets);
+// The one interleaved scan of a `supported` header as a multi-scan descriptor, tables jpeg_build_huff_set(h) as set 0.
+// Its bytes are the header's extent, up to the last EOI, where jpeg_parse_scans' stops at the first marker that is not
+// RSTn: the per-image decode's search for the next RSTn (br_restart) may look past a first EOI.
+void jpeg_baseline_scan(const JpegHeader& h, JpegScanDesc* out);
 // Per-file caps of jpeg_parse_scans' arrays, and the work budget of the serial multi-scan decoder: one thread
 // walks every block of every scan, so a hostile file (up to 256 scans over a large frame) is refused rather than
 // queued.  Real progressive files have ~10 scans; an 8192 x 8192 4:4:4 frame with 20 scans still passes.
@@ -94,10 +98,8 @@ struct JpegDecodeBatch {
     int16_t* coef;              // device
     uint8_t* frames;            // device, packed BGR / gray frames
     int n;
-    size_t coef_elems_total;    // for the memset
     int max_tiles_per_image;    // largest *tiles of jpeg_item_set_window over the batch
-    // parallel Huffman scratch (all device); used when use_parallel_huffman is set
-    bool use_parallel_huffman = false;
+    // parallel Huffman scratch (all device); used when the batch holds a single-scan item
     uint8_t* clean = nullptr;
     void* states = nullptr;      // SubState[]
     uint32_t* nslots = nullptr;
@@ -134,7 +136,7 @@ int jpeg_huff_parallel_launch(const JpegHuffParallelArgs& a, cudaStream_t st);
 int jpeg_huff_parallel_slots();
 // Diagnostics: clock64 cycles per phase of the sync kernels summed over CTAs (see jpeg_huff_parallel.cu)
 int jpeg_huff_phase_clocks(unsigned long long out[8], int reset);
-// Launches: memset(coef) -> huffman decode -> fused idct + upsample + colour.
+// Launches: huffman decode (each decoder clears the blocks it writes) -> fused idct + upsample + colour.
 int jpeg_decode_launch(const JpegDecodeBatch& b, cudaStream_t st, cudaEvent_t ev_after_huff);
 
 // ---- png_parse.cpp (host) / png_decode.cu ------------------------------------------------------

@@ -33,7 +33,7 @@ SAMPLINGS = {
 COLOR_SAMPLINGS = ("444", "422", "420", "411", "440")
 CONTENTS = ("noise", "smooth", "blocks")
 # plain = Huffman tables of Annex K, optimized = per-file tables, rstN = a restart interval of N MCUs, rstrow = one
-# MCU row; progressive files go through the multi-scan decoder, restart files through the serial one
+# MCU row; per image, progressive and restart files go through the multi-scan decoder
 MODES = ("plain", "optimized", "rst1", "rst3", "rstrow", "progressive")
 
 

@@ -1,6 +1,7 @@
 // Host build of lilliput_b200/csrc/jpeg_scan_core.h (multi-scan JPEG entropy decoding) for the CPU suite.  It runs
 // exactly the per-image walk jpeg_multiscan_kernel runs on the device, for a region of interest given in MCUs: the
-// ROI's coefficient blocks in scan order ([roi MCU][block in MCU]) and, outside the ROI, the nonzero masks.
+// ROI's coefficient blocks in scan order ([roi MCU][block in MCU]) and, outside the ROI, the nonzero masks.  It takes
+// multi-scan files and baseline files with restart markers (one scan, the per-image decode's route for them).
 // tests/test_jpeg_scan_streams.py compares a windowed decode with the whole-frame decode cut to the window.
 #include <cstring>
 #include <vector>
@@ -16,18 +17,25 @@ static const uint8_t kZigzag[64] = {0,  1,  8,  16, 9,  2,  3,  10, 17, 24, 32, 
 
 // info[0..3] = mcus_x, mcus_y, blocks per MCU, block visits.  roi = (mx0, my0, mcx, mcy) in MCUs; mcx = 0: the whole
 // frame.  out: roi blocks * 64 int16.  Returns the decoder's status (0, -3), or a negative lp_status from parsing,
-// or 1 when `cap` is too small.
+// -8 for a file of neither kind, or 1 when `cap` is too small.
 extern "C" int jscan_decode(const uint8_t* file, long len, const int* roi, int16_t* out, long cap, int* info) {
     lp::JpegHeader h;
     int rc = lp::jpeg_parse_header(file, (size_t)len, &h);
     if (rc) return rc;
-    if (!h.multiscan) return -8;
     std::vector<lp::JpegScanDesc> scans(lp::kMultiscanMaxScans);
     std::vector<lp::JpegHuffSet> sets(lp::kMultiscanMaxSets);
     int nscans = 0, nsets = 0;
-    rc = lp::jpeg_parse_scans(file, (size_t)len, h, scans.data(), (int)scans.size(), &nscans, sets.data(), (int)sets.size(),
-                              &nsets);
-    if (rc) return rc;
+    if (h.multiscan) {
+        rc = lp::jpeg_parse_scans(file, (size_t)len, h, scans.data(), (int)scans.size(), &nscans, sets.data(),
+                                  (int)sets.size(), &nsets);
+        if (rc) return rc;
+    } else if (h.supported && h.restart_interval) {  // a baseline file with restart markers, as decode_jpeg_into walks it
+        lp::jpeg_baseline_scan(h, &scans[0]);
+        lp::jpeg_build_huff_set(h, &sets[0]);
+        nscans = nsets = 1;
+    } else {
+        return -8;
+    }
     lp::JpegDecodeItem it;
     memset(&it, 0, sizeof(it));
     it.width = h.width;

@@ -145,7 +145,7 @@ def test_batch_mixed_sampling_layouts_in_any_order(cuda_lib, oracle):
 
 def test_batch_restart_interval_streams_decode_in_parallel(cuda_lib, oracle):
     """DRI streams (one thread per restart interval) next to plain ones (self-synchronising decoder) in ONE batch:
-    the kernel is chosen per image, outputs == lp_transform (which the serial per-image kernel decodes)."""
+    the kernel is chosen per image, outputs == lp_transform (which walks DRI streams with the multi-scan kernel)."""
     cv2 = pytest.importorskip("cv2")
     w, h = 480, 272
     opt = abi.ImageOptions(FileType=".jpeg", Width=96, Height=96, ResizeMethod=abi.ImageOpsFit,

@@ -1,7 +1,8 @@
 """GPU: the baseline JPEG streams of tests/jpeg_baseline_streams.py through the three device entropy decoders.
 
 Per image (lp_decode_host), a scan without restart markers runs on the self-synchronising parallel decoder and a DRI
-scan on the serial one; in lp_batch, DRI scans go to the restart-interval decoder instead.  Every catalogue file must
+scan on the multi-scan decoder, as one sequential scan; in lp_batch, DRI scans go to the restart-interval decoder
+instead.  Every catalogue file must
 decode to the oracle's pixels on each path, and the damaged files must be accepted or refused as written down below."""
 import ctypes as C
 
@@ -19,8 +20,8 @@ DAMAGED = jb.damaged()
 
 # (per-image decode accepts, lp_batch accepts) for each damaged file.  Where the oracle differs, the device follows
 # libjpeg-turbo: it refuses an all-ones code and a truncated scan.  The restart-interval decoder of the batch refuses
-# a scan whose RSTn markers do not count 0, 1, ... 7, 0 ... in step with its intervals, where the per-image serial
-# decoder (like the oracle) takes the next marker whatever its number.
+# a scan whose RSTn markers do not count 0, 1, ... 7, 0 ... in step with its intervals, where the per-image walk
+# (like the oracle) takes the next marker whatever its number.
 DEVICE_DAMAGED = {
     "all_ones_code": (False, False),
     "ac_run_past_63": (False, False),

@@ -1,8 +1,8 @@
 """GPU: decoded JPEG pixels, bit-exact against the oracle, at the tile edges of jpeg_idct_color_kernel.
 
 Per image (opencv_decoder_read_data), every case of tests/jpeg_decode_cases.py: one, two and three spans, one to
-ten bands, widths 1 to 4, in every sampling, through all three coefficient orders (the parallel decoder's scan order
-for plain files, the serial decoder's raster order for restart files, the multi-scan decoder for progressive ones).
+ten bands, widths 1 to 4, in every sampling, through both entropy decoders of the per-image path (the parallel decoder
+for plain files, the multi-scan decoder for restart and progressive files).
 
 Batch (lp_batch_stage + lp_batch_run): the decoded Fit crop windows themselves, each against the oracle's full
 decode cut to that window, and the resized frames against the oracle's Fit, over crops that cut left / right and

@@ -1,7 +1,8 @@
 """CPU: the multi-scan JPEG streams of tests/jpeg_scan_streams.py against libjpeg-turbo (cv2) and the oracle, and the
 host build of the shared multi-scan decode core (lilliput_b200/csrc/jpeg_scan_core.h, via
 tests/native/jpeg_scan_sim.cpp): a decode restricted to a region of interest, with nonzero masks outside it, must
-give exactly the region's coefficients of the whole-frame decode."""
+give exactly the region's coefficients of the whole-frame decode.  The same core walks the per-image decode's baseline
+files with restart markers (tests/jpeg_baseline_streams.py)."""
 import ctypes as C
 import os
 import shutil
@@ -10,7 +11,9 @@ import subprocess
 import numpy as np
 import pytest
 
+from tests import jpeg_baseline_streams as jb
 from tests import jpeg_scan_streams as js
+from tests.test_gpu_jpeg_baseline_streams import DEVICE_DAMAGED
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 CUDA_INC = os.path.join(os.environ.get("CUDA_HOME", "/usr/local/cuda"), "include")
@@ -99,6 +102,18 @@ def test_damaged_streams(oracle, name, data):
     except RuntimeError:
         mine = False
     assert (ref, mine) == DAMAGED[name]
+
+
+_DRI_FILES = ([(s.name, s.data, True) for s in jb.cases() if s.restart] +
+              [(name, data, DEVICE_DAMAGED[name][0]) for name, data, restart in jb.damaged() if restart])
+
+
+@pytest.mark.parametrize("name,data,accept", _DRI_FILES, ids=[f[0] for f in _DRI_FILES])
+def test_baseline_restart_files_walk_as_one_scan(sim, name, data, accept):
+    """Per image, a baseline file with restart markers is walked as a one-scan item: every catalogue file decodes,
+    and each damaged one is accepted or refused as the per-image decode is meant to."""
+    rc, _, _ = sim(data)
+    assert (rc == 0) == accept, rc
 
 
 def test_over_budget_file_counts_its_block_visits(sim):
