@@ -595,7 +595,12 @@ static GifFrameJob gif_frame_job(const GifFramePlan& f, size_t base, int prev_di
 // The walk gifDecoder + ImageOps.Transform would make over a WELL-FORMED file (every record readable, every
 // frame with a colour table, terminator present); anything else returns nullptr and the file takes the
 // per-image path, which reproduces the reference's handling of damaged files.
-GifAnimPlan* gif_plan_parse(const uint8_t* data, size_t len, int max_frames) {
+// first_frame_only: the walk of a Transform that stops after frame 0 (DisableAnimatedOutput).  The per-image decoder
+// reads nothing behind frame 0's image data then, so neither does the plan: later records may be damaged or missing,
+// max_frames is not consulted, and the blocks giflib_encoder_flush writes behind the frame are the ones the decoder
+// still holds -- frame 0's own, after the forced transparency and before the encoder's background drop.  The plan's
+// file span ends with frame 0's image data.
+GifAnimPlan* gif_plan_parse(const uint8_t* data, size_t len, int max_frames, bool first_frame_only) {
     GifReader r;
     r.p = data;
     r.n = len;
@@ -668,6 +673,7 @@ GifAnimPlan* gif_plan_parse(const uint8_t* data, size_t len, int max_frames) {
         }
         f.local = im.colors != nullptr;
         force_partial_transparent(ext, g, im, f.ncolors, r.sw, r.sh);
+        if (first_frame_only) p->trailing_ext = ext;
         f.enc_gcb = encoder_frame_gcb(ext, r, f.local, p->bg[3] == 255);
         f.ext.swap(ext);
         ext.clear();  // extensions are cleared after a frame (ref giflib.cpp:289-296)
@@ -678,10 +684,14 @@ GifAnimPlan* gif_plan_parse(const uint8_t* data, size_t len, int max_frames) {
         p->lzw_total += round_up(total + 32, (size_t)16);
         p->idx_total += round_up((size_t)im.width * im.height + 64, (size_t)16);
         p->frames.push_back(f);
+        if (first_frame_only) {
+            p->file_len = r.pos;
+            break;
+        }
         if ((int)p->frames.size() > max_frames) return nullptr;
     }
     if (p->frames.empty()) return nullptr;
-    p->trailing_ext.swap(ext);
+    if (!first_frame_only) p->trailing_ext.swap(ext);
     // gifDecoder.BackgroundColor() (ref giflib.cpp:1308-1431): set when the walk meets the file's first graphic
     // control block; a file that reaches its terminator without one keeps the initial white with alpha 0
     if (found_gcb) {
@@ -701,6 +711,7 @@ void gif_plan_info(const GifAnimPlan* p, int* width, int* height, int* nframes, 
     if (bgcolor) *bgcolor = p->bgcolor;
     if (loop_count) *loop_count = p->loop_count;
 }
+size_t gif_plan_file_bytes(const GifAnimPlan* p) { return p->file_len; }
 int gif_plan_delay_ms(const GifAnimPlan* p, int frame) { return p->frames[(size_t)frame].delay * 10; }  // ref giflib.go:212
 size_t gif_plan_device_bytes(const GifAnimPlan* p) {
     return round_up(p->file_len + 64, (size_t)256) + p->lzw_total + p->idx_total +

@@ -274,6 +274,9 @@ struct WebpPlan {
     std::vector<WebpFramePlan> frames;
 };
 bool webp_plan_parse(const uint8_t* data, size_t len, WebpPlan* out);
+// the plan cut to its frame 0, as a Transform that stops after frame 0 decodes it (rectangle, blend and dispose onto the
+// canvas unchanged); returns the bytes at the start of the file that frame needs: through the end of its image data
+size_t webp_plan_first_frame(WebpPlan* p);
 // device scratch webp_decode_batch lays out for one plan (uploaded file, VP8 work areas, lossless pixels, alpha planes,
 // job records), not counting the shared VP8L arena
 size_t webp_plan_device_bytes(const WebpPlan& p, size_t file_len);
@@ -287,8 +290,10 @@ int webp_decode_batch(const WebpPlan* const* plans, const uint8_t* const* files,
                       uint8_t* d_scratch, size_t scratch_bytes, uint8_t* d_arena, size_t arena_bytes, uint8_t* d_canvases,
                       const uint64_t* canvas_off, int* h_status, cudaEvent_t ev_uploaded, cudaStream_t st);
 struct GifAnimPlan;
-GifAnimPlan* gif_plan_parse(const uint8_t* data, size_t len, int max_frames);
+GifAnimPlan* gif_plan_parse(const uint8_t* data, size_t len, int max_frames, bool first_frame_only = false);
 void gif_plan_free(GifAnimPlan* p);
+// bytes at the start of the file the plan reads (the whole file, or through frame 0's image data): what to upload
+size_t gif_plan_file_bytes(const GifAnimPlan* p);
 void gif_plan_info(const GifAnimPlan* p, int* width, int* height, int* nframes, uint32_t* bgcolor, int* loop_count);
 int gif_plan_delay_ms(const GifAnimPlan* p, int frame);
 size_t gif_plan_device_bytes(const GifAnimPlan* p);

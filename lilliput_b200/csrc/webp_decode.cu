@@ -670,6 +670,12 @@ bool webp_plan_parse(const uint8_t* data, size_t len, WebpPlan* out) {
     return true;
 }
 
+size_t webp_plan_first_frame(WebpPlan* p) {
+    p->frames.resize(1);
+    const WebpFramePlan& f = p->frames[0];
+    return std::max(f.img_off + f.img_len, f.has_alph ? f.alph_off + f.alph_len : 0);
+}
+
 // the per-image decoder's VP8L arena bound, per stream
 static size_t vp8l_slice_bytes(const WebpFramePlan& f) { return round_up((size_t)f.width * f.height * 12 + (16u << 20), (size_t)256); }
 // the ALPH plane is decoded only onto a 4-channel canvas (webp_decoder_decode's need_alph)

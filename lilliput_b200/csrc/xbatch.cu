@@ -16,12 +16,17 @@
 //                 a per-pixel compositor over every file's frame sequence (webp_decode.cu), resize of every canvas
 //        GIF   -> every frame of every animation: LZW (one warp per frame), per-pixel compositor over the
 //                 frame sequence (gif_decode.cu), resize of every composited canvas
+//        DisableAnimatedOutput (GIF and animated WebP to WebP, GIF to GIF): Transform stops after frame 0, so the plan
+//                 stops there too (gif_plan_parse's first-frame walk, webp_plan_first_frame); only the file up to the
+//                 end of frame 0's image data is uploaded, the same kernels run over one frame per file, and the sink
+//                 writes a still WebP or a one-frame GIF
 //      and the sinks: JPEG (jpeg_encode.cu), lossy WebP still / animation (webp_encode.cu) carrying the ICC profile of
 //      a JPEG, PNG or WebP source as WebpEncoder does, GIF from GIF sources (palette mapping + LZW of every frame of the
 //      task, gif_decode.cu; the container assembled on the host), PNG from JPEG, PNG and WebP stills (filter, DEFLATE,
 //      checksums and container of every frame of a run in three launches, png_encode.cu);
 //   3. anything the grid path does not cover (gray or over-budget multi-scan JPEGs, EXIF-rotated sources, lossless WebP
-//      output, PNG output of animations, GIF output from other formats ...) and any item whose grid stage fails goes through
+//      output, PNG output of animations, GIF output from other formats, animations under MaxEncodeFrames or
+//      MaxEncodeDuration, one-frame GIFs to WebP with no time to encode ...) and any item whose grid stage fails goes through
 //      lp_transform on a worker thread -- still this library's device kernels, one image per call -- so the
 //      status and bytes of EVERY item are what lp_transform would have returned.
 // Two worker lanes, each with half of the device arena and its own stream, process chunks of groups
@@ -72,6 +77,7 @@ struct XItem {
     std::unique_ptr<WebpPlan> webp;  // (for WebP: the frames' spans, rectangles and blend / dispose)
     GifAnimPlan* gif = nullptr;
     int gif_frames = 0;
+    size_t span = 0;           // WebP, GIF: bytes at the start of the file the device reads (first-frame items: through frame 0)
     std::vector<uint8_t> icc;  // WebP sink: the source's profile the WebP writer carries (empty: none, or not sane)
 };
 
@@ -183,6 +189,7 @@ static void parse_item(lp_xbatch* X, int i) {
     const size_t n = X->in_len[i];
     it.kind = K_FALLBACK;
     it.icc.clear();
+    it.span = n;
     if (!d || n < 16 || X->sink == S_NONE) return;
     // To PNG every still is one frame in, the file out of the first Encode call: MaxEncodeFrames, DisableAnimatedOutput
     // and the deadline are never consulted.  A negative MaxEncodeDuration is exceeded before the frame is encoded, and
@@ -275,10 +282,12 @@ static void parse_item(lp_xbatch* X, int i) {
             f0.dispose = 0;
         } else {
             // animations -> animated WebP, with the option gates of GIF -> WebP; Transform checks its deadline after
-            // every non-final frame, so a zero budget fails there (ErrEncodeTimeout): per image
-            if (X->sink != S_WEBP || X->opt.disable_animated_output || X->opt.max_encode_frames != 0 ||
-                X->opt.max_encode_duration_ns != 0 || X->opt.encode_timeout_ns <= 0)
-                return;
+            // every non-final frame, so a zero budget fails there (ErrEncodeTimeout): per image.  DisableAnimatedOutput:
+            // Transform encodes frame 0 and flushes before its deadline check, so whatever the budget, the file is a
+            // still of the composited frame 0 and the device reads only that frame
+            if (X->sink != S_WEBP || X->opt.max_encode_frames != 0 || X->opt.max_encode_duration_ns != 0) return;
+            if (X->opt.disable_animated_output) it.span = webp_plan_first_frame(p.get());
+            else if (X->opt.encode_timeout_ns <= 0) return;
         }
         it.w = p->width;
         it.h = p->height;
@@ -291,20 +300,24 @@ static void parse_item(lp_xbatch* X, int i) {
         return;
     }
     if (!memcmp(d, "GIF8", 4)) {
-        if ((X->sink != S_WEBP && X->sink != S_GIF) || X->opt.disable_animated_output || X->opt.max_encode_frames != 0 ||
-            X->opt.max_encode_duration_ns != 0)
+        if ((X->sink != S_WEBP && X->sink != S_GIF) || X->opt.max_encode_frames != 0 || X->opt.max_encode_duration_ns != 0)
             return;
-        // a GIF written with no time to encode fails with ErrEncodeTimeout after its first frame (Transform's deadline)
-        if (X->sink == S_GIF && X->opt.encode_timeout_ns <= 0) return;
-        GifAnimPlan* p = gif_plan_parse(d, n, 4096);
+        // DisableAnimatedOutput: Transform encodes frame 0 and flushes before its deadline check, and its decoder reads
+        // nothing behind that frame.  Otherwise a GIF written with no time to encode fails with ErrEncodeTimeout after
+        // its first frame (Transform's deadline): per image
+        const bool first_only = X->opt.disable_animated_output != 0;
+        if (!first_only && X->sink == S_GIF && X->opt.encode_timeout_ns <= 0) return;
+        GifAnimPlan* p = gif_plan_parse(d, n, 4096, first_only);
         if (!p) return;
         int w = 0, h = 0, nf = 0;
         gif_plan_info(p, &w, &h, &nf, nullptr, nullptr);
         it.w = w;
         it.h = h;
         it.ch = 4;
-        // stills to WebP and odd files: per image (the GIF writer is the same for one frame)
-        if ((nf < 2 && X->sink == S_WEBP) || w > max_side || h > max_side || !plan_geometry(X->opt, &it)) {
+        it.span = gif_plan_file_bytes(p);
+        // a one-frame file to WebP meets the same deadline check after its frame: with no time to encode, per image
+        if ((nf < 2 && X->sink == S_WEBP && !first_only && X->opt.encode_timeout_ns <= 0) || w > max_side || h > max_side ||
+            !plan_geometry(X->opt, &it)) {
             gif_plan_free(p);
             return;
         }
@@ -700,7 +713,7 @@ static void run_webp(lp_xbatch* X, Lane& L, const std::vector<int>& idx) {
         const XItem& it = X->items[i];
         plans[k] = it.webp.get();
         files[k] = X->in[i];
-        flen[k] = X->in_len[i];
+        flen[k] = it.span;
         scratch += webp_plan_device_bytes(*plans[k], flen[k]);
         arena += webp_plan_arena_bytes(*plans[k]);
         const int nf = (int)plans[k]->frames.size();
@@ -845,7 +858,7 @@ static void run_gif(lp_xbatch* X, Lane& L, const std::vector<int>& idx) {
         first[a + 1] = first[a] + it.gif_frames;
         plans[a] = it.gif;
         files[a] = X->in[idx[a]];
-        flen[a] = X->in_len[idx[a]];
+        flen[a] = it.span;
         scratch_bytes += gif_plan_device_bytes(it.gif);
         L.h2d += flen[a];
     }
@@ -1140,7 +1153,7 @@ static size_t item_device_bytes(const lp_xbatch* X, const XItem& it, int i) {
             return 2 * X->in_len[i] + raw + outb + 8192;
         }
         case K_WEBP:  // the VP8L arena (at most a quarter of the lane) is shared by the task (reserved by split_by_memory)
-            return webp_plan_device_bytes(*it.webp, X->in_len[i]) +
+            return webp_plan_device_bytes(*it.webp, it.span) +
                    it.webp->frames.size() * (round_up((size_t)it.w * it.h * it.ch, (size_t)256) + outb) + 8192;
         case K_GIF:
             return gif_plan_device_bytes(it.gif) + (size_t)it.gif_frames * ((size_t)it.w * it.h * 4 + outb) + 8192 +
@@ -1250,7 +1263,7 @@ extern "C" int lp_xbatch_transform(lp_xbatch* X, const uint8_t* const* in, const
             used += need;
             if (kind == K_WEBP) {
                 const XItem& it = X->items[i];
-                work += (double)X->in_len[i] + 4096 +
+                work += (double)it.span + 4096 +
                         (double)it.webp->frames.size() * ((double)it.w * it.h * it.ch + (double)it.ow * it.oh * 12 + (256u << 10));
             }
         }
