@@ -222,8 +222,8 @@ const uint8_t* lp_batch_resized_dev(const lp_batch* b, size_t* image_stride);
 
 /* ---- heterogeneous batch: any supported formats and sizes, one set of options ----------------
  * (BASELINE configs 3, 4, 5: PNG -> WebP, animated GIF -> animated WebP, mixed JPEG / PNG / WebP -> JPEG.)
- * Sinks with a grid path: ".jpeg", lossy ".webp", ".gif" (from GIF sources) and ".png" (from JPEG, PNG and WebP
- * stills; RGBA sources keep their alpha).
+ * Sinks with a grid path: ".jpeg", lossy ".webp", lossless ".webp" (WebpQuality above 100, from PNG and GIF sources),
+ * ".gif" (from GIF sources) and ".png" (from JPEG, PNG and WebP stills; RGBA sources keep their alpha).
  * Per-item semantics, status and bytes are those of lp_transform(in[i], ..., opt, out[i], out_cap, ...).
  * Items are grouped by decoder and source geometry and every stage of a group is one grid launch
  * (csrc/xbatch.cu); whatever the grid path does not cover runs through lp_transform inside the call. */
@@ -285,6 +285,14 @@ int lp_jpeg_encode_dev(const uint8_t* frames, size_t frame_img_stride, size_t fr
 int lp_png_encode_batch_dev(const uint8_t* d_frames, size_t img_stride, size_t row_stride, int width, int height,
                             int channels, int n, int level, int adaptive, uint8_t* d_files, size_t slot,
                             uint32_t* d_len);
+/* Batched lossless WebP encode of `n` packed device BGR / BGRA frames of one geometry, as lp_xbatch's lossless ".webp"
+ * sink and the per-image WebP writer run it: the "VP8L" payload of frame i is copied to payloads + offsets[i],
+ * lengths[i] bytes long (payloads back to back).  part_bytes: bound on the packed output of one part of the call
+ * (0 = the library's 1 GiB); a call over it is encoded in parts with the same bytes.  LP_ERR_BUF_TOO_SMALL when the
+ * payloads do not fit payloads_cap. */
+int lp_webp_lossless_encode_batch_dev(const uint8_t* d_frames, size_t img_stride, size_t row_step, int width, int height,
+                                      int channels, int n, size_t part_bytes, uint8_t* payloads, size_t payloads_cap,
+                                      size_t* offsets, size_t* lengths);
 /* CRC-32 and Adler-32 of `n` bytes of device memory by the PNG encoder's device arithmetic (a warp per 32 KB piece,
  * pieces folded by the rules of csrc/crc32_core.h): for tests against zlib. */
 int lp_png_checksums_dev(const uint8_t* d_data, size_t n, uint32_t* crc32, uint32_t* adler32);

@@ -251,6 +251,11 @@ int webp_encode_lossy_batch(const uint8_t* d_frames, size_t img_stride, size_t r
                             int channels, int n, int quality, std::vector<WebpEncodedFrame>* out, cudaStream_t st);
 // Device bytes webp_encode_lossy_batch allocates for n frames of one geometry (its scratch, outside any arena)
 size_t webp_encode_lossy_scratch_bytes(int width, int height, int channels, int n);
+// n packed device frames of one geometry -> lossless "VP8L" payloads (lossless = true, has_alpha = channels == 4), each
+// byte-identical to vp8l_enc_core.h's stream of that frame.  part_bytes bounds the packed output of one part of the call
+// (0: 1 GiB); a longer call is packed in parts, with the same bytes.
+int webp_encode_lossless_batch(const uint8_t* d_frames, size_t img_stride, size_t row_step, int width, int height,
+                               int channels, int n, std::vector<WebpEncodedFrame>* out, cudaStream_t st, size_t part_bytes = 0);
 void webp_assemble(const WebpEncodedFrame* frames, int n, const uint8_t* icc, size_t icc_len, uint32_t bgcolor,
                    uint32_t loop_count, std::vector<uint8_t>* file);
 

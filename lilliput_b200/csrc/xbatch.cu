@@ -21,14 +21,16 @@
 //                 end of frame 0's image data is uploaded, the same kernels run over one frame per file, and the sink
 //                 writes a still WebP or a one-frame GIF
 //      and the sinks: JPEG (jpeg_encode.cu), lossy WebP still / animation (webp_encode.cu) carrying the ICC profile of
-//      a JPEG, PNG or WebP source as WebpEncoder does, GIF from GIF sources (palette mapping + LZW of every frame of the
-//      task, gif_decode.cu; the container assembled on the host), PNG from JPEG, PNG and WebP stills (filter, DEFLATE,
-//      checksums and container of every frame of a run in three launches, png_encode.cu);
+//      a JPEG, PNG or WebP source as WebpEncoder does, lossless WebP still / animation from PNG and GIF sources (the
+//      batched VP8L encoder over every frame of a run, webp_encode.cu; a PNG's ICC profile carried the same way), GIF
+//      from GIF sources (palette mapping + LZW of every frame of the task, gif_decode.cu; the container assembled on the
+//      host), PNG from JPEG, PNG and WebP stills (filter, DEFLATE, checksums and container of every frame of a run in
+//      three launches, png_encode.cu);
 //   3. anything the grid path does not cover (gray or over-budget multi-scan JPEGs, EXIF-rotated sources, lossless WebP
-//      output, PNG output of animations, GIF output from other formats, animations under MaxEncodeFrames or
-//      MaxEncodeDuration, one-frame GIFs to WebP with no time to encode ...) and any item whose grid stage fails goes through
-//      lp_transform on a worker thread -- still this library's device kernels, one image per call -- so the
-//      status and bytes of EVERY item are what lp_transform would have returned.
+//      output of JPEG and WebP sources, PNG output of animations, GIF output from other formats, animations under
+//      MaxEncodeFrames or MaxEncodeDuration, one-frame GIFs to WebP with no time to encode ...) and any item whose grid
+//      stage fails goes through lp_transform on a worker thread -- still this library's device kernels, one image per
+//      call -- so the status and bytes of EVERY item are what lp_transform would have returned.
 // Two worker lanes, each with half of the device arena and its own stream, process chunks of groups
 // concurrently, so one lane's PCIe copies and host-side container work overlap the other lane's kernels.
 // Nothing is exchanged between images, lanes or GPUs.
@@ -134,6 +136,7 @@ struct lp_xbatch {
     lp_image_options opt;
     Sink sink = S_NONE;
     int quality = 0;
+    bool lossless = false;     // S_WEBP: lossless (VP8L) frames, WebpQuality above 100
     bool progressive = false;  // S_JPEG: progressive files (JpegProgressive)
     int png_level = 1;         // S_PNG: zlib level and filter policy (png_encode_policy)
     bool png_adaptive = false;
@@ -200,6 +203,7 @@ static void parse_item(lp_xbatch* X, int i) {
     thread_local std::vector<uint8_t> icc_buf(32768);
     if (d[0] == 0xFF && d[1] == 0xD8) {
         if (X->sink != S_JPEG && X->sink != S_WEBP && X->sink != S_PNG) return;
+        if (X->lossless) return;  // lossless WebP output of JPEG sources: per image
         // A still to WebP: after its frame Transform checks its deadline (a zero budget fails with ErrEncodeTimeout),
         // MaxEncodeFrames == 1 asks the decoder to skip to the end (a JPEG cannot: ErrSkipNotSupported), and a negative
         // MaxEncodeDuration is exceeded at once (the same skip).  Those go per image.
@@ -253,8 +257,9 @@ static void parse_item(lp_xbatch* X, int i) {
             // PNGs with a profile stay per image, where they went before they could carry it, under the options whose
             // result the per-image path decides after the frame: a zero encode budget (the deadline check, as for WebP
             // stills), MaxEncodeFrames == 1 and a negative MaxEncodeDuration (the skip to the end a PNG decoder
-            // refuses, as a JPEG's does)
-            if (icc_n > 0 && (X->opt.encode_timeout_ns <= 0 || X->opt.max_encode_frames == 1 || X->opt.max_encode_duration_ns < 0))
+            // refuses, as a JPEG's does).  To lossless output every PNG follows that rule.
+            if ((icc_n > 0 || X->lossless) &&
+                (X->opt.encode_timeout_ns <= 0 || X->opt.max_encode_frames == 1 || X->opt.max_encode_duration_ns < 0))
                 return;
             keep_icc(&it, icc_buf.data(), icc_n);
         }
@@ -263,7 +268,7 @@ static void parse_item(lp_xbatch* X, int i) {
         return;
     }
     if (!memcmp(d, "RIFF", 4) && !memcmp(d + 8, "WEBP", 4)) {
-        if (X->sink == S_GIF) return;
+        if (X->sink == S_GIF || X->lossless) return;  // (lossless WebP output of WebP sources: per image)
         std::unique_ptr<WebpPlan> p(new WebpPlan);
         if (!webp_plan_parse(d, n, p.get())) return;  // damaged containers: per image
         if (p->width > max_side || p->height > max_side) return;
@@ -304,9 +309,9 @@ static void parse_item(lp_xbatch* X, int i) {
             return;
         // DisableAnimatedOutput: Transform encodes frame 0 and flushes before its deadline check, and its decoder reads
         // nothing behind that frame.  Otherwise a GIF written with no time to encode fails with ErrEncodeTimeout after
-        // its first frame (Transform's deadline): per image
+        // its first frame (Transform's deadline): per image, to GIF and to lossless WebP
         const bool first_only = X->opt.disable_animated_output != 0;
-        if (!first_only && X->sink == S_GIF && X->opt.encode_timeout_ns <= 0) return;
+        if (!first_only && (X->sink == S_GIF || X->lossless) && X->opt.encode_timeout_ns <= 0) return;
         GifAnimPlan* p = gif_plan_parse(d, n, 4096, first_only);
         if (!p) return;
         int w = 0, h = 0, nf = 0;
@@ -416,6 +421,14 @@ static void png_sink(lp_xbatch* X, Lane& L, Bump& bump, uint8_t* h_stage, size_t
     bump.used = mark;
 }
 
+// The WebP sink's encoder: n resized frames of one geometry (rows packed, `stride` apart) -> lossy VP8 or, when the
+// options ask for lossless output, VP8L payloads
+static int webp_encode_frames(const lp_xbatch* X, const uint8_t* d_frames, size_t stride, int ow, int oh, int ch, int n,
+                              std::vector<WebpEncodedFrame>* frames, cudaStream_t st) {
+    if (X->lossless) return webp_encode_lossless_batch(d_frames, stride, (size_t)ow * ch, ow, oh, ch, n, frames, st);
+    return webp_encode_lossy_batch(d_frames, stride, (size_t)ow * ch, ow, oh, ch, n, X->quality, frames, st);
+}
+
 // resized frames (n x ow x oh x ch, `stride` apart) -> encoded files in the callers' buffers.  h_stage: the pinned
 // staging area the JPEG and PNG sinks copy their files through.
 static void sink_encode(lp_xbatch* X, Lane& L, Bump& bump, uint8_t* h_stage, size_t h_stage_bytes, const std::vector<int>& idx,
@@ -468,9 +481,9 @@ static void sink_encode(lp_xbatch* X, Lane& L, Bump& bump, uint8_t* h_stage, siz
         deliver_staged(X, h_stage, idx.data(), n, off, len, slot, failed);
         return;
     }
-    // lossy WebP stills, each with its source's ICC profile
+    // WebP stills, lossy or lossless, each with its source's ICC profile
     std::vector<WebpEncodedFrame> frames;
-    int rc = webp_encode_lossy_batch(d_frames, stride, (size_t)ow * ch, ow, oh, ch, n, X->quality, &frames, L.st);
+    int rc = webp_encode_frames(X, d_frames, stride, ow, oh, ch, n, &frames, L.st);
     if (rc) {
         cudaGetLastError();
         failed->insert(failed->end(), idx.begin(), idx.end());
@@ -893,7 +906,7 @@ static void run_gif(lp_xbatch* X, Lane& L, const std::vector<int>& idx) {
     }
     cudaEventRecord(L.ev[2], L.st);
     std::vector<WebpEncodedFrame> frames;
-    int rc = webp_encode_lossy_batch(d_resized, out_stride, (size_t)g.ow * 4, g.ow, g.oh, 4, nf, X->quality, &frames, L.st);
+    int rc = webp_encode_frames(X, d_resized, out_stride, g.ow, g.oh, 4, nf, &frames, L.st);
     cudaEventRecord(L.ev[3], L.st);
     cudaEventSynchronize(L.ev[3]);
     lane_time(L, 2, 3, &L.ms_encode);
@@ -1195,6 +1208,7 @@ extern "C" int lp_xbatch_transform(lp_xbatch* X, const uint8_t* const* in, const
     std::string ext = opt->file_type ? opt->file_type : "";
     for (auto& c : ext) c = (char)tolower((unsigned char)c);
     X->sink = S_NONE;
+    X->lossless = false;
     X->progressive = false;
     if (ext == ".jpeg" || ext == ".jpg") {
         X->sink = S_JPEG;
@@ -1203,7 +1217,8 @@ extern "C" int lp_xbatch_transform(lp_xbatch* X, const uint8_t* const* in, const
     } else if (ext == ".webp") {
         const int q = option_value(*opt, CV_IMWRITE_WEBP_QUALITY, 100);
         X->quality = q < 1 ? 1 : q;
-        X->sink = q > 100 ? S_NONE : S_WEBP;  // lossless output: per image
+        X->sink = S_WEBP;
+        X->lossless = q > 100;
     } else if (ext == ".gif") {
         X->sink = S_GIF;
     } else if (ext == ".png") {
