@@ -348,6 +348,19 @@ int orient_crop_launch(const OrientJob* d_jobs, int n, const uint8_t* src, uint8
 int copy_region_launch(const uint8_t* src, size_t src_step, int src_ch, uint8_t* dst,
                        size_t dst_step, int dst_ch, int w, int h, cudaStream_t st);
 // ---- tonemap.cu ----------------------------------------------------------------------------
+// One 8-bit BGR / BGRA frame on the device, tone-mapped in place from the cICP transfer / primaries code points.
+struct TmFrame {
+    uint8_t* px;
+    size_t step;
+    int w, h, channels, transfer, primaries;
+};
+// Device scratch tonemap_batch_launch needs for these frames (0: none of them is tone-mapped; px is not read)
+size_t tonemap_batch_scratch_bytes(const TmFrame* frames, int n);
+// n frames of any sizes, each with its own transfer and primaries, in 7 launches and three host round trips.  A
+// frame's result does not depend on the other frames of the call.  Frames that are not 3- or 4-channel, or empty, are
+// left as they are (the reference returns silently).  Returns once the final map is enqueued on st.
+int tonemap_batch_launch(const TmFrame* frames, int n, void* d_scratch, size_t scratch_bytes, cudaStream_t st);
+// tonemap_batch_launch of one frame, its scratch allocated on st
 int tonemap_to_sdr_launch(uint8_t* d_px, size_t step, int channels, int w, int h, int transfer, int primaries, cudaStream_t st);
 
 int compact_launch(const uint8_t* src, size_t stride, const uint32_t* len, uint32_t cap, int n, uint8_t* dst,

@@ -11,7 +11,10 @@
 //                 (progressive) files form groups of their own, so a chunk of baseline files never waits for the
 //                 serial decode of a large progressive one.  To WebP or PNG the pipeline stops after the resize and the
 //                 group's frames go to that sink's encoder
-//        PNG   -> IDAT gather + warp-parallel inflate + defilter + convert (png_decode.cu), resize
+//        PNG   -> IDAT gather + warp-parallel inflate + defilter + convert (png_decode.cu; 16-bit samples keep their high
+//                 byte), resize.  A PQ or HLG cICP chunk: the window's HDR frames go through one batched tone map to SDR
+//                 BT.709 (tonemap.cu) between the defilter and the resize, whole, as Transform tone-maps right after the
+//                 decode; no cICP is written.  An SDR cICP changes no pixel (to PNG it stays per image, below)
 //        WebP  -> stills and animations: VP8 frames one per warp, VP8L / ALPH streams one per warp in arena-sized waves,
 //                 a per-pixel compositor over every file's frame sequence (webp_decode.cu), resize of every canvas
 //        GIF   -> every frame of every animation: LZW (one warp per frame), per-pixel compositor over the
@@ -26,11 +29,12 @@
 //      from GIF sources (palette mapping + LZW of every frame of the task, gif_decode.cu; the container assembled on the
 //      host), PNG from JPEG, PNG and WebP stills (filter, DEFLATE, checksums and container of every frame of a run in
 //      three launches, png_encode.cu);
-//   3. anything the grid path does not cover (gray or over-budget multi-scan JPEGs, EXIF-rotated sources, lossless WebP
-//      output of JPEG and WebP sources, PNG output of animations, GIF output from other formats, animations under
-//      MaxEncodeFrames or MaxEncodeDuration, one-frame GIFs to WebP with no time to encode ...) and any item whose grid
-//      stage fails goes through lp_transform on a worker thread -- still this library's device kernels, one image per
-//      call -- so the status and bytes of EVERY item are what lp_transform would have returned.
+//   3. anything the grid path does not cover (gray or over-budget multi-scan JPEGs, gray PNGs, EXIF-rotated sources,
+//      SDR-cICP PNGs to PNG (Transform re-attaches the chunk), lossless WebP output of JPEG and WebP sources, PNG
+//      output of animations, GIF output from other formats, animations under MaxEncodeFrames or MaxEncodeDuration,
+//      one-frame GIFs to WebP with no time to encode ...) and any item whose grid stage fails goes through lp_transform
+//      on a worker thread -- still this library's device kernels, one image per call -- so the status and bytes of
+//      EVERY item are what lp_transform would have returned.
 // Two worker lanes, each with half of the device arena and its own stream, process chunks of groups
 // concurrently, so one lane's PCIe copies and host-side container work overlap the other lane's kernels.
 // Nothing is exchanged between images, lanes or GPUs.
@@ -76,6 +80,8 @@ struct XItem {
     int jpeg_sampling = 0;          // (h0<<12)|(v0<<8)|... groups JPEGs of one component layout
     bool jpeg_multiscan = false;    // progressive, or one scan per component
     std::unique_ptr<PngHeader> png;
+    bool hdr = false;                 // PNG: a cICP chunk with a PQ (16) or HLG (18) transfer, tone-mapped after the decode
+    int transfer = 0, primaries = 0;  // (its code points)
     std::unique_ptr<WebpPlan> webp;  // (for WebP: the frames' spans, rectangles and blend / dispose)
     GifAnimPlan* gif = nullptr;
     int gif_frames = 0;
@@ -238,11 +244,17 @@ static void parse_item(lp_xbatch* X, int i) {
         if (X->sink == S_GIF) return;  // GIF output needs a GIF source: per image (ErrGifEncoderNeedsDecoder)
         std::unique_ptr<PngHeader> h(new PngHeader);
         if (png_parse(d, n, h.get()) != LP_OK) return;
+        // an eXIf orientation other than 1: Transform turns the frame before the resize, which the grid does not: per image
         if (h->orientation != 1 || h->idat.empty() || h->idat_total < 2) return;
         if (h->width > max_side || h->height > max_side) return;
-        if (h->bit_depth == 16) return;  // reported as a 16-bit type: the 8-bit Framebuffer path has its own rules
-        uint8_t cicp[4];
-        if (png_extract_cicp(d, n, cicp)) return;                      // cICP handling stays with Transform
+        uint8_t cicp[4];  // primaries, transfer, matrix, full range: the chunk Transform's decoder reports
+        if (png_extract_cicp(d, n, cicp)) {
+            it.hdr = cicp[1] == 16 || cicp[1] == 18;
+            // an SDR tag changes no pixel, but Transform re-attaches it to a PNG output (ops.go:306-332): per image
+            if (!it.hdr && X->sink == S_PNG) return;
+            it.transfer = cicp[1];
+            it.primaries = cicp[0];
+        }
         // the IDAT payloads must form one forward run of the file (they do in every valid PNG)
         for (size_t k = 1; k < h->idat.size(); k++)
             if (h->idat[k].offset < h->idat[k - 1].offset + h->idat[k - 1].length) return;
@@ -655,13 +667,30 @@ static void run_png(lp_xbatch* X, Lane& L, const std::vector<int>& idx) {
         max_h = std::max(max_h, xi.h);
     }
     win_first.push_back(n);
+    // HDR frames are tone-mapped between the defilter and the resize of their window, whole (before the Fit crop, as
+    // Transform does); one scratch area sized for the window that needs the most
+    std::vector<TmFrame> hdr;
+    auto window_hdr = [&](int k0, int k1, uint8_t* frames) {
+        hdr.clear();
+        for (int k = k0; k < k1; k++) {
+            const XItem& xi = X->items[idx[k]];
+            if (xi.hdr)
+                hdr.push_back(TmFrame{frames ? frames + frame_off[k] : nullptr, (size_t)xi.w * xi.ch, xi.w, xi.h, xi.ch, xi.transfer, xi.primaries});
+        }
+    };
+    size_t tm_bytes = 0;
+    for (size_t wdx = 0; wdx + 1 < win_first.size(); wdx++) {
+        window_hdr(win_first[wdx], win_first[wdx + 1], nullptr);
+        tm_bytes = std::max(tm_bytes, tonemap_batch_scratch_bytes(hdr.data(), (int)hdr.size()));
+    }
     uint8_t* d_in = bump.take<uint8_t>(zg + 4096);
     PngDecodeItem* d_items = bump.take<PngDecodeItem>((size_t)n * sizeof(PngDecodeItem));
     SegCopy* d_segs = bump.take<SegCopy>(segs.size() * sizeof(SegCopy) + 16);
     uint8_t* d_raw = bump.take<uint8_t>(raw_bytes + 256);
     uint8_t* d_frames = bump.take<uint8_t>(win_max + 256);
     uint8_t* d_out = bump.take<uint8_t>(out_bytes + 256);
-    if (!d_in || !d_items || !d_segs || !d_raw || !d_frames || !d_out) {
+    uint8_t* d_tm = tm_bytes ? bump.take<uint8_t>(tm_bytes) : nullptr;
+    if (!d_in || !d_items || !d_segs || !d_raw || !d_frames || !d_out || (tm_bytes && !d_tm)) {
         for (int i : idx) push_fallback(X, i);
         return;
     }
@@ -690,6 +719,8 @@ static void run_png(lp_xbatch* X, Lane& L, const std::vector<int>& idx) {
     for (size_t wdx = 0; wdx + 1 < win_first.size() && ok; wdx++) {
         const int k0 = win_first[wdx], k1 = win_first[wdx + 1];
         ok = png_unfilter_launch(b, k0, k1 - k0, L.st) == LP_OK;
+        window_hdr(k0, k1, d_frames);
+        if (ok && !hdr.empty()) ok = tonemap_batch_launch(hdr.data(), (int)hdr.size(), d_tm, tm_bytes, L.st) == LP_OK;
         if (ok) ok = resize_range(X, L, idx, k0, k1, d_frames, frame_off, d_out, out_off);
     }
     cudaEventRecord(L.ev[1], L.st);
@@ -700,7 +731,7 @@ static void run_png(lp_xbatch* X, Lane& L, const std::vector<int>& idx) {
         for (int i : idx) push_fallback(X, i);
         return;
     }
-    lane_time(L, 0, 1, &L.ms_decode);  // (the resize launches sit between the defilter launches here: counted as decode)
+    lane_time(L, 0, 1, &L.ms_decode);  // (the tone map and resize launches sit between the defilter launches: counted as decode)
     std::vector<char> good((size_t)n);
     for (int k = 0; k < n; k++) good[k] = items[k].status == 0;
     encode_runs(X, L, bump, idx, d_out, out_off, good, &failed);
@@ -1160,10 +1191,13 @@ static size_t item_device_bytes(const lp_xbatch* X, const XItem& it, int i) {
     const size_t outb = (size_t)it.ow * it.oh * 4 * 3 + (256u << 10) + (X->sink == S_PNG ? png_sink_item_bytes(X, it.ow, it.oh, it.ch) : 0);
     switch (it.kind) {
         case K_PNG: {
-            // compressed span (+ its gathered copy) + inflated scanlines + resized output; the packed frames live in a
-            // window buffer shared by the task (a fifth of the lane's arena, reserved by split_by_memory)
-            const size_t raw = ((size_t)it.w * (it.ch == 4 ? 4 : 3) + 2) * it.h * (it.png && it.png->interlace ? 2 : 1);
-            return 2 * X->in_len[i] + raw + outb + 8192;
+            // compressed span (+ its gathered copy) + inflated scanlines (the header's row bytes: twice the samples' count
+            // at 16 bits) + resized output + an HDR frame's tone-map records; the packed frames live in a window buffer
+            // shared by the task (a fifth of the lane's arena, reserved by split_by_memory)
+            const size_t row = std::max((size_t)it.w * (it.ch == 4 ? 4 : 3), it.png ? it.png->row_bytes : 0);
+            const size_t raw = (row + 2) * it.h * (it.png && it.png->interlace ? 2 : 1);
+            const TmFrame tm{nullptr, 0, it.w, it.h, it.ch, it.transfer, it.primaries};
+            return 2 * X->in_len[i] + raw + outb + 8192 + (it.hdr ? tonemap_batch_scratch_bytes(&tm, 1) : 0);
         }
         case K_WEBP:  // the VP8L arena (at most a quarter of the lane) is shared by the task (reserved by split_by_memory)
             return webp_plan_device_bytes(*it.webp, it.span) +
