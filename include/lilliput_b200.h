@@ -247,6 +247,16 @@ int lp_xbatch_transform(lp_xbatch* x, const uint8_t* const* in, const size_t* in
                         const lp_image_options* opt, uint8_t* const* out, size_t out_cap, size_t* out_len,
                         int* status);
 void lp_xbatch_get_stats(const lp_xbatch* x, lp_xbatch_stats* out);
+/* Several outputs ("renditions") of every item in one call: opts[0..k-1], k in 1..LP_XBATCH_MAX_RENDITIONS.  out,
+ * out_len and status have n * k entries, item-major: pair (i, r) is at i * k + r and gets exactly the status and bytes
+ * of lp_transform(in[i], in_len[i], &opts[r], ...).  Each file is uploaded and decoded once for all the renditions it
+ * takes on the grid path (an animation: once per rendition); the pairs the grid path does not take run through
+ * lp_transform.  grid_items and fallback_items of the stats count pairs.  lp_xbatch_transform is this call with k = 1.
+ * A bad k or a null opts: LP_ERR_BAD_ARGUMENT, and nothing is written. */
+#define LP_XBATCH_MAX_RENDITIONS 16
+int lp_xbatch_transform_renditions(lp_xbatch* x, const uint8_t* const* in, const size_t* in_len, int n,
+                                   const lp_image_options* opts, int k, uint8_t* const* out, size_t out_cap,
+                                   size_t* out_len, int* status);
 
 /* ---- the same call over several GPUs of one node (SURVEY 8(e): shard by image index, no collective) ----
  * One lp_xbatch per device behind one call: the batch is cut into contiguous blocks balanced by compressed bytes,
@@ -258,6 +268,10 @@ int lp_multi_device_count(const lp_multi* m);
 int lp_multi_transform(lp_multi* m, const uint8_t* const* in, const size_t* in_len, int n,
                        const lp_image_options* opt, uint8_t* const* out, size_t out_cap, size_t* out_len,
                        int* status);
+/* lp_xbatch_transform_renditions over the devices: sharded by item, so all renditions of an item run on one GPU. */
+int lp_multi_transform_renditions(lp_multi* m, const uint8_t* const* in, const size_t* in_len, int n,
+                                  const lp_image_options* opts, int k, uint8_t* const* out, size_t out_cap,
+                                  size_t* out_len, int* status);
 void lp_multi_get_stats(const lp_multi* m, int device_index, lp_xbatch_stats* out);
 /* Host-only: the block boundaries lp_multi_transform uses (first[0..parts], contiguous, balanced by bytes). */
 void lp_shard_blocks(const size_t* in_len, int n, int parts, int* first);

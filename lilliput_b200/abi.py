@@ -470,6 +470,24 @@ class _XBatchStats(C.Structure):
                 ("h2d_bytes", C.c_size_t), ("d2h_bytes", C.c_size_t), ("ms_busy_max_lane", C.c_double)]
 
 
+def _renditions(fn, h, bufs, opts, out_cap):
+    """lp_xbatch_transform_renditions / lp_multi_transform_renditions: every file through every ImageOptions of
+    `opts`.  Returns (outs, status), both indexed [item][rendition]."""
+    n, k = len(bufs), len(opts)
+    ptrs, lens, keep = Batch._ptr_arrays(bufs)
+    out = np.empty((max(n * k, 1), out_cap), dtype=np.uint8)
+    out_ptrs = (C.c_void_p * (n * k))(*[out[p].ctypes.data for p in range(n * k)])
+    out_lens = (C.c_size_t * (n * k))()
+    status = (C.c_int * (n * k))()
+    cs = [o._c() for o in opts]  # (they own the strings and option arrays the copies point at)
+    copts = (_ImageOptions * k)(*cs)
+    rc = fn(h, ptrs, lens, n, copts, k, out_ptrs, out_cap, out_lens, status)
+    if rc:
+        raise LilliputError(rc)
+    return ([[out[i * k + r, : out_lens[i * k + r]].tobytes() for r in range(k)] for i in range(n)],
+            [[status[i * k + r] for r in range(k)] for i in range(n)])
+
+
 class XBatch:
     """lp_xbatch_*: N independent images of any supported format / size, one set of options, grouped into grid
     launches; per-item results are those of lp_transform (include/lilliput_b200.h)."""
@@ -484,6 +502,9 @@ class XBatch:
         l.lp_xbatch_transform.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.POINTER(_ImageOptions),
                                           C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p]
         l.lp_xbatch_get_stats.argtypes = [C.c_void_p, C.POINTER(_XBatchStats)]
+        l.lp_xbatch_transform_renditions.restype = C.c_int
+        l.lp_xbatch_transform_renditions.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.POINTER(_ImageOptions),
+                                                     C.c_int, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p]
         cfg = _XBatchConfig(device, arena_bytes, host_threads, max_size)
         self.h = l.lp_xbatch_create(C.byref(cfg))
         if not self.h:
@@ -511,6 +532,11 @@ class XBatch:
             raise LilliputError(rc)
         return [out[i, : out_lens[i]].tobytes() for i in range(n)], list(status)
 
+    def transform_renditions(self, bufs, opts, out_cap: int = 1 << 20):
+        """Every file through every ImageOptions of `opts` in one call (each file decoded once): (outs, status)
+        indexed [item][rendition], each pair equal to lp_transform(bufs[i], opts[r])."""
+        return _renditions(self.lib.l.lp_xbatch_transform_renditions, self.h, bufs, opts, out_cap)
+
     def stats(self) -> dict:
         s = _XBatchStats()
         self.lib.l.lp_xbatch_get_stats(self.h, C.byref(s))
@@ -531,6 +557,9 @@ class MultiBatch:
         l.lp_multi_transform.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.POINTER(_ImageOptions),
                                          C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p]
         l.lp_multi_get_stats.argtypes = [C.c_void_p, C.c_int, C.POINTER(_XBatchStats)]
+        l.lp_multi_transform_renditions.restype = C.c_int
+        l.lp_multi_transform_renditions.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.POINTER(_ImageOptions),
+                                                    C.c_int, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p]
         devs = (C.c_int * len(devices))(*devices)
         cfg = _XBatchConfig(0, arena_bytes, host_threads, max_size)
         self.n_devices = len(devices)
@@ -558,6 +587,10 @@ class MultiBatch:
         if rc:
             raise LilliputError(rc)
         return [out[i, : out_lens[i]].tobytes() for i in range(n)], list(status)
+
+    def transform_renditions(self, bufs, opts, out_cap: int = 1 << 20):
+        """XBatch.transform_renditions over the devices, sharded by item."""
+        return _renditions(self.lib.l.lp_multi_transform_renditions, self.h, bufs, opts, out_cap)
 
     def stats(self, device_index: int) -> dict:
         s = _XBatchStats()

@@ -86,6 +86,10 @@ struct lp_batch {
     int out_w2 = 0, out_h2 = 0;
     int crop2_x = 0, crop2_y = 0, crop2_w = 0, crop2_h = 0;
     size_t oriented_bytes = 0;  // slot stride of d_oriented: the larger of the two classes' packed crops
+    // resize-only contexts with several outputs: each decoded window (the union of their crops, in crop_*) is resized
+    // into every geometry; geometry g's frames are at d_resized + geom_off[g], g.out_w * g.out_h * 3 bytes apart
+    std::vector<BatchGeom> geoms;
+    std::vector<size_t> geom_off;
     // per-image scratch layout, fixed by the first image staged into this context
     bool layout_known = false;
     uint32_t blocks = 0;
@@ -184,8 +188,10 @@ static void batch_free(lp_batch* b) {
 namespace lp {
 lp_batch* batch_create_in(const lp_batch_config* cfg, uint8_t* dev_arena, size_t dev_bytes, uint8_t* host_arena,
                           size_t host_bytes, bool progressive_jpeg = false, bool multiscan_sources = true,
-                          bool resize_only = false, bool oriented_sources = false, bool gray_sources = false);
+                          bool resize_only = false, bool oriented_sources = false, bool gray_sources = false,
+                          const BatchGeom* geoms = nullptr, int n_geoms = 0);
 int batch_resized_status(lp_batch* b, int* status);
+const uint8_t* batch_resized_geom(const lp_batch* b, int g, size_t* image_stride);
 void batch_arena_used(const lp_batch* b, size_t* dev_bytes, size_t* host_bytes);
 }
 extern "C" lp_batch* lp_batch_create(const lp_batch_config* cfg) {
@@ -200,11 +206,14 @@ extern "C" lp_batch* lp_batch_create(const lp_batch_config* cfg) {
 // lp_batch_fetch refuse it), and the caller encodes the frames at lp_batch_resized_dev.  oriented_sources: take
 // EXIF-rotated files (and allocate the oriented-crop buffers); otherwise they get LP_ERR_UNSUPPORTED.  gray_sources: take
 // one-component files (they fit the colour slots: only the image map is allocated for them); otherwise they get
-// LP_ERR_UNSUPPORTED.
+// LP_ERR_UNSUPPORTED.  geoms (n_geoms > 1, resize-only contexts of unrotated colour sources only): the outputs each
+// decoded window is resized into, in place of cfg's one; the window decoded is the bounding box of their crops, and
+// batch_resized_geom gives each one's frames.
 lp_batch* lp::batch_create_in(const lp_batch_config* cfg, uint8_t* dev_arena, size_t dev_bytes, uint8_t* host_arena,
                               size_t host_bytes, bool progressive_jpeg, bool multiscan_sources, bool resize_only,
-                              bool oriented_sources, bool gray_sources) {
+                              bool oriented_sources, bool gray_sources, const BatchGeom* geoms, int n_geoms) {
     if (!cfg || cfg->max_images < 1 || cfg->src_width < 1 || cfg->src_height < 1) return nullptr;
+    if (n_geoms > 1 && (!geoms || !resize_only || oriented_sources || gray_sources)) return nullptr;
     if (ensure_device()) return nullptr;
     DeviceGuard dev_guard(cfg->device);
     if (!dev_guard.ok) return nullptr;
@@ -245,6 +254,20 @@ lp_batch* lp::batch_create_in(const lp_batch_config* cfg, uint8_t* dev_arena, si
         b->out_h2 = b->out_h;
         b->crop2_w = b->H;
         b->crop2_h = b->W;
+    }
+    if (n_geoms > 1) {  // the decoded window: the bounding box of every output's crop
+        b->geoms.assign(geoms, geoms + n_geoms);
+        int x0 = b->W, y0 = b->H, x1 = 0, y1 = 0;
+        for (const BatchGeom& g : b->geoms) {
+            x0 = std::min(x0, g.crop_x);
+            y0 = std::min(y0, g.crop_y);
+            x1 = std::max(x1, g.crop_x + g.crop_w);
+            y1 = std::max(y1, g.crop_y + g.crop_h);
+        }
+        b->crop_x = x0;
+        b->crop_y = y0;
+        b->crop_w = x1 - x0;
+        b->crop_h = y1 - y0;
     }
     const int slots = jpeg_huff_parallel_slots();
     // default chunk: three full waves of the per-image Huffman CTAs (no mostly-empty tail wave; larger
@@ -305,7 +328,16 @@ lp_batch* lp::batch_create_in(const lp_batch_config* cfg, uint8_t* dev_arena, si
     BALLOC(b->d_coef, (size_t)b->chunk * max_blocks * 64 * sizeof(int16_t));
     // (a rotated item's window is at most the frame; its slots are 256-byte aligned)
     BALLOC(b->d_frames, (size_t)b->chunk * (b->orient ? round_up(b->frame_bytes, (size_t)256) : b->frame_bytes) + 256);
-    BALLOC(b->d_resized, N * b->resized_bytes + 256);
+    if (b->geoms.empty()) {
+        BALLOC(b->d_resized, N * b->resized_bytes + 256);
+    } else {
+        size_t all = 0;
+        for (const BatchGeom& g : b->geoms) {
+            b->geom_off.push_back(all);
+            all += N * ((size_t)g.out_w * g.out_h * 3);
+        }
+        BALLOC(b->d_resized, all + 256);
+    }
     if (!b->resize_only) {
         size_t enc = jpeg_encode_scratch_bytes(b->out_w, b->out_h, 3, b->chunk, cfg->out_cap, b->progressive);
         if (b->orient)
@@ -747,6 +779,33 @@ static int batch_launch_chunk(lp_batch* b, int i0, int cnt, cudaStream_t st, cud
         }
         job0 += n1 + n2;
     }
+    if (!b->geoms.empty()) {  // several outputs: the chunk's windows go into each before the next chunk reuses them
+        for (size_t g = 0; g < b->geoms.size(); g++) {
+            const BatchGeom& o = b->geoms[g];
+            const size_t os = (size_t)o.out_w * o.out_h * 3;
+            ResizeArgs r;
+            r.src = b->d_frames;
+            r.src_img_stride = lay.frame_stride;
+            r.src_row_stride = b->frame_bytes / (size_t)b->win_h;
+            r.channels = 3;
+            r.crop_x = o.crop_x - b->win_x0;
+            r.crop_y = o.crop_y - b->crop_y;  // (the window's top row is the union's)
+            r.crop_w = o.crop_w;
+            r.crop_h = o.crop_h;
+            r.dst = b->d_resized + b->geom_off[g] + (size_t)i0 * os;
+            r.dst_img_stride = os;
+            r.dst_row_stride = (size_t)o.out_w * 3;
+            r.dst_w = o.out_w;
+            r.dst_h = o.out_h;
+            r.n = cnt;
+            r.interpolation = 3;
+            rc = resize_launch(r, st);
+            if (rc) return rc;
+        }
+        if (ev)
+            for (int k = 3; k < 6; k++) LP_CUDA_OK(cudaEventRecord(ev[k], st));
+        return LP_OK;
+    }
     uint8_t* const resized = b->d_resized + (size_t)i0 * b->resized_bytes;
     for (int s = 0, at = 0; s < 6; at += count[s++]) {
         if (!count[s]) continue;
@@ -1044,6 +1103,12 @@ extern "C" const uint8_t* lp_batch_decoded_dev(const lp_batch* b, size_t* image_
 extern "C" const uint8_t* lp_batch_resized_dev(const lp_batch* b, size_t* image_stride) {
     if (image_stride) *image_stride = b->resized_bytes;
     return b->d_resized;
+}
+// A context made with several geometries: the resized frames of geometry g
+const uint8_t* lp::batch_resized_geom(const lp_batch* b, int g, size_t* image_stride) {
+    const BatchGeom& o = b->geoms[(size_t)g];
+    *image_stride = (size_t)o.out_w * o.out_h * 3;
+    return b->d_resized + b->geom_off[(size_t)g];
 }
 
 // ---- device helpers + single stages ---------------------------------------------------------

@@ -28,6 +28,14 @@ struct ResizeArgs {
 };
 int resize_launch(const ResizeArgs& a, cudaStream_t st);
 
+// ---- batch.cu (internal) -------------------------------------------------------------------
+// One output of a resize-only lp_batch context that resizes each decoded window into several geometries (lp_xbatch's
+// renditions): the output size and the crop in the source frame
+struct BatchGeom {
+    int out_w, out_h;
+    int crop_x, crop_y, crop_w, crop_h;
+};
+
 // ---- jpeg_parse.cpp (host) -----------------------------------------------------------------
 struct JpegComp {
     int id, h, v, tq, td, ta;
