@@ -16,8 +16,8 @@ import pytest
 from lilliput_b200 import abi
 from lilliput_b200.synth import synth_image
 from tests.test_gpu_xbatch import per_image, rgb_png
-from tests.test_gpu_xbatch_hdr_png import hdr_png, png_file, source
-from tests.test_gpu_xbatch_jpeg_webp import cv2_jpeg, png_profile, with_exif_orientation, with_iccp
+from tests.test_gpu_xbatch_hdr_png import hdr_png, png_file, source, with_cicp
+from tests.test_gpu_xbatch_jpeg_webp import cv2_jpeg, png_profile, webp_still_with_icc, with_exif_orientation, with_iccp
 
 pytestmark = pytest.mark.gpu
 T = 10**12
@@ -205,6 +205,29 @@ def test_gates_that_differ_per_rendition(cuda_lib, xb):
     _, status, st = check_renditions(cuda_lib, xb, data, opts)
     assert st["grid_items"] == len(data) and st["fallback_items"] == 2 * len(data), st
     assert all(s[1] == 0 and s[0] != 0 and s[2] != 0 for s in status), status
+
+
+@pytest.mark.parametrize("kind", ["png", "webp"])
+def test_rendition_skipping_an_item_between_equal_geometries(cuda_lib, xb, kind):
+    """Four files of one geometry, the second of which one rendition sends per image (an SDR cICP chunk keeps a PNG's
+    PNG output per image, an ICC profile a WebP still's WebP output under a zero encode budget); the first three share
+    a task.  The third file is resized from its own decoded frame, not from the second's."""
+    if kind == "png":
+        a, b, c, d = (rgb_png(synth_image(500 + k, 200, 150, 3)) for k in range(4))
+        data, opts = [a, with_cicp(b, 1, 13), c, d], [png(64, 64, FIT), jpeg(64, 64, FIT)]
+        _, _, st = check_renditions(cuda_lib, xb, data, opts)
+    else:
+        # (under a zero budget the grid writes a plain lossy still where lp_transform reports ErrEncodeTimeout, so each
+        # rendition is held against a call with its options alone, whose task has no file in between)
+        a, c, d = (cv2_webp(synth_image(510 + k, 200, 150, 3), 80) for k in range(3))
+        data = [a, webp_still_with_icc(png_profile(), 200, 150, 513), c, d]
+        opts = [webp(64, 64, FIT, EncodeTimeout_ns=0), jpeg(64, 64, FIT)]
+        outs, status = xb.transform_renditions(data, opts, out_cap=CAP)
+        st = xb.stats()
+        for r, o in enumerate(opts):
+            alone, alone_status = xb.transform(data, o, out_cap=CAP)
+            assert [s[r] for s in status] == alone_status and [b[r] for b in outs] == alone, r
+    assert st["grid_items"] == 7 and st["fallback_items"] == 1, st
 
 
 @pytest.mark.parametrize("src", [(640, 360), (360, 640), (257, 255), (1920, 1080)], ids=["wide", "tall", "odd", "1080p"])
