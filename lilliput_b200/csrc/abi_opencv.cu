@@ -209,23 +209,8 @@ static int decode_jpeg_into(const Decoder* d, Mat* m) {
     it.scan_off = 0;
     it.scan_len = (uint32_t)h.scan_length;
     it.table_set = 0;
-    it.width = h.width;
-    it.height = h.height;
-    it.ncomp = h.ncomp;
-    it.mcus_x = h.mcus_x;
-    it.mcus_y = h.mcus_y;
     it.restart_interval = h.restart_interval;
-    uint32_t total_blocks = 0;
-    for (int c = 0; c < h.ncomp; c++) {
-        it.h[c] = h.comp[c].h;
-        it.v[c] = h.comp[c].v;
-        it.dw[c] = (h.width * h.comp[c].h + h.maxh - 1) / h.maxh;
-        it.dh[c] = (h.height * h.comp[c].v + h.maxv - 1) / h.maxv;
-        total_blocks += (uint32_t)h.mcus_x * h.mcus_y * h.comp[c].h * h.comp[c].v;
-        memcpy(it.qt[c], h.qt[h.comp[c].tq], sizeof(it.qt[c]));
-        it.td[c] = h.comp[c].td;
-        it.ta[c] = h.comp[c].ta;
-    }
+    const uint32_t total_blocks = jpeg_decode_item(h, &it);
     uint32_t tiles = 0;
     const uint32_t blocks = jpeg_item_set_window(&it, 0, 0, h.width, h.height, false, &tiles);  // whole image
     if (!parallel) {  // its scans are [0, nscans) of d_scans; the whole frame is the window, so no masks
@@ -233,7 +218,6 @@ static int decode_jpeg_into(const Decoder* d, Mat* m) {
         it.table_set = 0;
         it.nscans = (uint32_t)nscans;
     }
-    it.frame_channels = h.ncomp == 1 ? 1 : 3;
 
     uint8_t* scratch = nullptr;
     const size_t upload_len = parallel ? h.scan_length : d->len;  // walked scan by scan: the whole file
@@ -298,25 +282,7 @@ static int decode_png_into(const Decoder* d, Mat* m) {
     if (h.idat_total < 2) return LP_ERR_DECODING_FAILED;
     cudaStream_t st = thread_stream();
     PngDecodeItem it;
-    memset(&it, 0, sizeof(it));
-    it.z_len = (uint32_t)h.idat_total;
-    it.width = h.width;
-    it.height = h.height;
-    it.bit_depth = h.bit_depth;
-    it.color_type = h.color_type;
-    it.src_channels = h.src_channels;
-    it.out_channels = h.out_channels;
-    it.bpp = h.bpp;
-    it.row_bytes = (uint32_t)h.row_bytes;
-    it.frame_stride = (uint32_t)m->dev_step;
-    it.interlace = h.interlace ? 1 : 0;
-    png_item_set_passes(&it);
-    it.npal = h.npal;
-    it.ntrns = h.ntrns;
-    it.has_trns = h.has_trns;
-    memcpy(it.trns_rgb, h.trns_rgb, sizeof(it.trns_rgb));
-    memcpy(it.palette, h.palette, sizeof(it.palette));
-    memcpy(it.trns, h.trns, sizeof(it.trns));
+    png_decode_item(h, (uint32_t)m->dev_step, &it);
     // the IDAT payloads form ONE zlib stream: gather them on the host, one H2D copy
     std::vector<uint8_t> z(h.idat_total + 16, 0);
     size_t o = 0;

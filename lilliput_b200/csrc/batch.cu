@@ -517,18 +517,8 @@ static int batch_parse_chunk(lp_batch* b, const uint8_t* const* in, const size_t
             memset(&it, 0, sizeof(it));
             if (!rc) {
                 it.scan_len = (uint32_t)(ms ? in_len[k] : h.scan_length);  // multi-scan: the whole file
-                it.width = h.width; it.height = h.height; it.ncomp = h.ncomp;
-                it.mcus_x = h.mcus_x; it.mcus_y = h.mcus_y; it.restart_interval = ms ? 0 : h.restart_interval;
-                uint32_t total_blocks = 0;
-                for (int c = 0; c < h.ncomp; c++) {
-                    it.h[c] = h.comp[c].h; it.v[c] = h.comp[c].v;
-                    it.dw[c] = (h.width * h.comp[c].h + h.maxh - 1) / h.maxh;
-                    it.dh[c] = (h.height * h.comp[c].v + h.maxv - 1) / h.maxv;
-                    total_blocks += (uint32_t)h.mcus_x * h.mcus_y * h.comp[c].h * h.comp[c].v;
-                    memcpy(it.qt[c], h.qt[h.comp[c].tq], sizeof(it.qt[c]));
-                    it.td[c] = h.comp[c].td; it.ta[c] = h.comp[c].ta;
-                }
-                it.frame_channels = h.ncomp == 1 ? 1 : 3;
+                it.restart_interval = ms ? 0 : h.restart_interval;
+                const uint32_t total_blocks = jpeg_decode_item(h, &it);
                 // decode only what Fit will read: the crop window (+ the chroma-upsampling margin); a rotated item's
                 // crop is in its oriented frame, and the window is that crop's pre-image in the source
                 int x0 = b->crop_x, y0 = b->crop_y, x1 = b->crop_x + b->crop_w, y1 = b->crop_y + b->crop_h;

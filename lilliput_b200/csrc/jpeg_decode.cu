@@ -17,6 +17,8 @@
 //                             conversion from there into the packed BGR frame.
 // Scans without restart markers go to the self-synchronising decoder (jpeg_huff_parallel.cu).  Every entropy decoder
 // writes quantised coefficients (int16, natural order) in scan order and clears the blocks it writes.
+#include <cstring>
+
 #include "common.cuh"
 #include "kernels.cuh"
 #include "jpeg_scan_core.h"
@@ -64,7 +66,28 @@ __host__ __device__ inline TileLayout tile_layout(const JpegDecodeItem& it, int 
     return L;
 }
 
-// ------------------------------------------------------------------ ROI layout (host)
+// ------------------------------------------------------------------ item and ROI layout (host)
+
+uint32_t jpeg_decode_item(const JpegHeader& h, JpegDecodeItem* it) {
+    it->width = h.width;
+    it->height = h.height;
+    it->ncomp = h.ncomp;
+    it->mcus_x = h.mcus_x;
+    it->mcus_y = h.mcus_y;
+    uint32_t total_blocks = 0;
+    for (int c = 0; c < h.ncomp; c++) {
+        it->h[c] = h.comp[c].h;
+        it->v[c] = h.comp[c].v;
+        it->dw[c] = (h.width * h.comp[c].h + h.maxh - 1) / h.maxh;
+        it->dh[c] = (h.height * h.comp[c].v + h.maxv - 1) / h.maxv;
+        total_blocks += (uint32_t)h.mcus_x * h.mcus_y * h.comp[c].h * h.comp[c].v;
+        memcpy(it->qt[c], h.qt[h.comp[c].tq], sizeof(it->qt[c]));
+        it->td[c] = h.comp[c].td;
+        it->ta[c] = h.comp[c].ta;
+    }
+    it->frame_channels = h.ncomp == 1 ? 1 : 3;
+    return total_blocks;
+}
 
 uint32_t jpeg_item_set_window(JpegDecodeItem* it, int x0, int y0, int x1, int y1, bool align16,
                               uint32_t* tiles_out) {

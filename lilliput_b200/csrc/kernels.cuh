@@ -64,6 +64,9 @@ int jpeg_parse_header(const uint8_t* data, size_t len, JpegHeader* out);
 
 // ---- jpeg_decode.cu ------------------------------------------------------------------------
 
+// Fills the header-derived fields of a zeroed `it`: geometry, MCUs, per-component sampling, downsampled sizes,
+// quantisation tables, table selectors and frame_channels.  Returns the blocks of the whole frame.
+uint32_t jpeg_decode_item(const JpegHeader& h, JpegDecodeItem* it);
 // Fills the ROI / window / layout fields of `it` (whose width, height, ncomp, h, v, mcus_* are set)
 // for the pixel window [x0,x1) x [y0,y1).  align16 rounds the window's x range outwards to 16 px so
 // the vectorised colour step can use 16-byte stores.  Returns blocks in the ROI; *tiles (if given) = the CTAs
@@ -192,8 +195,9 @@ struct PngDecodeItem {
     uint32_t pass_off[7], pass_rb[7];  // byte offset / scanline bytes (without the filter byte)
     int32_t pass_w[7], pass_h[7];
 };
-// Fills npass / raw_total / pass_* from width, height, bit depth, channels, interlace.
-void png_item_set_passes(PngDecodeItem* it);
+// The item of a parsed PNG, zeroed and filled from the header: geometry, format, palette, tRNS and the Adam7 passes
+// (npass / raw_total / pass_*).  The caller sets z_off, raw_off and frame_off.
+void png_decode_item(const PngHeader& h, uint32_t frame_stride, PngDecodeItem* it);
 struct PngDecodeBatch {
     PngDecodeItem* items;  // device
     const uint8_t* z;      // device: zlib streams
@@ -278,6 +282,7 @@ struct WebpFramePlan {
     int duration = 0;
     int dispose = 0;  // 1 = dispose to background (clear the rectangle after the frame)
     int blend = 0;    // 1 = do not blend (copy the rectangle)
+    bool has_alpha = false;  // an ALPH chunk, or the VP8L header's alpha bit
 };
 struct WebpPlan {
     int width = 0, height = 0, channels = 3;  // canvas; 4 when the container has the alpha flag

@@ -14,6 +14,8 @@
 //                        that "up" comes from lane r-1 by shuffle and "left"/"upper-left" stay in
 //                        registers (Sub/Up/Average/Paeth, modulo 256), in place.
 //   png_convert_kernel   one thread per output pixel.
+#include <cstring>
+
 #include "common.cuh"
 #include "kernels.cuh"
 #include "inflate_core.h"
@@ -354,7 +356,25 @@ extern "C" void lp_png_inflate_stats(unsigned long long* out16, int reset) {
 }
 #endif
 
-void png_item_set_passes(PngDecodeItem* it) {
+void png_decode_item(const PngHeader& h, uint32_t frame_stride, PngDecodeItem* it) {
+    memset(it, 0, sizeof(*it));
+    it->z_len = (uint32_t)h.idat_total;
+    it->width = h.width;
+    it->height = h.height;
+    it->bit_depth = h.bit_depth;
+    it->color_type = h.color_type;
+    it->src_channels = h.src_channels;
+    it->out_channels = h.out_channels;
+    it->bpp = h.bpp;
+    it->row_bytes = (uint32_t)h.row_bytes;
+    it->frame_stride = frame_stride;
+    it->npal = h.npal;
+    it->ntrns = h.ntrns;
+    it->has_trns = h.has_trns;
+    memcpy(it->trns_rgb, h.trns_rgb, sizeof(it->trns_rgb));
+    memcpy(it->palette, h.palette, sizeof(it->palette));
+    memcpy(it->trns, h.trns, sizeof(it->trns));
+    it->interlace = h.interlace ? 1 : 0;
     static const int X0[7] = {0, 4, 0, 2, 0, 1, 0}, Y0[7] = {0, 0, 4, 0, 2, 0, 1};
     static const int DX[7] = {8, 8, 4, 4, 2, 2, 1}, DY[7] = {8, 8, 8, 4, 4, 2, 2};
     const size_t bits = (size_t)it->src_channels * it->bit_depth;

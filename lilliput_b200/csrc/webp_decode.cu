@@ -10,8 +10,9 @@
 // streams whose contexts chain through the picture, so the unit of parallelism is the frame: one
 // warp per frame.  Lane 0 walks the bitstream and reconstructs macroblocks into the frame's YUV
 // planes in HBM; the loop filter then runs warp-wide (32 lanes = the 16 luma + 8 + 8 chroma sample
-// positions of one macroblock edge); a second, fully parallel kernel does libwebp's "fancy"
-// chroma upsampling and the fixed-point YUV->BGR(A) conversion per output pixel.
+// positions of one macroblock edge); the compositor (webp_compose_kernel), fully parallel, does libwebp's
+// "fancy" chroma upsampling and the fixed-point YUV->BGR(A) conversion per output pixel.  The per-image
+// decoder runs each frame through the same launches as the batch (webp_decode_batch with one file).
 #include <algorithm>
 #include <cstring>
 #include <vector>
@@ -299,30 +300,9 @@ __global__ void __launch_bounds__(kVp8WarpsPerBlock * 32) vp8_decode_kernel(cons
         for (int mb_x = 0; mb_x < mb_w; mb_x++) filter_macroblock_warp(h, w, mb_x, mb_y, lane);
 }
 
-// Upsampling + colour conversion of decoded frames of one geometry, blockIdx.z = frame: work areas `work_stride` apart,
-// frames `dst_stride` apart in dst, rows `dst_step` apart.  channels 3 or 4; the fourth byte comes from `alpha` (a
-// width x height plane, one-frame launches only) or is 255.
-__global__ void vp8_output_kernel(uint8_t* work, size_t work_stride, int mb_w, int mb_h, int width, int height, uint8_t* dst,
-                                  size_t dst_stride, size_t dst_step, int channels, const uint8_t* alpha) {
-    const int x = blockIdx.x * blockDim.x + threadIdx.x;
-    const int y = blockIdx.y;
-    if (x >= width) return;
-    vp8::Work w;
-    vp8::work_carve(work + (size_t)blockIdx.z * work_stride, mb_w, mb_h, w);
-    const int u = vp8::upsample_at(w.u, mb_w * 8, width, height, x, y);
-    const int v = vp8::upsample_at(w.v, mb_w * 8, width, height, x, y);
-    uint8_t bgr[3];
-    vp8::yuv_to_bgr(w.y[(size_t)y * (mb_w * 16) + x], u, v, bgr);
-    uint8_t* d = dst + (size_t)blockIdx.z * dst_stride + (size_t)y * dst_step + (size_t)x * channels;
-    d[0] = bgr[0];
-    d[1] = bgr[1];
-    d[2] = bgr[2];
-    if (channels == 4) d[3] = alpha ? alpha[(size_t)y * width + x] : 255;
-}
-
 // VP8L (lossless) frames and ALPH planes: an LZ77 + prefix-coded stream is one serial chain, so
 // lane 0 of one warp per stream walks it (vp8l_core.h) inside its own slice of a bump arena in HBM.
-// The colour-order conversion to the mat (or to the canvas) is a separate, parallel kernel.
+// The colour-order conversion onto the canvas is the compositor's.
 struct Vp8lItem {
     const uint8_t* data;   // "VP8L" chunk payload, or "ALPH" chunk payload
     uint32_t size;
@@ -331,8 +311,7 @@ struct Vp8lItem {
     size_t arena_cap;
     int is_alph;
     uint8_t* alpha_out;    // is_alph: width*height plane
-    uint32_t** px_out;     // !is_alph, or null: where to leave the pointer to the final ARGB pixels
-    uint32_t* argb_out;    // !is_alph, or null: where the warp copies them (the arena is reused by the next wave)
+    uint32_t* argb_out;    // !is_alph: where the warp copies the final ARGB pixels (the arena is reused by the next wave)
     int* status;
 };
 
@@ -350,16 +329,28 @@ __global__ void __launch_bounds__(kVp8lWarpsPerBlock * 32) vp8l_decode_kernel(co
             rc = vp8l::decode_alph(it.data, it.size, it.width, it.height, a, it.alpha_out);
         } else {
             rc = vp8l::decode_vp8l(it.data, it.size, it.width, it.height, a, &px);
-            if (it.px_out) *it.px_out = px;
         }
         if (rc) *it.status = rc;
     }
-    if (it.is_alph || !it.argb_out) return;
+    if (it.is_alph) return;
     rc = __shfl_sync(0xffffffffu, rc, 0);
     px = reinterpret_cast<uint32_t*>(__shfl_sync(0xffffffffu, reinterpret_cast<unsigned long long>(px), 0));
     if (rc || !px) return;
-    const size_t npix = (size_t)it.width * it.height;
-    for (size_t i = lane; i < npix; i += 32) it.argb_out[i] = px[i];
+    // One warp copies the frame, so it keeps eight 16-byte loads in flight per lane (arena allocations and scratch slots
+    // are 16-byte aligned).  The pixels were written in this launch: plain loads, not the read-only path.
+    const size_t npix = (size_t)it.width * it.height, nvec = npix / 4;
+    const uint4* src = reinterpret_cast<const uint4*>(px);
+    uint4* dst = reinterpret_cast<uint4*>(it.argb_out);
+    size_t i = lane;
+    for (; i + 7 * 32 < nvec; i += 8 * 32) {
+        uint4 v[8];
+#pragma unroll
+        for (int u = 0; u < 8; u++) v[u] = src[i + u * 32];
+#pragma unroll
+        for (int u = 0; u < 8; u++) dst[i + u * 32] = v[u];
+    }
+    for (; i < nvec; i += 32) dst[i] = src[i];
+    for (size_t j = nvec * 4 + lane; j < npix; j += 32) it.argb_out[j] = px[j];
 }
 
 static int vp8l_decode_launch(const Vp8lItem* d_items, int n, cudaStream_t st) {
@@ -424,20 +415,6 @@ __global__ void webp_compose_kernel(const WebpAnimJob* anims, const WebpFrameJob
         for (int c = 0; c < ch; c++) d[c] = px[c];
         if (inside && f.dispose) px[0] = px[1] = px[2] = px[3] = 0;
     }
-}
-
-__global__ void argb_output_kernel(uint32_t* const* px_ptr, int width, int height, uint8_t* dst, size_t dst_step,
-                                   int channels) {
-    const int x = blockIdx.x * blockDim.x + threadIdx.x;
-    const int y = blockIdx.y;
-    const uint32_t* px = *px_ptr;
-    if (x >= width || !px) return;
-    const uint32_t v = px[(size_t)y * width + x];
-    uint8_t* d = dst + (size_t)y * dst_step + (size_t)x * channels;
-    d[0] = (uint8_t)v;
-    d[1] = (uint8_t)(v >> 8);
-    d[2] = (uint8_t)(v >> 16);
-    if (channels == 4) d[3] = (uint8_t)(v >> 24);
 }
 
 // ------------------------------------------------------------------ container walk (host)
@@ -665,6 +642,7 @@ bool webp_plan_parse(const uint8_t* data, size_t len, WebpPlan* out) {
         p.duration = f.duration;
         p.dispose = f.dispose;
         p.blend = f.blend;
+        p.has_alpha = f.has_alpha;
         out->frames.push_back(p);
     }
     return true;
@@ -676,9 +654,9 @@ size_t webp_plan_first_frame(WebpPlan* p) {
     return std::max(f.img_off + f.img_len, f.has_alph ? f.alph_off + f.alph_len : 0);
 }
 
-// the per-image decoder's VP8L arena bound, per stream
+// the VP8L arena bound, per stream
 static size_t vp8l_slice_bytes(const WebpFramePlan& f) { return round_up((size_t)f.width * f.height * 12 + (16u << 20), (size_t)256); }
-// the ALPH plane is decoded only onto a 4-channel canvas (webp_decoder_decode's need_alph)
+// the ALPH plane is decoded only onto a 4-channel canvas (3 channels drop it)
 static bool frame_needs_alph(const WebpPlan& p, const WebpFramePlan& f) { return f.has_alph && !f.lossless && p.channels == 4; }
 static size_t file_slot_bytes(size_t file_len) { return round_up(file_len + 4096, (size_t)256); }
 // VP8 work area, lossless ARGB words or the ALPH plane of one frame
@@ -758,7 +736,7 @@ int webp_decode_batch(const WebpPlan* const* plans, const uint8_t* const* files,
             const size_t npix = (size_t)f.width * f.height;
             if (f.lossless) {
                 j.px_off = take(npix * 4);
-                vp8l.push_back(Vp8lItem{d_file + f.img_off, (uint32_t)f.img_len, f.width, f.height, nullptr, 0, 0, nullptr, nullptr,
+                vp8l.push_back(Vp8lItem{d_file + f.img_off, (uint32_t)f.img_len, f.width, f.height, nullptr, 0, 0, nullptr,
                                         reinterpret_cast<uint32_t*>(d_scratch + j.px_off), d_status + k});
                 slice.push_back(vp8l_slice_bytes(f));
             } else {
@@ -767,7 +745,7 @@ int webp_decode_batch(const WebpPlan* const* plans, const uint8_t* const* files,
                 if (frame_needs_alph(p, f)) {
                     j.px_off = take(npix);
                     vp8l.push_back(Vp8lItem{d_file + f.alph_off, (uint32_t)f.alph_len, f.width, f.height, nullptr, 0, 1,
-                                            d_scratch + j.px_off, nullptr, nullptr, d_status + k});
+                                            d_scratch + j.px_off, nullptr, d_status + k});
                     slice.push_back(vp8l_slice_bytes(f));
                 }
             }
@@ -846,24 +824,15 @@ using namespace lp;
 
 struct webp_decoder_struct {
     const uint8_t* bytes = nullptr;
-    size_t len = 0;
-    WebpContainer c;
-    bool has_alpha = false, has_animation = false;
+    WebpPlan plan;
     int total_duration = 0;
     int current_frame_index = 1;
     int prev_delay = 0, prev_x = 0, prev_y = 0, prev_dispose = 0, prev_blend = 0;
     bool prev_has_alpha = false;
-    // device scratch, grown on demand
-    uint8_t* d_in = nullptr;
-    uint8_t* d_work = nullptr;
-    Vp8Item* d_item = nullptr;
-    Vp8lItem* d_litem = nullptr;
-    int* d_status = nullptr;
-    uint8_t* d_arena = nullptr;   // VP8L / ALPH bump arena
-    uint8_t* d_alpha = nullptr;   // decoded ALPH plane
-    uint8_t* d_alph_in = nullptr; // ALPH chunk bytes
-    uint32_t** d_px = nullptr;    // where the VP8L kernel leaves its result pointer
-    size_t in_cap = 0, work_cap = 0, arena_cap = 0, alpha_cap = 0, alph_in_cap = 0;
+    // device scratch of webp_decode_batch (webp_plan_device_bytes) and its VP8L / ALPH arena, grown on demand
+    uint8_t* d_scratch = nullptr;
+    uint8_t* d_arena = nullptr;
+    size_t scratch_cap = 0, arena_cap = 0;
 };
 
 extern "C" {
@@ -876,27 +845,19 @@ webp_decoder webp_decoder_create(const opencv_mat buf) {
     if (!bytes) return nullptr;
     auto* d = new webp_decoder_struct;
     d->bytes = bytes;
-    d->len = len;
-    if (!webp_parse(bytes, len, &d->c)) {
+    if (!webp_plan_parse(bytes, len, &d->plan)) {
         delete d;
         return nullptr;
     }
-    d->has_alpha = (d->c.flags & kFlagAlpha) != 0;
-    for (const WebpFrame& f : d->c.frames) d->total_duration += f.duration;
-    d->c.bgcolor = (d->c.flags & kFlagAnim) ? d->c.bgcolor : 0xFFFFFFFFu;
-    if (d->c.flags & kFlagAnim) {
-        d->has_animation = true;
-    } else {
-        d->total_duration = 0;
-        d->c.loop_count = 0;
-    }
+    if (d->plan.animated)
+        for (const WebpFramePlan& f : d->plan.frames) d->total_duration += f.duration;
     return d;
 }
 
-int webp_decoder_get_width(const webp_decoder d) { return d->c.canvas_w; }
-int webp_decoder_get_height(const webp_decoder d) { return d->c.canvas_h; }
-int webp_decoder_get_pixel_type(const webp_decoder d) { return d->has_alpha ? CV_8UC4 : CV_8UC3; }
-int webp_decoder_get_num_frames(const webp_decoder d) { return d ? (int)d->c.frames.size() : 0; }
+int webp_decoder_get_width(const webp_decoder d) { return d->plan.width; }
+int webp_decoder_get_height(const webp_decoder d) { return d->plan.height; }
+int webp_decoder_get_pixel_type(const webp_decoder d) { return d->plan.channels == 4 ? CV_8UC4 : CV_8UC3; }
+int webp_decoder_get_num_frames(const webp_decoder d) { return d ? (int)d->plan.frames.size() : 0; }
 int webp_decoder_get_total_duration(const webp_decoder d) { return d ? d->total_duration : 0; }
 int webp_decoder_get_prev_frame_delay(const webp_decoder d) { return d->prev_delay; }
 int webp_decoder_get_prev_frame_dispose(const webp_decoder d) { return d->prev_dispose; }
@@ -904,32 +865,25 @@ int webp_decoder_get_prev_frame_blend(const webp_decoder d) { return d->prev_ble
 int webp_decoder_get_prev_frame_x_offset(const webp_decoder d) { return d->prev_x; }
 int webp_decoder_get_prev_frame_y_offset(const webp_decoder d) { return d->prev_y; }
 bool webp_decoder_get_prev_frame_has_alpha(const webp_decoder d) { return d->prev_has_alpha; }
-uint32_t webp_decoder_get_bg_color(const webp_decoder d) { return d->c.bgcolor; }
-uint32_t webp_decoder_get_loop_count(const webp_decoder d) { return d->c.loop_count; }
+uint32_t webp_decoder_get_bg_color(const webp_decoder d) { return d->plan.bgcolor; }
+uint32_t webp_decoder_get_loop_count(const webp_decoder d) { return d->plan.loop_count; }
 
 // ref webp.cpp:251-262
 size_t webp_decoder_get_icc(const webp_decoder d, void* dst, size_t dst_len) {
-    if (!d->c.has_icc || d->c.icc_len == 0 || d->c.icc_len > dst_len) return 0;
-    memcpy(dst, d->bytes + d->c.icc_off, d->c.icc_len);
-    return d->c.icc_len;
+    if (d->plan.icc_len == 0 || d->plan.icc_len > dst_len) return 0;
+    memcpy(dst, d->bytes + d->plan.icc_off, d->plan.icc_len);
+    return d->plan.icc_len;
 }
 
 // ref webp.cpp:269-281
-int webp_decoder_has_more_frames(webp_decoder d) { return d->current_frame_index < (int)d->c.frames.size(); }
+int webp_decoder_has_more_frames(webp_decoder d) { return d->current_frame_index < (int)d->plan.frames.size(); }
 void webp_decoder_advance_frame(webp_decoder d) { d->current_frame_index++; }
 
 void webp_decoder_release(webp_decoder d) {
     if (!d) return;
     cudaStream_t st = thread_stream();
-    if (d->d_in) cudaFreeAsync(d->d_in, st);
-    if (d->d_work) cudaFreeAsync(d->d_work, st);
-    if (d->d_item) cudaFreeAsync(d->d_item, st);
-    if (d->d_litem) cudaFreeAsync(d->d_litem, st);
-    if (d->d_status) cudaFreeAsync(d->d_status, st);
+    if (d->d_scratch) cudaFreeAsync(d->d_scratch, st);
     if (d->d_arena) cudaFreeAsync(d->d_arena, st);
-    if (d->d_alpha) cudaFreeAsync(d->d_alpha, st);
-    if (d->d_alph_in) cudaFreeAsync(d->d_alph_in, st);
-    if (d->d_px) cudaFreeAsync(d->d_px, st);
     cudaStreamSynchronize(st);
     delete d;
 }
@@ -937,73 +891,56 @@ void webp_decoder_release(webp_decoder d) {
 // ref webp.cpp:291-359
 bool webp_decoder_decode(const webp_decoder d, opencv_mat mat) {
     if (!d || !mat) return false;
-    if (d->current_frame_index < 1 || d->current_frame_index > (int)d->c.frames.size()) return false;
-    const WebpFrame& f = d->c.frames[d->current_frame_index - 1];
+    if (d->current_frame_index < 1 || d->current_frame_index > (int)d->plan.frames.size()) return false;
+    const WebpFramePlan& f = d->plan.frames[d->current_frame_index - 1];
     const int type = webp_decoder_get_pixel_type(d);
     uint8_t* frame_dev = nullptr;
     size_t frame_step = 0;
     if (mat_bind_device_frame(mat, f.width, f.height, type, &frame_dev, &frame_step) != 0) return false;
     d->prev_delay = f.duration;
-    d->prev_x = f.x_off;
-    d->prev_y = f.y_off;
+    d->prev_x = f.x;
+    d->prev_y = f.y;
     d->prev_dispose = f.dispose;
     d->prev_blend = f.blend;
     d->prev_has_alpha = f.has_alpha;
+    // the compositor writes packed rows, as a freshly bound mat has them
+    if (frame_step != (size_t)f.width * d->plan.channels) return false;
+    // The frame alone, as the batch decodes a still: a canvas of the frame's size with the frame copied at its origin.
+    // Only the frame's own chunks go up (an ALPH chunk precedes its image), with offsets from the first of them.
+    const size_t begin = f.has_alph ? f.alph_off : f.img_off;
+    WebpPlan one;
+    one.width = f.width;
+    one.height = f.height;
+    one.channels = d->plan.channels;
+    one.frames.push_back(f);
+    WebpFramePlan& g = one.frames[0];
+    g.img_off -= begin;
+    g.alph_off = 0;
+    g.x = g.y = 0;
+    g.blend = 1;
+    g.dispose = 0;
+    const uint8_t* file = d->bytes + begin;
+    const size_t span = f.img_off + f.img_len - begin;
     cudaStream_t st = thread_stream();
-    const int channels = type == CV_8UC4 ? 4 : 3;
     auto grow = [&](uint8_t** p, size_t* cap, size_t need) -> bool {
         if (need <= *cap) return true;
         if (*p) cudaFreeAsync(*p, st);
-        *cap = need;
-        return cudaMallocAsync(p, need, st) == cudaSuccess;
-    };
-    if (!d->d_item) {
-        if (cudaMallocAsync(&d->d_item, sizeof(Vp8Item), st) != cudaSuccess) return false;
-        if (cudaMallocAsync(&d->d_litem, sizeof(Vp8lItem), st) != cudaSuccess) return false;
-        if (cudaMallocAsync(&d->d_status, sizeof(int), st) != cudaSuccess) return false;
-        if (cudaMallocAsync(&d->d_px, sizeof(uint32_t*), st) != cudaSuccess) return false;
-    }
-    cudaMemsetAsync(d->d_status, 0, sizeof(int), st);
-    cudaMemsetAsync(d->d_px, 0, sizeof(uint32_t*), st);
-    if (!grow(&d->d_in, &d->in_cap, f.img_len + 4096)) return false;
-    cudaMemcpyAsync(d->d_in, d->bytes + f.img_off, f.img_len, cudaMemcpyHostToDevice, st);
-    const size_t npix = (size_t)f.width * f.height;
-    const size_t arena_need = npix * 12 + (16u << 20);
-    const bool need_alph = f.has_alph && !f.lossless && channels == 4;
-    if (f.lossless || need_alph) {
-        if (!grow(&d->d_arena, &d->arena_cap, arena_need)) return false;
-    }
-    if (f.lossless) {
-        Vp8lItem li{d->d_in, (uint32_t)f.img_len, f.width, f.height, d->d_arena, d->arena_cap, 0, nullptr, d->d_px, nullptr, d->d_status};
-        cudaMemcpyAsync(d->d_litem, &li, sizeof(li), cudaMemcpyHostToDevice, st);
-        if (vp8l_decode_launch(d->d_litem, 1, st)) return false;
-        dim3 grid(ceil_div(f.width, 128), f.height);
-        argb_output_kernel<<<grid, 128, 0, st>>>(d->d_px, f.width, f.height, frame_dev, frame_step, channels);
-        g_launches++;
-    } else {
-        const int mb_w = (f.width + 15) >> 4, mb_h = (f.height + 15) >> 4;
-        if (!grow(&d->d_work, &d->work_cap, vp8::work_bytes(mb_w, mb_h))) return false;
-        if (need_alph) {
-            if (!grow(&d->d_alph_in, &d->alph_in_cap, f.alph_len + 4096)) return false;
-            if (!grow(&d->d_alpha, &d->alpha_cap, npix + 256)) return false;
-            cudaMemcpyAsync(d->d_alph_in, d->bytes + f.alph_off, f.alph_len, cudaMemcpyHostToDevice, st);
-            Vp8lItem ai{d->d_alph_in, (uint32_t)f.alph_len, f.width, f.height, d->d_arena, d->arena_cap, 1, d->d_alpha, nullptr, nullptr, d->d_status};
-            cudaMemcpyAsync(d->d_litem, &ai, sizeof(ai), cudaMemcpyHostToDevice, st);
-            if (vp8l_decode_launch(d->d_litem, 1, st)) return false;
+        *cap = 0;
+        if (cudaMallocAsync(p, need, st) != cudaSuccess) {
+            *p = nullptr;
+            return false;
         }
-        Vp8Item item{d->d_in, (uint32_t)f.img_len, d->d_work, d->d_status, mb_w, mb_h};
-        cudaMemcpyAsync(d->d_item, &item, sizeof(item), cudaMemcpyHostToDevice, st);
-        vp8_decode_kernel<<<1, kVp8WarpsPerBlock * 32, 0, st>>>(d->d_item, 1);
-        g_launches++;
-        dim3 grid(ceil_div(f.width, 128), f.height);
-        vp8_output_kernel<<<grid, 128, 0, st>>>(d->d_work, 0, mb_w, mb_h, f.width, f.height, frame_dev, 0, frame_step, channels,
-                                                need_alph ? d->d_alpha : nullptr);
-        g_launches++;
-    }
+        *cap = need;
+        return true;
+    };
+    if (!grow(&d->d_scratch, &d->scratch_cap, webp_plan_device_bytes(one, span))) return false;
+    if (!grow(&d->d_arena, &d->arena_cap, webp_plan_arena_bytes(one))) return false;
+    const WebpPlan* plans[1] = {&one};
+    const uint64_t canvas_off = 0;
     int status = 0;
-    cudaMemcpyAsync(&status, d->d_status, sizeof(int), cudaMemcpyDeviceToHost, st);
-    if (cudaStreamSynchronize(st) != cudaSuccess) return false;
-    if (status != 0) return false;
+    if (webp_decode_batch(plans, &file, &span, 1, d->d_scratch, d->scratch_cap, d->d_arena, d->arena_cap, frame_dev,
+                          &canvas_off, &status, nullptr, st) != LP_OK || status != 0)
+        return false;
     mat_mark_device_written(mat);
     return true;
 }

@@ -767,25 +767,7 @@ static void run_png(lp_xbatch* X, Lane& L, const Task& t) {
         const XItem& xi = X->items[rep[k]];
         const PngHeader& ph = *xi.png;
         PngDecodeItem& it = items[k];
-        memset(&it, 0, sizeof(it));
-        it.z_len = (uint32_t)ph.idat_total;
-        it.width = ph.width;
-        it.height = ph.height;
-        it.bit_depth = ph.bit_depth;
-        it.color_type = ph.color_type;
-        it.src_channels = ph.src_channels;
-        it.out_channels = ph.out_channels;
-        it.bpp = ph.bpp;
-        it.row_bytes = (uint32_t)ph.row_bytes;
-        it.frame_stride = (uint32_t)((size_t)xi.w * xi.ch);
-        it.interlace = ph.interlace ? 1 : 0;
-        png_item_set_passes(&it);
-        it.npal = ph.npal;
-        it.ntrns = ph.ntrns;
-        it.has_trns = ph.has_trns;
-        memcpy(it.trns_rgb, ph.trns_rgb, sizeof(it.trns_rgb));
-        memcpy(it.palette, ph.palette, sizeof(it.palette));
-        memcpy(it.trns, ph.trns, sizeof(it.trns));
+        png_decode_item(ph, (uint32_t)((size_t)xi.w * xi.ch), &it);
         if (ph.idat.size() == 1) {
             it.z_off = file_off[k];
         } else {
