@@ -258,6 +258,37 @@ int lp_xbatch_transform_renditions(lp_xbatch* x, const uint8_t* const* in, const
                                    const lp_image_options* opts, int k, uint8_t* const* out, size_t out_cap,
                                    size_t* out_len, int* status);
 
+/* Pixels instead of files: the frame every item would be encoded from, written into the caller's device tensor.
+ * Item i's frame is the one lp_transform(in[i], opt with file_type ".png") hands to its encoder: decoded, tone-mapped
+ * if HDR, oriented, with Fit / Resize / NoResize applied; of a GIF or animated WebP, frame 0 composited as Transform
+ * composites it.  status[i] is that call's status, width[i] x height[i] the frame's size.  opt->file_type and the
+ * encode options are ignored.
+ *   - slice i of dst (item i's H x W x C or C x H x W elements) holds the frame at its top-left, zero elsewhere
+ *   - a gray frame is replicated to three channels; an opaque one gets 255 as channel 3 when channels == 4; a BGRA
+ *     frame's alpha is dropped (not composited) when channels == 3
+ *   - a frame larger than the box in either dimension: LP_ERR_BUF_TOO_SMALL
+ *   - an item whose status is not LP_OK: an all-zero slice and 0 x 0
+ * dst must stay allocated for the call, on the context's device; every write into it is complete when the call
+ * returns.  LP_ERR_BAD_ARGUMENT, with nothing written, for: n < 0; null in / in_len / opt / width / height / status
+ * with n > 0; a null dst or data; data not device memory of the context's device, or not aligned to the dtype;
+ * bytes < n slices; height or width < 1; channels not 3 or 4; an unknown dtype.
+ * Stats: grid_items / fallback_items count items; ms_encode is the pack; d2h_bytes carries no pixels. */
+enum { LP_DTYPE_U8 = 0, LP_DTYPE_F16 = 1, LP_DTYPE_BF16 = 2, LP_DTYPE_F32 = 3 };
+typedef struct lp_frame_tensor {
+    void* data;              /* device memory on the context's device */
+    size_t bytes;            /* capacity of data */
+    int height, width;       /* box per item: item i's frame at its top-left, the rest of its slice zero */
+    int channels;            /* 3 or 4 */
+    int nchw;                /* 0: N x H x W x C, 1: N x C x H x W (dense, item i is slice i) */
+    int rgb;                 /* 0: B, G, R[, A]   1: R, G, B[, A] */
+    int dtype;               /* LP_DTYPE_* */
+    float scale[4], bias[4]; /* float dtypes: out[c] = fmaf(sample, scale[c], bias[c]) in fp32, then rounded to
+                                nearest into the dtype; indexed by OUTPUT channel; ignored for U8 */
+} lp_frame_tensor;
+int lp_xbatch_decode_frames(lp_xbatch* x, const uint8_t* const* in, const size_t* in_len, int n,
+                            const lp_image_options* opt, const lp_frame_tensor* dst, int* width, int* height,
+                            int* status);
+
 /* ---- the same call over several GPUs of one node (SURVEY 8(e): shard by image index, no collective) ----
  * One lp_xbatch per device behind one call: the batch is cut into contiguous blocks balanced by compressed bytes,
  * every block runs on its own GPU from its own host thread, results land in the caller's arrays by index. */

@@ -470,6 +470,16 @@ class _XBatchStats(C.Structure):
                 ("h2d_bytes", C.c_size_t), ("d2h_bytes", C.c_size_t), ("ms_busy_max_lane", C.c_double)]
 
 
+# lp_frame_tensor dtypes (lp_xbatch_decode_frames)
+FRAME_DTYPES = {"u8": 0, "f16": 1, "bf16": 2, "f32": 3}
+
+
+class _FrameTensor(C.Structure):
+    _fields_ = [("data", C.c_void_p), ("bytes", C.c_size_t), ("height", C.c_int), ("width", C.c_int),
+                ("channels", C.c_int), ("nchw", C.c_int), ("rgb", C.c_int), ("dtype", C.c_int),
+                ("scale", C.c_float * 4), ("bias", C.c_float * 4)]
+
+
 def _renditions(fn, h, bufs, opts, out_cap):
     """lp_xbatch_transform_renditions / lp_multi_transform_renditions: every file through every ImageOptions of
     `opts`.  Returns (outs, status), both indexed [item][rendition]."""
@@ -505,6 +515,9 @@ class XBatch:
         l.lp_xbatch_transform_renditions.restype = C.c_int
         l.lp_xbatch_transform_renditions.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.POINTER(_ImageOptions),
                                                      C.c_int, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p]
+        l.lp_xbatch_decode_frames.restype = C.c_int
+        l.lp_xbatch_decode_frames.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.POINTER(_ImageOptions),
+                                              C.POINTER(_FrameTensor), C.c_void_p, C.c_void_p, C.c_void_p]
         cfg = _XBatchConfig(device, arena_bytes, host_threads, max_size)
         self.h = l.lp_xbatch_create(C.byref(cfg))
         if not self.h:
@@ -536,6 +549,24 @@ class XBatch:
         """Every file through every ImageOptions of `opts` in one call (each file decoded once): (outs, status)
         indexed [item][rendition], each pair equal to lp_transform(bufs[i], opts[r])."""
         return _renditions(self.lib.l.lp_xbatch_transform_renditions, self.h, bufs, opts, out_cap)
+
+    def decode_frames(self, bufs, opt: ImageOptions, data_ptr: int, bytes: int, height: int, width: int,
+                      channels: int = 3, nchw: bool = False, rgb: bool = True, dtype: str = "u8", scale=None, bias=None):
+        """lp_xbatch_decode_frames: the frame lp_transform(bufs[i], opt with ".png") would encode, written into slice i of
+        the device tensor at data_ptr (`bytes` long, on this context's device; N x H x W x C, or N x C x H x W when nchw).
+        Float dtypes store sample * scale[c] + bias[c] per output channel.  Returns (width, height, status) lists."""
+        n = len(bufs)
+        ptrs, lens, keep = Batch._ptr_arrays(bufs)
+        t = _FrameTensor(data_ptr, bytes, height, width, channels, int(bool(nchw)), int(bool(rgb)),
+                         FRAME_DTYPES.get(dtype, -1) if isinstance(dtype, str) else int(dtype),
+                         (C.c_float * 4)(*(list(scale) if scale is not None else [1.0] * 4)),
+                         (C.c_float * 4)(*(list(bias) if bias is not None else [0.0] * 4)))
+        w, h, status = (C.c_int * max(n, 1))(), (C.c_int * max(n, 1))(), (C.c_int * max(n, 1))()
+        copt = opt._c()
+        rc = self.lib.l.lp_xbatch_decode_frames(self.h, ptrs, lens, n, C.byref(copt), C.byref(t), w, h, status)
+        if rc:
+            raise LilliputError(rc)
+        return list(w[:n]), list(h[:n]), list(status[:n])
 
     def stats(self) -> dict:
         s = _XBatchStats()

@@ -386,4 +386,25 @@ int seg_copy_launch(const SegCopy* d_segs, int n, uint8_t* base, cudaStream_t st
 int blend_region_launch(const uint8_t* src, size_t src_step, int src_ch, uint8_t* dst,
                         size_t dst_step, int dst_ch, int w, int h, cudaStream_t st);
 
+// ---- frames_pack.cu ------------------------------------------------------------------------
+// One frame for lp_xbatch_decode_frames: w x h u8 pixels of `ch` bytes (1 gray, 3 BGR, 4 BGRA), rows `step` apart, and the
+// item whose slice of the tensor it fills.
+struct FramePackItem {
+    const uint8_t* src;
+    uint32_t step;
+    int32_t w, h, ch;
+    int64_t slice;
+};
+// The tensor of an lp_frame_tensor: every slice H x W x C elements of `dtype` (LP_DTYPE_*)
+struct FramePackLayout {
+    void* data;
+    int H, W, C, nchw, rgb, dtype;
+    float scale[4], bias[4];
+};
+// Bytes of one element of an LP_DTYPE_* (0: not a dtype)
+size_t frames_dtype_bytes(int dtype);
+// One launch over n items (d_items: a device table of n entries; or n == 1 and `one`, passed by value): each item's slice
+// written whole, its frame at the top-left in the tensor's layout and zero around it.  data must be aligned to the dtype.
+int frames_pack_launch(const FramePackItem* d_items, const FramePackItem* one, int n, const FramePackLayout& t, cudaStream_t st);
+
 }  // namespace lp

@@ -36,7 +36,8 @@
 //      batched VP8L encoder over every frame of a run, webp_encode.cu; a PNG's ICC profile carried the same way), GIF
 //      from GIF sources (palette mapping + LZW of every frame of the task, gif_decode.cu; the container assembled on the
 //      host), PNG from JPEG, PNG and WebP stills (filter, DEFLATE, checksums and container of every frame of a run in
-//      three launches, png_encode.cu).  Whatever the decoder kind, a task's decoded frames go through one run walk
+//      three launches, png_encode.cu), and pixels instead of files (lp_xbatch_decode_frames: each run's frames packed
+//      into the caller's device tensor in one launch, frames_pack.cu).  Whatever the decoder kind, a task's decoded frames go through one run walk
 //      (task_runs: adjacent items that take a rendition and share a geometry), one resize launch per run, and one sink
 //      entry (sink_encode) per run of resized frames;
 //   3. anything the grid path does not cover (gray or over-budget multi-scan JPEGs, gray PNGs, EXIF-rotated sources,
@@ -72,18 +73,19 @@ namespace lp {
 lp_batch* batch_create_in(const lp_batch_config* cfg, uint8_t* dev_arena, size_t dev_bytes, uint8_t* host_arena,
                           size_t host_bytes, bool progressive_jpeg, bool multiscan_sources, bool resize_only,
                           bool oriented_sources = false,  // (rotated and gray JPEGs are handed to lp_transform before
-                          bool gray_sources = false,      // grouping, so these contexts take neither)
+                          bool gray_sources = false,      // grouping, except by lp_xbatch_decode_frames)
                           const BatchGeom* geoms = nullptr, int n_geoms = 0);
 int batch_resized_status(lp_batch* b, int* status);
 const uint8_t* batch_resized_geom(const lp_batch* b, int g, size_t* image_stride);
 size_t batch_multiscan_pool_bytes(size_t n);
 void batch_arena_used(const lp_batch* b, size_t* dev_bytes, size_t* host_bytes);
+int mat_device_view(void* mat, int* cols, int* rows, int* type, const uint8_t** dev, size_t* step);
 }  // namespace lp
 
 namespace {
 
 enum Kind { K_FALLBACK = 0, K_JPEG = 1, K_PNG = 2, K_WEBP = 3, K_GIF = 4 };
-enum Sink { S_NONE = 0, S_JPEG = 1, S_WEBP = 2, S_GIF = 3, S_PNG = 4 };
+enum Sink { S_NONE = 0, S_JPEG = 1, S_WEBP = 2, S_GIF = 3, S_PNG = 4, S_FRAMES = 5 };  // S_FRAMES: lp_xbatch_decode_frames
 constexpr int kMaxRenditions = LP_XBATCH_MAX_RENDITIONS;  // (a rendition mask is one 32-bit word)
 
 // One output the call asks of every item: its options and what the sink takes from them
@@ -171,6 +173,9 @@ struct lp_xbatch {
     size_t out_cap = 0;
     size_t* out_len = nullptr;
     int* status = nullptr;  // (out, out_len and status: one entry per pair, item-major)
+    lp_frame_tensor frames;  // lp_xbatch_decode_frames: the caller's tensor, and each item's frame size
+    int* frame_w = nullptr;
+    int* frame_h = nullptr;
     int k = 1;              // renditions
     std::vector<Rendition> rend;
     std::vector<XItem> items;   // pairs: item i, rendition r at i * k + r
@@ -231,6 +236,29 @@ static void keep_icc(XItem* it, const uint8_t* icc, long n) {
     if (n > 0 && lilliput::iccHeaderIsSane(icc, (size_t)n)) it->icc.assign(icc, icc + n);
 }
 
+// A multi-scan JPEG the serial decoder takes: its scans parse and stay within the work budget (otherwise per image)
+static bool multiscan_in_budget(const uint8_t* d, size_t n, const JpegHeader& h) {
+    std::vector<JpegScanDesc> scans(kMultiscanMaxScans);
+    int nscans = 0, nsets = 0;
+    return jpeg_parse_scans(d, n, h, scans.data(), (int)scans.size(), &nscans, (JpegHeader*)nullptr, kMultiscanMaxSets, &nsets) ==
+               LP_OK &&
+           jpeg_multiscan_visits(h, scans.data(), nscans) <= kMultiscanMaxVisits;
+}
+
+// A PNG the grid decodes: a colour (RGB / RGBA) frame of at most max_side, without an eXIf turn (Transform turns the frame
+// before the resize, which the grid does not), its IDAT payloads one forward run of the file (they are in every valid PNG)
+static std::shared_ptr<const PngHeader> png_grid_header(const uint8_t* d, size_t n, int max_side) {
+    std::shared_ptr<PngHeader> h(new PngHeader);
+    if (png_parse(d, n, h.get()) != LP_OK) return nullptr;
+    if (h->orientation != 1 || h->idat.empty() || h->idat_total < 2) return nullptr;
+    if (h->width > max_side || h->height > max_side) return nullptr;
+    for (size_t q = 1; q < h->idat.size(); q++)
+        if (h->idat[q].offset < h->idat[q - 1].offset + h->idat[q - 1].length) return nullptr;
+    if (h->idat.back().offset + h->idat.back().length > n) return nullptr;
+    if (h->out_channels != 3 && h->out_channels != 4) return nullptr;  // gray PNGs: per image
+    return h;
+}
+
 // An item's container and header parse, shared by its renditions: each runs at most once per item, and a refusal is
 // remembered as well (-1: not parsed yet, 0: refused, 1: usable)
 struct ItemHeaders {
@@ -247,6 +275,89 @@ struct ItemHeaders {
     std::shared_ptr<GifAnimPlan> gp[2];
 };
 
+// The gates of an item of lp_xbatch_decode_frames: the frame Transform hands its still ".png" encoder, which answers at
+// once (no deadline, frame limit or flush follows it), so only MaxEncodeDuration -- held against a frame's duration
+// before the encode -- and NoResize send an item per image, besides what each decoder's gate refuses.  JPEG: rotated and
+// gray files too (the group's resize-only lp_batch context orients and decodes both; an item whose orientation swaps the
+// axes gets the turned frame's output size).  PNG: RGB / RGBA of 8 or 16 bits, HDR tone-mapped; an SDR cICP changes no
+// pixel and is written nowhere.  WebP: stills, and animations cut to frame 0.  GIF: the first-frame plan.
+static void parse_frames_pair(XItem& it, const lp_image_options& opt, const uint8_t* d, size_t n, int max_side) {
+    if (opt.max_encode_duration_ns != 0) return;
+    static const uint8_t png_sig[8] = {0x89, 0x50, 0x4E, 0x47, 0x0D, 0x0A, 0x1A, 0x0A};
+    if (d[0] == 0xFF && d[1] == 0xD8) {
+        JpegHeader h;
+        if (jpeg_parse_header(d, n, &h) != LP_OK || (!h.supported && !h.multiscan)) return;
+        if ((h.ncomp != 3 && h.ncomp != 1) || h.width > max_side || h.height > max_side) return;
+        if (!h.supported && !multiscan_in_budget(d, n, h)) return;
+        it.jpeg_multiscan = !h.supported;
+        it.w = h.width;
+        it.h = h.height;
+        it.ch = h.ncomp;
+        it.jpeg_sampling = 0;
+        for (int q = 0; q < h.ncomp; q++) it.jpeg_sampling = (it.jpeg_sampling << 8) | (h.comp[q].h << 4) | h.comp[q].v;
+        if (!plan_geometry(opt, &it)) return;
+        // orientations 5..8: the requested size is the header's turned only under NormalizeOrientation, and Fit works on
+        // the turned frame (ops.go:449-470, as lp_batch sizes its class 2)
+        if (h.orientation >= 5 && h.orientation <= 8 && opt.resize_method == LP_OPS_FIT) {
+            const bool turn = opt.normalize_orientation != 0;
+            lilliput::calculateExpectedSize(turn ? h.height : h.width, turn ? h.width : h.height, opt.width, opt.height, &it.ow, &it.oh);
+        }
+        it.kind = K_JPEG;
+        return;
+    }
+    if (!memcmp(d, png_sig, 8)) {
+        std::shared_ptr<const PngHeader> ph = png_grid_header(d, n, max_side);
+        if (!ph) return;
+        uint8_t cicp[4];
+        if (png_extract_cicp(d, n, cicp)) {
+            it.hdr = cicp[1] == 16 || cicp[1] == 18;
+            it.transfer = cicp[1];
+            it.primaries = cicp[0];
+        }
+        it.w = ph->width;
+        it.h = ph->height;
+        it.ch = ph->out_channels;
+        if (!plan_geometry(opt, &it)) return;
+        it.png = std::move(ph);
+        it.kind = K_PNG;
+        return;
+    }
+    if (!memcmp(d, "RIFF", 4) && !memcmp(d + 8, "WEBP", 4)) {
+        std::unique_ptr<WebpPlan> p(new WebpPlan);
+        if (!webp_plan_parse(d, n, p.get()) || p->width > max_side || p->height > max_side) return;
+        WebpFramePlan& f0 = p->frames[0];
+        it.webp_animation = p->frames.size() > 1;
+        if (!it.webp_animation) {  // Transform does not composite a still: it resizes the decoded frame, which must be the canvas
+            if (f0.x || f0.y || f0.width != p->width || f0.height != p->height) return;
+            f0.blend = 1;
+            f0.dispose = 0;
+        } else {
+            it.span = webp_plan_first_frame(p.get());
+        }
+        it.w = p->width;
+        it.h = p->height;
+        it.ch = p->channels;
+        if (!plan_geometry(opt, &it)) return;
+        it.webp = std::move(p);
+        it.kind = K_WEBP;
+        return;
+    }
+    if (!memcmp(d, "GIF8", 4)) {
+        std::shared_ptr<GifAnimPlan> p(gif_plan_parse(d, n, 4096, true), gif_plan_free);
+        if (!p) return;
+        int w = 0, h = 0, nf = 0;
+        gif_plan_info(p.get(), &w, &h, &nf, nullptr, nullptr);
+        it.w = w;
+        it.h = h;
+        it.ch = 4;
+        it.span = gif_plan_file_bytes(p.get());
+        if (w > max_side || h > max_side || !plan_geometry(opt, &it)) return;
+        it.gif = std::move(p);
+        it.gif_frames = nf;
+        it.kind = K_GIF;
+    }
+}
+
 // the gates of pair (i, r): it takes the grid when they pass; anything else goes to lp_transform(in[i], opts[r])
 static void parse_pair(lp_xbatch* X, int i, int r, ItemHeaders* c) {
     XItem& it = X->items[(size_t)i * X->k + r];
@@ -258,11 +369,15 @@ static void parse_pair(lp_xbatch* X, int i, int r, ItemHeaders* c) {
     it.icc.clear();
     it.span = n;
     if (!d || n < 16 || R.sink == S_NONE) return;
+    const int max_side = X->cfg.max_size > 0 ? X->cfg.max_size : 8192;
+    if (R.sink == S_FRAMES) {
+        parse_frames_pair(it, opt, d, n, max_side);
+        return;
+    }
     // To PNG every still is one frame in, the file out of the first Encode call: MaxEncodeFrames, DisableAnimatedOutput
     // and the deadline are never consulted.  A negative MaxEncodeDuration is exceeded before the frame is encoded, and
     // Transform then asks the decoder to skip to the end, which no still decoder can (ErrSkipNotSupported): per image.
     if (R.sink == S_PNG && opt.max_encode_duration_ns < 0) return;
-    const int max_side = X->cfg.max_size > 0 ? X->cfg.max_size : 8192;
     static const uint8_t png_sig[8] = {0x89, 0x50, 0x4E, 0x47, 0x0D, 0x0A, 0x1A, 0x0A};
     thread_local std::vector<uint8_t> icc_buf(32768);
     if (d[0] == 0xFF && d[1] == 0xD8) {
@@ -281,12 +396,7 @@ static void parse_pair(lp_xbatch* X, int i, int r, ItemHeaders* c) {
             if (h.orientation >= 2 && h.orientation <= 8) return;
             if (h.width > max_side || h.height > max_side) return;
             if (!h.supported) {  // multi-scan: damaged scans and files over the serial decoder's budget go per image
-                std::vector<JpegScanDesc> scans(kMultiscanMaxScans);
-                int nscans = 0, nsets = 0;
-                if (jpeg_parse_scans(d, n, h, scans.data(), (int)scans.size(), &nscans, (JpegHeader*)nullptr, kMultiscanMaxSets,
-                                     &nsets) != LP_OK ||
-                    jpeg_multiscan_visits(h, scans.data(), nscans) > kMultiscanMaxVisits)
-                    return;
+                if (!multiscan_in_budget(d, n, h)) return;
                 c->jpeg_multiscan = true;
             }
             c->jpeg = 1;
@@ -308,20 +418,9 @@ static void parse_pair(lp_xbatch* X, int i, int r, ItemHeaders* c) {
     if (!memcmp(d, png_sig, 8)) {
         if (R.sink == S_GIF) return;  // GIF output needs a GIF source: per image (ErrGifEncoderNeedsDecoder)
         if (c->png < 0) {
-            c->png = 0;
-            std::shared_ptr<PngHeader> h(new PngHeader);
-            if (png_parse(d, n, h.get()) != LP_OK) return;
-            // an eXIf orientation other than 1: Transform turns the frame before the resize, which the grid does not: per image
-            if (h->orientation != 1 || h->idat.empty() || h->idat_total < 2) return;
-            if (h->width > max_side || h->height > max_side) return;
-            // the IDAT payloads must form one forward run of the file (they do in every valid PNG)
-            for (size_t q = 1; q < h->idat.size(); q++)
-                if (h->idat[q].offset < h->idat[q - 1].offset + h->idat[q - 1].length) return;
-            if (h->idat.back().offset + h->idat.back().length > n) return;
-            if (h->out_channels != 3 && h->out_channels != 4) return;  // gray PNGs: per image
-            c->png_cicp = png_extract_cicp(d, n, c->cicp);
-            c->ph = std::move(h);
-            c->png = 1;
+            c->ph = png_grid_header(d, n, max_side);
+            c->png = c->ph != nullptr;
+            if (c->png) c->png_cicp = png_extract_cicp(d, n, c->cicp);
         }
         if (!c->png) return;
         if (c->png_cicp) {
@@ -708,6 +807,65 @@ static void gif_sink(lp_xbatch* X, Lane& L, Bump& bump, const std::vector<int>& 
     }
 }
 
+static FramePackLayout frames_layout(const lp_frame_tensor& t) {
+    FramePackLayout o;
+    o.data = t.data;
+    o.H = t.height;
+    o.W = t.width;
+    o.C = t.channels;
+    o.nchw = t.nchw != 0;
+    o.rgb = t.rgb != 0;
+    o.dtype = t.dtype;
+    for (int c = 0; c < 4; c++) {
+        o.scale[c] = t.scale[c];
+        o.bias[c] = t.bias[c];
+    }
+    return o;
+}
+
+// lp_xbatch_decode_frames: every frame of the run into its item's slice of the caller's tensor in one launch.  The run's
+// items travel in a small device table, so items that are not neighbours in the batch land in their own slices, each
+// with its own frame size (a JPEG group's turned or gray items).  A frame larger than the box is refused; one whose
+// decode failed goes to the per-image path.  Nothing comes back to the host.
+static void frames_sink(lp_xbatch* X, Lane& L, Bump& bump, const std::vector<int>& pairs, const std::vector<int>& st,
+                        const uint8_t* d_frames, size_t stride, std::vector<int>* failed) {
+    const lp_frame_tensor& T = X->frames;
+    std::vector<FramePackItem> tab;
+    std::vector<int> packed;
+    for (size_t q = 0; q < pairs.size(); q++) {
+        const int i = pairs[q];  // (one rendition: the pair is the item)
+        const XItem& it = X->items[i];
+        if (st[q] != LP_OK) {
+            failed->push_back(i);
+        } else if (it.ow > T.width || it.oh > T.height) {
+            X->status[i] = LP_ERR_BUF_TOO_SMALL;
+        } else {
+            tab.push_back(FramePackItem{d_frames + q * stride, (uint32_t)(it.ow * it.ch), it.ow, it.oh, it.ch, i});
+            packed.push_back(i);
+        }
+    }
+    if (tab.empty()) return;
+    const size_t mark = bump.used;
+    FramePackItem* d_tab = bump.take<FramePackItem>(tab.size() * sizeof(FramePackItem));
+    int rc = d_tab ? LP_OK : LP_ERR_BUF_TOO_SMALL;
+    if (!rc && cudaMemcpyAsync(d_tab, tab.data(), tab.size() * sizeof(FramePackItem), cudaMemcpyHostToDevice, L.st) != cudaSuccess)
+        rc = LP_ERR_CUDA;
+    if (!rc) rc = frames_pack_launch(d_tab, nullptr, (int)tab.size(), frames_layout(T), L.st);
+    if (!rc && cudaStreamSynchronize(L.st) != cudaSuccess) rc = LP_ERR_CUDA;
+    bump.used = mark;
+    if (rc) {
+        cudaGetLastError();
+        failed->insert(failed->end(), packed.begin(), packed.end());
+        return;
+    }
+    L.h2d += tab.size() * sizeof(FramePackItem);
+    for (const FramePackItem& f : tab) {
+        X->status[f.slice] = LP_OK;
+        X->frame_w[f.slice] = f.w;
+        X->frame_h[f.slice] = f.h;
+    }
+}
+
 static void lane_time(Lane& L, int from, int to, double* acc) {
     float ms = 0;
     if (cudaEventElapsedTime(&ms, L.ev[from], L.ev[to]) == cudaSuccess) *acc += ms;
@@ -730,6 +888,7 @@ static void sink_encode(lp_xbatch* X, Lane& L, Bump& bump, uint8_t* h_stage, siz
     cudaEventRecord(L.ev[2], L.st);
     if (R.sink == S_WEBP) webp_sink(X, R, L, pairs, pst, d_frames, stride, failed);
     else if (R.sink == S_GIF) gif_sink(X, L, bump, pairs, pst, d_frames, stride, failed);
+    else if (R.sink == S_FRAMES) frames_sink(X, L, bump, pairs, pst, d_frames, stride, failed);
     else slot_sink(X, R, L, bump, h_stage, h_stage_bytes, pairs, pst, d_frames, stride, jpeg_cap, failed);
     cudaEventRecord(L.ev[3], L.st);
     cudaEventSynchronize(L.ev[3]);
@@ -1098,6 +1257,7 @@ static void run_jpeg(lp_xbatch* X, Lane& L, const Task& t) {
     c.dst_width = R.opt.width;
     c.dst_height = R.opt.height;
     c.resize_method = R.opt.resize_method;
+    c.normalize_orientation = R.opt.normalize_orientation;  // (sizes only the turned items lp_xbatch_decode_frames hands it)
     c.jpeg_quality = R.quality;
     c.max_in_bytes = in_bytes + (1 << 20);
     // slot per output: never larger than the callers' buffers (lp_batch copies a whole result into out[i])
@@ -1105,7 +1265,8 @@ static void run_jpeg(lp_xbatch* X, Lane& L, const Task& t) {
     // images per chunk: whole Huffman waves while the per-chunk scratch fits the lane's arena
     const size_t mcus = (size_t)ceil_div(g.w, 8) * ceil_div(g.h, 8);
     // multi-scan groups: + the nonzero masks per block, + the scan and table-set pools (batch.cu)
-    const size_t per_img = (mcus * 3 + 64) * (128 + 64 + 2 + (g.jpeg_multiscan ? 8 : 0)) + (size_t)g.w * g.h * 3 + 65536;
+    // (a context that takes rotated files: + each chunk slot's oriented crop, at most the frame)
+    const size_t per_img = (mcus * 3 + 64) * (128 + 64 + 2 + (g.jpeg_multiscan ? 8 : 0)) + (size_t)g.w * g.h * 3 * (R.sink == S_FRAMES ? 2 : 1) + 65536;
     const size_t pools = g.jpeg_multiscan ? batch_multiscan_pool_bytes((size_t)n) : 0;
     // every rendition's resized frames stay resident for the group; the sinks run one after another, so the largest
     // sink's room is kept
@@ -1129,8 +1290,9 @@ static void run_jpeg(lp_xbatch* X, Lane& L, const Task& t) {
     int chunk = (int)std::min<long>(fit, 3L * std::max(slots, 1));
     if (slots > 0 && chunk > slots) chunk = chunk / slots * slots;
     c.chunk = std::max(1, std::min(chunk, n));
+    const bool frames = R.sink == S_FRAMES;  // (a call with one rendition: the context may take rotated and gray files)
     lp_batch* b = batch_create_in(&c, L.dev, L.dev_bytes, L.host, L.host_bytes, R.progressive, g.jpeg_multiscan, resize_only,
-                                  false, false, several ? geoms.data() : nullptr, several ? (int)geoms.size() : 0);
+                                  frames, frames, several ? geoms.data() : nullptr, several ? (int)geoms.size() : 0);
     if (!b) {
         push_task_fallback(X, t);
         return;
@@ -1304,11 +1466,33 @@ static Rendition make_rendition(const lp_image_options& opt) {
     return R;
 }
 
-extern "C" int lp_xbatch_transform_renditions(lp_xbatch* X, const uint8_t* const* in, const size_t* in_len, int n,
-                                              const lp_image_options* opts, int k, uint8_t* const* out, size_t out_cap,
-                                              size_t* out_len, int* status) {
-    if (!X || n < 0 || !opts || k < 1 || k > kMaxRenditions || (n > 0 && (!in || !in_len || !out || !out_len || !status)))
-        return LP_ERR_BAD_ARGUMENT;
+// lp_xbatch_decode_frames' per-image route: Transform up to its encoder, whose frame (on the device already, or uploaded
+// by mat_device_view) is packed into slice i on this worker's stream by the grid path's kernel
+static int frames_transform(lp_xbatch* X, int i, const lp_image_options* opt, int max_size) {
+    const lp_frame_tensor& T = X->frames;
+    return lilliput::TransformToFrame(X->in[i], X->in_len[i], opt, max_size, [&](lilliput::Framebuffer* f) -> int {
+        int cols = 0, rows = 0, type = 0;
+        const uint8_t* dev = nullptr;
+        size_t step = 0;
+        int rc = mat_device_view(f->mat, &cols, &rows, &type, &dev, &step);
+        if (rc) return rc;
+        const int ch = opencv_type_channels(type);
+        if (opencv_type_depth(type) != 8 || (ch != 1 && ch != 3 && ch != 4)) return LP_ERR_UNSUPPORTED;  // (framebuffers are 8-bit)
+        if (cols > T.width || rows > T.height) return LP_ERR_BUF_TOO_SMALL;
+        const FramePackItem one{dev, (uint32_t)step, cols, rows, ch, i};
+        cudaStream_t st = thread_stream();
+        rc = frames_pack_launch(nullptr, &one, 1, frames_layout(T), st);
+        if (!rc && cudaStreamSynchronize(st) != cudaSuccess) rc = LP_ERR_CUDA;
+        if (rc) return rc;
+        X->frame_w[i] = cols;
+        X->frame_h[i] = rows;
+        return LP_OK;
+    });
+}
+
+// One call over n items and k renditions (rends: each one's sink, made from opts[r]); the arguments are checked
+static int xbatch_call(lp_xbatch* X, const uint8_t* const* in, const size_t* in_len, int n, const lp_image_options* opts,
+                       const Rendition* rends, int k, uint8_t* const* out, size_t out_cap, size_t* out_len, int* status) {
     int prev = 0;
     cudaGetDevice(&prev);
     LP_CUDA_OK(cudaSetDevice(X->device));
@@ -1322,7 +1506,7 @@ extern "C" int lp_xbatch_transform_renditions(lp_xbatch* X, const uint8_t* const
     X->status = status;
     X->k = k;
     X->rend.clear();
-    for (int r = 0; r < k; r++) X->rend.push_back(make_rendition(opts[r]));
+    X->rend.assign(rends, rends + k);
     X->items.clear();
     X->items.resize(np);
     X->mask.assign((size_t)n, 0);
@@ -1497,8 +1681,12 @@ extern "C" int lp_xbatch_transform_renditions(lp_xbatch* X, const uint8_t* const
             const long l0 = g_launches;
             const int p = fb[q], i = p / k;
             size_t len = 0;
-            status[p] = lp_transform(in[i], in_len[i], &opts[p % k], out[p], out_cap, &len, max_size);
-            out_len[p] = status[p] == LP_OK ? len : 0;
+            if (X->rend[p % k].sink == S_FRAMES) {
+                status[p] = frames_transform(X, i, &opts[p % k], max_size);
+            } else {
+                status[p] = lp_transform(in[i], in_len[i], &opts[p % k], out[p], out_cap, &len, max_size);
+                out_len[p] = status[p] == LP_OK ? len : 0;
+            }
             fb_launches += g_launches - l0;
         });
         X->stats.fallback_items = (int)fb.size();
@@ -1527,10 +1715,81 @@ extern "C" int lp_xbatch_transform_renditions(lp_xbatch* X, const uint8_t* const
     return LP_OK;
 }
 
+extern "C" int lp_xbatch_transform_renditions(lp_xbatch* X, const uint8_t* const* in, const size_t* in_len, int n,
+                                              const lp_image_options* opts, int k, uint8_t* const* out, size_t out_cap,
+                                              size_t* out_len, int* status) {
+    if (!X || n < 0 || !opts || k < 1 || k > kMaxRenditions || (n > 0 && (!in || !in_len || !out || !out_len || !status)))
+        return LP_ERR_BAD_ARGUMENT;
+    std::vector<Rendition> rends;
+    for (int r = 0; r < k; r++) rends.push_back(make_rendition(opts[r]));
+    return xbatch_call(X, in, in_len, n, opts, rends.data(), k, out, out_cap, out_len, status);
+}
+
 extern "C" int lp_xbatch_transform(lp_xbatch* X, const uint8_t* const* in, const size_t* in_len, int n,
                                    const lp_image_options* opt, uint8_t* const* out, size_t out_cap, size_t* out_len,
                                    int* status) {
     return lp_xbatch_transform_renditions(X, in, in_len, n, opt, 1, out, out_cap, out_len, status);
+}
+
+// Weak: the host-side tests link these objects against a stand-in runtime without pointer queries (there the call's
+// tensor is never on the device); the library's static runtime defines it
+#pragma weak cudaPointerGetAttributes
+
+// Whether [p, p + bytes) lies in device memory of `device` (both of its ends)
+static bool on_device(const void* p, size_t bytes, int device) {
+    if (!&cudaPointerGetAttributes) return false;
+    for (const void* q : {p, (const void*)((const uint8_t*)p + bytes - 1)}) {
+        cudaPointerAttributes a;
+        if (cudaPointerGetAttributes(&a, q) != cudaSuccess) {
+            cudaGetLastError();
+            return false;
+        }
+        if (a.type != cudaMemoryTypeDevice || a.device != device) return false;
+    }
+    return true;
+}
+
+extern "C" int lp_xbatch_decode_frames(lp_xbatch* X, const uint8_t* const* in, const size_t* in_len, int n,
+                                       const lp_image_options* opt, const lp_frame_tensor* dst, int* width, int* height,
+                                       int* status) {
+    if (!X || n < 0 || !opt || !dst || (n > 0 && (!in || !in_len || !width || !height || !status))) return LP_ERR_BAD_ARGUMENT;
+    const lp_frame_tensor T = *dst;
+    const size_t es = frames_dtype_bytes(T.dtype);
+    if (!es || !T.data || (uintptr_t)T.data % es || (T.channels != 3 && T.channels != 4) || T.height < 1 || T.width < 1)
+        return LP_ERR_BAD_ARGUMENT;
+    size_t slice = 0;
+    if (__builtin_mul_overflow((size_t)T.height * (size_t)T.width, (size_t)T.channels * es, &slice) ||
+        (n > 0 && slice > T.bytes / (size_t)n))
+        return LP_ERR_BAD_ARGUMENT;
+    {
+        DeviceGuard g(X->device);
+        if (!g.ok || !on_device(T.data, std::max<size_t>(1, slice * (size_t)n), X->device)) return LP_ERR_BAD_ARGUMENT;
+    }
+    X->frames = T;
+    X->frame_w = width;
+    X->frame_h = height;
+    for (int i = 0; i < n; i++) width[i] = height[i] = 0;
+    Rendition R = make_rendition(*opt);
+    R.sink = S_FRAMES;
+    std::vector<uint8_t*> out((size_t)n, nullptr);  // (no files: every output of the call is in the tensor)
+    std::vector<size_t> out_len((size_t)n, 0);
+    int rc = xbatch_call(X, in, in_len, n, opt, &R, 1, out.data(), 0, out_len.data(), status);
+    // the slices of the items that failed: zero, as is their size
+    DeviceGuard g(X->device);
+    cudaStream_t st = X->lanes[0].st;
+    for (int i = 0; i < n && !rc;) {
+        if (status[i] == LP_OK) {
+            i++;
+            continue;
+        }
+        int e = i;
+        for (; e < n && status[e] != LP_OK; e++) width[e] = height[e] = 0;
+        if (cudaMemsetAsync((uint8_t*)T.data + (size_t)i * slice, 0, (size_t)(e - i) * slice, st) != cudaSuccess) rc = LP_ERR_CUDA;
+        i = e;
+    }
+    if (!rc && cudaStreamSynchronize(st) != cudaSuccess) rc = LP_ERR_CUDA;
+    X->frame_w = X->frame_h = nullptr;
+    return rc;
 }
 
 // ------------------------------------------------------------------ library-level multi-GPU dispatch

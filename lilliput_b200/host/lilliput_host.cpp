@@ -797,7 +797,7 @@ Error ImageOps::skipToEnd(Decoder* d) {  // ref ops.go:336-344
 // stay the reference's).  HDR (PQ / HLG) sources ARE tone-mapped after every decode, as ops.go:154-165 does.  What IS mirrored of the cICP policy: an SDR cICP chunk of a PNG source
 // is re-attached to a PNG output (ops.go:306-332); an HDR (PQ / HLG) tag is never re-emitted (ops.go:513-517).
 Error ImageOps::Transform(Decoder* d, const ImageOptions& opt, uint8_t* dst, size_t dst_cap,
-                          size_t* out_len) {
+                          size_t* out_len, Encoder* encoder) {
     struct CompositeGuard {  // the deferred close at ops.go:353-358
         std::unique_ptr<Framebuffer>& p;
         ~CompositeGuard() { p.reset(); }
@@ -820,8 +820,9 @@ Error ImageOps::Transform(Decoder* d, const ImageOptions& opt, uint8_t* dst, siz
         return opencv_png_insert_cicp(dst, n, dst_cap, outputCICP->Primaries, outputCICP->Transfer,
                                       outputCICP->Matrix, outputCICP->FullRange ? 1 : 0);
     };
-    std::unique_ptr<Encoder> enc;
-    if ((e = NewEncoder(opt.FileType, d, dst, dst_cap, &enc))) return e;
+    std::unique_ptr<Encoder> own;
+    if (!encoder && (e = NewEncoder(opt.FileType, d, dst, dst_cap, &own))) return e;
+    Encoder* enc = encoder ? encoder : own.get();
 
     int frameCount = 0;
     int64_t duration = 0;
@@ -907,22 +908,68 @@ static ImageOptions fromC(const lp_image_options* o) {
 // hostile header cannot make a helper allocate gigabytes.
 static const int kHelperMaxSide = 8192;
 
-static int lp_transform_impl(const uint8_t* in, size_t in_len, const lp_image_options* opt,
-                            uint8_t* dst, size_t dst_cap, size_t* out_len, int max_size) {
-    if (!in || !opt || !dst || !out_len) return LP_ERR_BAD_ARGUMENT;
-    std::unique_ptr<Decoder> d;
-    Error e = NewDecoder(in, in_len, &d);
-    if (e) return e;
-    // One ImageOps per calling thread, reused across calls like a long-lived
-    // Go ImageOps (ref ops.go:83-91); re-created if max_size changes.
+// One ImageOps per calling thread, reused across calls like a long-lived
+// Go ImageOps (ref ops.go:83-91); re-created if max_size changes.
+static ImageOps* thread_ops(int max_size) {
     thread_local std::unique_ptr<ImageOps> ops;
     thread_local int ops_size = 0;
     if (!ops || ops_size != max_size) {
         ops.reset(new ImageOps(max_size));
         ops_size = max_size;
     }
-    return ops->Transform(d.get(), fromC(opt), dst, dst_cap, out_len);
+    return ops.get();
 }
+
+static int lp_transform_impl(const uint8_t* in, size_t in_len, const lp_image_options* opt,
+                            uint8_t* dst, size_t dst_cap, size_t* out_len, int max_size) {
+    if (!in || !opt || !dst || !out_len) return LP_ERR_BAD_ARGUMENT;
+    std::unique_ptr<Decoder> d;
+    Error e = NewDecoder(in, in_len, &d);
+    if (e) return e;
+    return thread_ops(max_size)->Transform(d.get(), fromC(opt), dst, dst_cap, out_len);
+}
+
+namespace lilliput {
+
+// Stands where the still ".png" encoder (OpenCVEncoder) stands in Transform, and answers as it does: the first frame
+// completes the output, an end of stream before any frame is LP_ERR_EOF
+class FrameEncoder : public Encoder {
+  public:
+    explicit FrameEncoder(const FrameSink& s) : sink(s) {}
+    Error Encode(Framebuffer* f, const std::map<int, int>&, bool* content, size_t* out_len) override {
+        *content = false;
+        if (!f) return LP_ERR_EOF;
+        Error e = sink(f);
+        if (e) return e;
+        *out_len = 0;
+        *content = true;
+        return LP_OK;
+    }
+
+  private:
+    const FrameSink& sink;
+};
+
+Error TransformToFrame(const uint8_t* in, size_t in_len, const lp_image_options* c_opt, int max_size, const FrameSink& sink) {
+    try {
+        if (!in || !c_opt) return LP_ERR_BAD_ARGUMENT;
+        std::unique_ptr<Decoder> d;
+        Error e = NewDecoder(in, in_len, &d);
+        if (e) return e;
+        ImageOptions opt = fromC(c_opt);
+        opt.FileType = ".png";
+        FrameEncoder enc(sink);
+        size_t n = 0;
+        uint8_t none = 0;
+        return thread_ops(max_size)->Transform(d.get(), opt, &none, 0, &n, &enc);
+    } catch (const std::bad_alloc&) {  // (as lp_transform reports an allocation the input makes impossible)
+        return LP_ERR_BUF_TOO_SMALL;
+    } catch (...) {
+        return LP_ERR_BAD_ARGUMENT;
+    }
+}
+
+}  // namespace lilliput
 
 static int lp_decode_host_impl(const uint8_t* in, size_t in_len, uint8_t* pixels,
                               size_t pixels_cap, int* width, int* height, int* type,

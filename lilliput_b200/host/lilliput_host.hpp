@@ -21,6 +21,7 @@
 #include <cstddef>
 #include <cstdint>
 #include <array>
+#include <functional>
 #include <map>
 #include <memory>
 #include <string>
@@ -161,8 +162,10 @@ bool pngChunkTypes(const uint8_t* img, size_t len, std::vector<std::array<uint8_
 class ImageOps {  // ref ops.go:67-150
   public:
     explicit ImageOps(int maxSize);  // NewImageOps, ref ops.go:83-91
+    // ref ops.go:352-444.  encoder: used in place of NewEncoder(opt.FileType, ...) when given (dst and dst_cap then
+    // only matter to what it writes)
     Error Transform(Decoder* d, const ImageOptions& opt, uint8_t* dst, size_t dst_cap,
-                    size_t* out_len);  // ref ops.go:352-444
+                    size_t* out_len, Encoder* encoder = nullptr);
     void Clear();
 
   private:
@@ -185,5 +188,11 @@ class ImageOps {  // ref ops.go:67-150
     std::unique_ptr<Framebuffer> animatedCompositeBuffer;
     int maxSize;
 };
+
+// The frame Transform would encode to PNG, handed to `sink` instead of an encoder: lp_transform(in, opt with FileType
+// ".png") up to its first Encode call, whose Framebuffer (8-bit gray, BGR or BGRA) goes to sink.  Returns Transform's
+// status, which is sink's when Transform gets that far.
+using FrameSink = std::function<Error(Framebuffer*)>;
+Error TransformToFrame(const uint8_t* in, size_t in_len, const lp_image_options* opt, int max_size, const FrameSink& sink);
 
 }  // namespace lilliput
