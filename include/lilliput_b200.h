@@ -289,6 +289,24 @@ int lp_xbatch_decode_frames(lp_xbatch* x, const uint8_t* const* in, const size_t
                             const lp_image_options* opt, const lp_frame_tensor* dst, int* width, int* height,
                             int* status);
 
+/* Files from pixels: slice i of the caller's device tensor src (the same lp_frame_tensor as lp_xbatch_decode_frames)
+ * holds item i's frame at its top-left, width[i] x height[i].  The frame is converted to 8-bit BGR (channels 3) or BGRA
+ * (channels 4) and goes through ImageOps.Transform with opt: status and bytes of item i are exactly those of
+ * lp_transform(P_i, opt, out[i], out_cap, ..., max_size), where P_i is an 8-bit PNG of that frame (colour type 2 or 6,
+ * no ancillary chunks).
+ *   - conversion per element of tensor channel c: U8 as is; F16 and BF16 widened to fp32 exactly, then as F32:
+ *     fmaf(x, scale[c], bias[c]) in fp32, rounded half to even, clamped to [0, 255]; NaN gives 0 (+inf 255, -inf 0).
+ *     rgb and nchw mean what they mean for lp_xbatch_decode_frames; channel 3, when present, is alpha.  A tensor
+ *     lp_xbatch_decode_frames wrote with scale 1/255 comes back with scale 255.
+ *   - width[i] or height[i] outside 1..box: that item gets LP_ERR_BAD_ARGUMENT and out_len 0; the others go on
+ * The tensor's contents must be complete before the call: the library's streams do not wait on the caller's.  The call
+ * only reads the tensor.  LP_ERR_BAD_ARGUMENT, with nothing written, for the tensor checks of lp_xbatch_decode_frames,
+ * n < 0, and a null opt / width / height / out / out_len / status with n > 0.
+ * Stats: ms_decode is the unpack; h2d_bytes carries no pixels (the item table only); d2h_bytes is the files. */
+int lp_xbatch_encode_frames(lp_xbatch* x, const lp_frame_tensor* src, int n, const int* width, const int* height,
+                            const lp_image_options* opt, uint8_t* const* out, size_t out_cap, size_t* out_len,
+                            int* status);
+
 /* ---- the same call over several GPUs of one node (SURVEY 8(e): shard by image index, no collective) ----
  * One lp_xbatch per device behind one call: the batch is cut into contiguous blocks balanced by compressed bytes,
  * every block runs on its own GPU from its own host thread, results land in the caller's arrays by index. */

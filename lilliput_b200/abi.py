@@ -518,6 +518,9 @@ class XBatch:
         l.lp_xbatch_decode_frames.restype = C.c_int
         l.lp_xbatch_decode_frames.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.POINTER(_ImageOptions),
                                               C.POINTER(_FrameTensor), C.c_void_p, C.c_void_p, C.c_void_p]
+        l.lp_xbatch_encode_frames.restype = C.c_int
+        l.lp_xbatch_encode_frames.argtypes = [C.c_void_p, C.POINTER(_FrameTensor), C.c_int, C.c_void_p, C.c_void_p,
+                                              C.POINTER(_ImageOptions), C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p]
         cfg = _XBatchConfig(device, arena_bytes, host_threads, max_size)
         self.h = l.lp_xbatch_create(C.byref(cfg))
         if not self.h:
@@ -567,6 +570,28 @@ class XBatch:
         if rc:
             raise LilliputError(rc)
         return list(w[:n]), list(h[:n]), list(status[:n])
+
+    def encode_frames(self, data_ptr: int, bytes: int, widths, heights, opt: ImageOptions, height: int, width: int,
+                      channels: int = 3, nchw: bool = False, rgb: bool = True, dtype: str = "u8", scale=None, bias=None,
+                      out_cap: int = 1 << 20):
+        """lp_xbatch_encode_frames: files from slices of the device tensor at data_ptr (laid out as for decode_frames),
+        item i the top-left widths[i] x heights[i] of slice i, each file equal to lp_transform of an 8-bit PNG of that
+        frame with opt.  Float dtypes read round(x * scale[c] + bias[c]) clamped to 0..255.  Returns (outs, status)."""
+        n = len(widths)
+        t = _FrameTensor(data_ptr, bytes, height, width, channels, int(bool(nchw)), int(bool(rgb)),
+                         FRAME_DTYPES.get(dtype, -1) if isinstance(dtype, str) else int(dtype),
+                         (C.c_float * 4)(*(list(scale) if scale is not None else [1.0] * 4)),
+                         (C.c_float * 4)(*(list(bias) if bias is not None else [0.0] * 4)))
+        ws, hs = (C.c_int * max(n, 1))(*widths), (C.c_int * max(n, 1))(*heights)
+        out = np.empty((max(n, 1), out_cap), dtype=np.uint8)
+        out_ptrs = (C.c_void_p * max(n, 1))(*[out[i].ctypes.data for i in range(n)])
+        out_lens = (C.c_size_t * max(n, 1))()
+        status = (C.c_int * max(n, 1))()
+        copt = opt._c()
+        rc = self.lib.l.lp_xbatch_encode_frames(self.h, C.byref(t), n, ws, hs, C.byref(copt), out_ptrs, out_cap, out_lens, status)
+        if rc:
+            raise LilliputError(rc)
+        return [out[i, : out_lens[i]].tobytes() for i in range(n)], list(status[:n])
 
     def stats(self) -> dict:
         s = _XBatchStats()

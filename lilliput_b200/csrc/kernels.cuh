@@ -406,5 +406,17 @@ size_t frames_dtype_bytes(int dtype);
 // One launch over n items (d_items: a device table of n entries; or n == 1 and `one`, passed by value): each item's slice
 // written whole, its frame at the top-left in the tensor's layout and zero around it.  data must be aligned to the dtype.
 int frames_pack_launch(const FramePackItem* d_items, const FramePackItem* one, int n, const FramePackLayout& t, cudaStream_t st);
+// One item of lp_xbatch_encode_frames: the top-left w x h of tensor slice `slice`, unpacked into a u8 BGR / BGRA frame
+// (the tensor's channel count) at dst, rows w * C bytes apart.  dst is 16-byte aligned.
+struct FrameUnpackItem {
+    uint8_t* dst;
+    int32_t w, h;
+    int64_t slice;
+};
+// One launch over n items (a device table, or n == 1 and `one` by value), the inverse of frames_pack_launch: per element
+// of tensor channel c, U8 as is; float dtypes fmaf(x, scale[c], bias[c]) in fp32, rounded half to even and clamped to
+// [0, 255], NaN as 0.  max_frame_bytes: the largest item's w * h * C.
+int frames_unpack_launch(const FrameUnpackItem* d_items, const FrameUnpackItem* one, int n, uint64_t max_frame_bytes,
+                         const FramePackLayout& t, cudaStream_t st);
 
 }  // namespace lp

@@ -27,6 +27,10 @@
 //                 a per-pixel compositor over every file's frame sequence (webp_decode.cu), resize of every canvas
 //        GIF   -> every frame of every animation: LZW (one warp per frame), per-pixel compositor over the
 //                 frame sequence (gif_decode.cu), resize of every composited canvas
+//        frames -> lp_xbatch_encode_frames: no file but slice i of a caller's device tensor, w[i] x h[i] at its top-left,
+//                 unpacked into u8 BGR / BGRA frames by one launch over the task (frames_pack.cu); the item passes the
+//                 gates of an 8-bit RGB / RGBA PNG (parse_frame_pair), and under NoResize its frame goes to the sink
+//                 unresized
 //        DisableAnimatedOutput (GIF and animated WebP to WebP, GIF to GIF): Transform stops after frame 0, so the plan
 //                 stops there too (gif_plan_parse's first-frame walk, webp_plan_first_frame); only the file up to the
 //                 end of frame 0's image data is uploaded, the same kernels run over one frame per file, and the sink
@@ -80,11 +84,12 @@ const uint8_t* batch_resized_geom(const lp_batch* b, int g, size_t* image_stride
 size_t batch_multiscan_pool_bytes(size_t n);
 void batch_arena_used(const lp_batch* b, size_t* dev_bytes, size_t* host_bytes);
 int mat_device_view(void* mat, int* cols, int* rows, int* type, const uint8_t** dev, size_t* step);
+int mat_bind_device_frame(void* mat, int cols, int rows, int type, uint8_t** dev, size_t* step);
 }  // namespace lp
 
 namespace {
 
-enum Kind { K_FALLBACK = 0, K_JPEG = 1, K_PNG = 2, K_WEBP = 3, K_GIF = 4 };
+enum Kind { K_FALLBACK = 0, K_JPEG = 1, K_PNG = 2, K_WEBP = 3, K_GIF = 4, K_FRAME = 5 };  // K_FRAME: lp_xbatch_encode_frames
 enum Sink { S_NONE = 0, S_JPEG = 1, S_WEBP = 2, S_GIF = 3, S_PNG = 4, S_FRAMES = 5 };  // S_FRAMES: lp_xbatch_decode_frames
 constexpr int kMaxRenditions = LP_XBATCH_MAX_RENDITIONS;  // (a rendition mask is one 32-bit word)
 
@@ -176,6 +181,8 @@ struct lp_xbatch {
     lp_frame_tensor frames;  // lp_xbatch_decode_frames: the caller's tensor, and each item's frame size
     int* frame_w = nullptr;
     int* frame_h = nullptr;
+    const int* src_w = nullptr;  // lp_xbatch_encode_frames: the items are slices of `frames`, of these sizes (no files)
+    const int* src_h = nullptr;
     int k = 1;              // renditions
     std::vector<Rendition> rend;
     std::vector<XItem> items;   // pairs: item i, rendition r at i * k + r
@@ -358,26 +365,71 @@ static void parse_frames_pair(XItem& it, const lp_image_options& opt, const uint
     }
 }
 
+// The option gates of a PNG still past its header gates (8-bit or 16-bit RGB / RGBA, no eXIf turn, no SDR cICP to PNG),
+// which a tensor item of lp_xbatch_encode_frames takes as a PNG with a profile.  GIF output needs a GIF source: per image
+// (ErrGifEncoderNeedsDecoder).  To WebP, PNGs with a profile stay per image, where they went before they could carry
+// it, under the options whose result the per-image path decides after the frame: a zero encode budget (the deadline
+// check, as for WebP stills), MaxEncodeFrames == 1 and a negative MaxEncodeDuration (the skip to the end a PNG decoder
+// refuses, as a JPEG's does).  To lossless output every PNG follows that rule.
+static bool png_option_gates(const Rendition& R, bool icc) {
+    const lp_image_options& opt = R.opt;
+    if (R.sink == S_GIF) return false;
+    return !(R.sink == S_WEBP && (icc || R.lossless) &&
+             (opt.encode_timeout_ns <= 0 || opt.max_encode_frames == 1 || opt.max_encode_duration_ns < 0));
+}
+
+// A tensor item of lp_xbatch_encode_frames: its "header" is w x h x C, with no container, so no ICC profile and no cICP,
+// and it takes the gates of an 8-bit RGB / RGBA PNG (png_grid_header's size limit, png_option_gates) with three
+// differences.  Two send items per image where lp_transform fails them and the PNG gates keep an ICC-less PNG on the
+// grid, as they always have:
+//   - the option gates are those of a PNG with a profile: Transform checks a still's deadline and MaxEncodeFrames after
+//     its frame goes to the .webp encoder (which waits for the end of the stream), and fails with ErrEncodeTimeout or
+//     ErrSkipNotSupported;
+//   - a negative MaxEncodeDuration, whatever the sink: Transform asks the decoder to skip to the end before the encode,
+//     which it refuses (ErrSkipNotSupported).
+// The third is NoResize: Transform hands a still's frame straight to the encoder, so the item takes the grid and its
+// unpacked frame goes to the sink unresized.  A size outside the box stays per image, which refuses it.
+static void parse_frame_pair(const lp_xbatch* X, int i, XItem& it, const Rendition& R, int max_side) {
+    const int w = X->src_w[i], h = X->src_h[i];
+    if (w < 1 || h < 1 || w > X->frames.width || h > X->frames.height || w > max_side || h > max_side) return;
+    if (R.opt.max_encode_duration_ns < 0 || !png_option_gates(R, true)) return;
+    it.w = w;
+    it.h = h;
+    it.ch = X->frames.channels;
+    if (R.opt.resize_method == LP_OPS_NO_RESIZE) {
+        it.ow = it.cw = w;
+        it.oh = it.chh = h;
+        it.cx = it.cy = 0;
+    } else if (!plan_geometry(R.opt, &it)) {
+        return;
+    }
+    it.kind = K_FRAME;
+}
+
 // the gates of pair (i, r): it takes the grid when they pass; anything else goes to lp_transform(in[i], opts[r])
 static void parse_pair(lp_xbatch* X, int i, int r, ItemHeaders* c) {
     XItem& it = X->items[(size_t)i * X->k + r];
     const Rendition& R = X->rend[r];
     const lp_image_options& opt = R.opt;
-    const uint8_t* d = X->in[i];
-    const size_t n = X->in_len[i];
     it.kind = K_FALLBACK;
     it.icc.clear();
-    it.span = n;
-    if (!d || n < 16 || R.sink == S_NONE) return;
     const int max_side = X->cfg.max_size > 0 ? X->cfg.max_size : 8192;
+    // To PNG every still is one frame in, the file out of the first Encode call: MaxEncodeFrames, DisableAnimatedOutput
+    // and the deadline are never consulted.  A negative MaxEncodeDuration is exceeded before the frame is encoded, and
+    // Transform then asks the decoder to skip to the end, which no still decoder can (ErrSkipNotSupported): per image.
+    if (R.sink == S_NONE || (R.sink == S_PNG && opt.max_encode_duration_ns < 0)) return;
+    if (X->src_w) {
+        parse_frame_pair(X, i, it, R, max_side);
+        return;
+    }
+    const uint8_t* d = X->in[i];
+    const size_t n = X->in_len[i];
+    it.span = n;
+    if (!d || n < 16) return;
     if (R.sink == S_FRAMES) {
         parse_frames_pair(it, opt, d, n, max_side);
         return;
     }
-    // To PNG every still is one frame in, the file out of the first Encode call: MaxEncodeFrames, DisableAnimatedOutput
-    // and the deadline are never consulted.  A negative MaxEncodeDuration is exceeded before the frame is encoded, and
-    // Transform then asks the decoder to skip to the end, which no still decoder can (ErrSkipNotSupported): per image.
-    if (R.sink == S_PNG && opt.max_encode_duration_ns < 0) return;
     static const uint8_t png_sig[8] = {0x89, 0x50, 0x4E, 0x47, 0x0D, 0x0A, 0x1A, 0x0A};
     thread_local std::vector<uint8_t> icc_buf(32768);
     if (d[0] == 0xFF && d[1] == 0xD8) {
@@ -416,7 +468,6 @@ static void parse_pair(lp_xbatch* X, int i, int r, ItemHeaders* c) {
         return;
     }
     if (!memcmp(d, png_sig, 8)) {
-        if (R.sink == S_GIF) return;  // GIF output needs a GIF source: per image (ErrGifEncoderNeedsDecoder)
         if (c->png < 0) {
             c->ph = png_grid_header(d, n, max_side);
             c->png = c->ph != nullptr;
@@ -435,17 +486,9 @@ static void parse_pair(lp_xbatch* X, int i, int r, ItemHeaders* c) {
         it.h = h.height;
         it.ch = h.out_channels;
         if (!plan_geometry(opt, &it)) return;
-        if (R.sink == S_WEBP) {
-            const int icc_n = png_extract_icc(d, n, icc_buf.data(), icc_buf.size());
-            // PNGs with a profile stay per image, where they went before they could carry it, under the options whose
-            // result the per-image path decides after the frame: a zero encode budget (the deadline check, as for WebP
-            // stills), MaxEncodeFrames == 1 and a negative MaxEncodeDuration (the skip to the end a PNG decoder
-            // refuses, as a JPEG's does).  To lossless output every PNG follows that rule.
-            if ((icc_n > 0 || R.lossless) &&
-                (opt.encode_timeout_ns <= 0 || opt.max_encode_frames == 1 || opt.max_encode_duration_ns < 0))
-                return;
-            keep_icc(&it, icc_buf.data(), icc_n);
-        }
+        const int icc_n = R.sink == S_WEBP ? png_extract_icc(d, n, icc_buf.data(), icc_buf.size()) : 0;
+        if (!png_option_gates(R, icc_n > 0)) return;
+        if (R.sink == S_WEBP) keep_icc(&it, icc_buf.data(), icc_n);
         it.png = c->ph;
         it.kind = K_PNG;
         return;
@@ -1112,6 +1155,65 @@ static void run_webp(lp_xbatch* X, Lane& L, const Task& t) {
     for (int p : failed) push_fallback(X, p);
 }
 
+// Tensor task (lp_xbatch_encode_frames, one rendition): one unpack launch turns every item's slice into a packed u8 frame
+// (its "decode"), then the PNG task's path: per run of equal geometry one resize and the sink.  Under NoResize no resize
+// runs and the sink reads the unpacked frames.  Only the item table crosses PCIe on the way in.
+static void run_frame(lp_xbatch* X, Lane& L, const Task& t) {
+    const std::vector<int>& idx = t.idx;
+    const int n = (int)idx.size();
+    const bool resize = X->rend[0].opt.resize_method != LP_OPS_NO_RESIZE;
+    Bump bump{L.dev, L.dev_bytes};
+    std::vector<uint64_t> frame_off((size_t)n), out_off((size_t)n);
+    size_t frame_bytes = 0, out_bytes = 0;
+    uint64_t max_frame = 0;
+    for (int k = 0; k < n; k++) {
+        const XItem& it = X->items[idx[k]];
+        const size_t fb = (size_t)it.w * it.h * it.ch;
+        frame_off[k] = frame_bytes;
+        frame_bytes += round_up(fb, (size_t)256);
+        max_frame = std::max<uint64_t>(max_frame, fb);
+        out_off[k] = out_bytes;
+        out_bytes += round_up((size_t)it.ow * it.oh * it.ch, (size_t)256);
+    }
+    FrameUnpackItem* d_tab = bump.take<FrameUnpackItem>((size_t)n * sizeof(FrameUnpackItem));
+    uint8_t* d_frames = bump.take<uint8_t>(frame_bytes + 256);
+    uint8_t* d_out = resize ? bump.take<uint8_t>(out_bytes + 256) : d_frames;
+    if (!d_tab || !d_frames || !d_out) {
+        push_task_fallback(X, t);
+        return;
+    }
+    if (!resize) out_off = frame_off;
+    std::vector<FrameUnpackItem> tab((size_t)n);
+    for (int k = 0; k < n; k++) {
+        const XItem& it = X->items[idx[k]];
+        tab[k] = FrameUnpackItem{d_frames + frame_off[k], it.w, it.h, idx[k]};
+    }
+    bool ok = cudaMemcpyAsync(d_tab, tab.data(), tab.size() * sizeof(FrameUnpackItem), cudaMemcpyHostToDevice, L.st) == cudaSuccess;
+    L.h2d += tab.size() * sizeof(FrameUnpackItem);
+    cudaEventRecord(L.ev[0], L.st);
+    if (ok) ok = frames_unpack_launch(d_tab, nullptr, n, max_frame, frames_layout(X->frames), L.st) == LP_OK;
+    cudaEventRecord(L.ev[1], L.st);
+    if (resize)
+        for (const Run& u : task_runs(X, t, 0, 0, n, false))
+            ok = ok && resize_run(L, X->items[idx[u.k0]], d_frames + frame_off[u.k0], d_out + out_off[u.k0], u.k1 - u.k0);
+    cudaEventRecord(L.ev[2], L.st);
+    if (ok) ok = cudaStreamSynchronize(L.st) == cudaSuccess;
+    if (!ok) {
+        cudaGetLastError();
+        push_task_fallback(X, t);
+        return;
+    }
+    lane_time(L, 0, 1, &L.ms_decode);
+    lane_time(L, 1, 2, &L.ms_resize);
+    std::vector<int> failed;
+    for (const Run& u : task_runs(X, t, 0, 0, n, true)) {
+        const XItem& g = X->items[idx[u.k0]];
+        sink_encode(X, L, bump, L.host, L.host_bytes, t, 0, u, nullptr, d_out + out_off[u.k0], round_up((size_t)g.ow * g.oh * g.ch, (size_t)256),
+                    &failed);
+    }
+    for (int p : failed) push_fallback(X, p);
+}
+
 // ------------------------------------------------------------------ GIF groups (animations -> animated WebP or GIF)
 
 // a GIF task holds one rendition: its pairs go through the decode, resize and sink as in a call with those options
@@ -1437,6 +1539,8 @@ static size_t item_device_bytes(const lp_xbatch* X, int i, uint32_t rm) {
                    it.webp->frames.size() * (round_up((size_t)it.w * it.h * it.ch, (size_t)256) + outb) + 8192;
         case K_GIF:
             return gif_plan_device_bytes(it.gif.get()) + (size_t)it.gif_frames * ((size_t)it.w * it.h * 4 + outb) + 8192 + gif_enc;
+        case K_FRAME:  // the unpacked frame, its table entry and its output
+            return round_up((size_t)it.w * it.h * it.ch, (size_t)256) + sizeof(FrameUnpackItem) + outb + 8192;
         default:
             return 0;
     }
@@ -1490,6 +1594,26 @@ static int frames_transform(lp_xbatch* X, int i, const lp_image_options* opt, in
     });
 }
 
+// lp_xbatch_encode_frames' per-image route: Transform with a decoder that answers as a PNG of the frame would, whose
+// DecodeTo unpacks slice i with the grid path's kernel into the framebuffer's device mirror on this worker's stream.
+// A size outside the box is refused here.
+static int transform_from_frame(lp_xbatch* X, int i, const lp_image_options* opt, int max_size, uint8_t* dst, size_t* len) {
+    const lp_frame_tensor& T = X->frames;
+    const int w = X->src_w[i], h = X->src_h[i];
+    if (w < 1 || h < 1 || w > T.width || h > T.height) return LP_ERR_BAD_ARGUMENT;
+    return lilliput::TransformFromFrame(w, h, T.channels, opt, max_size, [&](lilliput::Framebuffer* f) -> int {
+        uint8_t* dev = nullptr;
+        size_t step = 0;
+        int rc = mat_bind_device_frame(f->mat, w, h, f->Type().v, &dev, &step);
+        if (rc) return rc;
+        const FrameUnpackItem one{dev, w, h, i};
+        cudaStream_t st = thread_stream();
+        rc = frames_unpack_launch(nullptr, &one, 1, (uint64_t)w * h * T.channels, frames_layout(T), st);
+        if (!rc && cudaStreamSynchronize(st) != cudaSuccess) rc = LP_ERR_CUDA;
+        return rc;
+    }, dst, X->out_cap, len);
+}
+
 // One call over n items and k renditions (rends: each one's sink, made from opts[r]); the arguments are checked
 static int xbatch_call(lp_xbatch* X, const uint8_t* const* in, const size_t* in_len, int n, const lp_image_options* opts,
                        const Rendition* rends, int k, uint8_t* const* out, size_t out_cap, size_t* out_len, int* status) {
@@ -1535,12 +1659,13 @@ static int xbatch_call(lp_xbatch* X, const uint8_t* const* in, const size_t* in_
     std::vector<Task> tasks;
     std::vector<double> cost;  // rough device time: the longest tasks start first
     const size_t lane_cap = X->lanes[0].dev_bytes;
-    // PNG and WebP: all geometries of a kind in as few tasks as the arena allows (the map keeps equal
+    // PNG, WebP and tensor items: all geometries of a kind in as few tasks as the arena allows (the map keeps equal
     // geometries adjacent); at least two, so both lanes work.  GIF: by canvas size.  JPEG: by geometry.
     std::map<int, std::vector<int>> merged;
     for (auto& kv : groups) {
         const Kind kind = (Kind)std::get<0>(kv.first);
-        if (kind == K_PNG || kind == K_WEBP) merged[(int)kind].insert(merged[(int)kind].end(), kv.second.begin(), kv.second.end());
+        if (kind == K_PNG || kind == K_WEBP || kind == K_FRAME)
+            merged[(int)kind].insert(merged[(int)kind].end(), kv.second.begin(), kv.second.end());
     }
     // g: items with the renditions each runs in the tasks made from it
     auto split_by_memory = [&](Kind kind, const std::vector<std::pair<int, uint32_t>>& g) {
@@ -1612,7 +1737,7 @@ static int xbatch_call(lp_xbatch* X, const uint8_t* const* in, const size_t* in_
     for (auto& kv : groups) {
         const Kind kind = (Kind)std::get<0>(kv.first);
         const std::vector<int>& g = kv.second;
-        if (kind == K_PNG || kind == K_WEBP) continue;
+        if (kind == K_PNG || kind == K_WEBP || kind == K_FRAME) continue;
         if (kind == K_JPEG) {
             // host staging bounds a JPEG task: out slots (the pipelined JPEG path only) + item mirrors come from the lane's
             // pinned arena
@@ -1660,6 +1785,7 @@ static int xbatch_call(lp_xbatch* X, const uint8_t* const* in, const size_t* in_
                 case K_PNG: run_png(X, L, task); break;
                 case K_WEBP: run_webp(X, L, task); break;
                 case K_GIF: run_gif(X, L, task); break;
+                case K_FRAME: run_frame(X, L, task); break;
                 default: push_task_fallback(X, task); break;
             }
         }
@@ -1683,6 +1809,9 @@ static int xbatch_call(lp_xbatch* X, const uint8_t* const* in, const size_t* in_
             size_t len = 0;
             if (X->rend[p % k].sink == S_FRAMES) {
                 status[p] = frames_transform(X, i, &opts[p % k], max_size);
+            } else if (X->src_w) {
+                status[p] = transform_from_frame(X, i, &opts[p % k], max_size, out[p], &len);
+                out_len[p] = status[p] == LP_OK ? len : 0;
             } else {
                 status[p] = lp_transform(in[i], in_len[i], &opts[p % k], out[p], out_cap, &len, max_size);
                 out_len[p] = status[p] == LP_OK ? len : 0;
@@ -1749,22 +1878,30 @@ static bool on_device(const void* p, size_t bytes, int device) {
     return true;
 }
 
+// The tensor checks of lp_xbatch_decode_frames and lp_xbatch_encode_frames: a known dtype, data aligned to it, 3 or 4
+// channels, a box of at least 1 x 1, n slices within `bytes`, all of them device memory of the context's device.
+// *slice: the bytes of one slice.
+static int check_frame_tensor(const lp_xbatch* X, const lp_frame_tensor* t, int n, size_t* slice) {
+    if (!t) return LP_ERR_BAD_ARGUMENT;
+    const lp_frame_tensor& T = *t;
+    const size_t es = frames_dtype_bytes(T.dtype);
+    if (!es || !T.data || (uintptr_t)T.data % es || (T.channels != 3 && T.channels != 4) || T.height < 1 || T.width < 1)
+        return LP_ERR_BAD_ARGUMENT;
+    if (__builtin_mul_overflow((size_t)T.height * (size_t)T.width, (size_t)T.channels * es, slice) ||
+        (n > 0 && *slice > T.bytes / (size_t)n))
+        return LP_ERR_BAD_ARGUMENT;
+    DeviceGuard g(X->device);
+    if (!g.ok || !on_device(T.data, std::max<size_t>(1, *slice * (size_t)n), X->device)) return LP_ERR_BAD_ARGUMENT;
+    return LP_OK;
+}
+
 extern "C" int lp_xbatch_decode_frames(lp_xbatch* X, const uint8_t* const* in, const size_t* in_len, int n,
                                        const lp_image_options* opt, const lp_frame_tensor* dst, int* width, int* height,
                                        int* status) {
     if (!X || n < 0 || !opt || !dst || (n > 0 && (!in || !in_len || !width || !height || !status))) return LP_ERR_BAD_ARGUMENT;
-    const lp_frame_tensor T = *dst;
-    const size_t es = frames_dtype_bytes(T.dtype);
-    if (!es || !T.data || (uintptr_t)T.data % es || (T.channels != 3 && T.channels != 4) || T.height < 1 || T.width < 1)
-        return LP_ERR_BAD_ARGUMENT;
     size_t slice = 0;
-    if (__builtin_mul_overflow((size_t)T.height * (size_t)T.width, (size_t)T.channels * es, &slice) ||
-        (n > 0 && slice > T.bytes / (size_t)n))
-        return LP_ERR_BAD_ARGUMENT;
-    {
-        DeviceGuard g(X->device);
-        if (!g.ok || !on_device(T.data, std::max<size_t>(1, slice * (size_t)n), X->device)) return LP_ERR_BAD_ARGUMENT;
-    }
+    if (check_frame_tensor(X, dst, n, &slice)) return LP_ERR_BAD_ARGUMENT;
+    const lp_frame_tensor T = *dst;
     X->frames = T;
     X->frame_w = width;
     X->frame_h = height;
@@ -1789,6 +1926,21 @@ extern "C" int lp_xbatch_decode_frames(lp_xbatch* X, const uint8_t* const* in, c
     }
     if (!rc && cudaStreamSynchronize(st) != cudaSuccess) rc = LP_ERR_CUDA;
     X->frame_w = X->frame_h = nullptr;
+    return rc;
+}
+
+extern "C" int lp_xbatch_encode_frames(lp_xbatch* X, const lp_frame_tensor* src, int n, const int* width, const int* height,
+                                       const lp_image_options* opt, uint8_t* const* out, size_t out_cap, size_t* out_len,
+                                       int* status) {
+    if (!X || n < 0 || (n > 0 && (!opt || !width || !height || !out || !out_len || !status))) return LP_ERR_BAD_ARGUMENT;
+    size_t slice = 0;
+    if (check_frame_tensor(X, src, n, &slice)) return LP_ERR_BAD_ARGUMENT;
+    X->frames = *src;
+    X->src_w = width;
+    X->src_h = height;
+    const Rendition R = opt ? make_rendition(*opt) : Rendition();  // (opt may be null when n == 0)
+    const int rc = xbatch_call(X, nullptr, nullptr, n, opt, &R, 1, out, out_cap, out_len, status);
+    X->src_w = X->src_h = nullptr;
     return rc;
 }
 

@@ -969,6 +969,55 @@ Error TransformToFrame(const uint8_t* in, size_t in_len, const lp_image_options*
     }
 }
 
+// A decoder of one w x h frame of 3 (BGR) or 4 (BGRA) channels whose pixels `fill` writes, answering as OpenCVDecoder
+// answers for an 8-bit PNG of colour type 2 or 6 without ancillary chunks: orientation 1, one frame, no ICC profile, no
+// cICP, no GIF handle
+class FrameDecoder : public Decoder {
+  public:
+    FrameDecoder(int w, int h, int channels, const FrameSink& f) : width(w), height(h), type(channels == 4 ? CV_8UC4 : CV_8UC3), fill(f) {}
+    Error Header(ImageHeader* h) override {
+        h->width = width;
+        h->height = height;
+        h->pixelType.v = type;
+        h->orientation = 1;
+        h->numFrames = 1;
+        return LP_OK;
+    }
+    std::string Description() override { return "PNG"; }
+    Error DecodeTo(Framebuffer* f) override {  // as OpenCVDecoder::DecodeTo
+        if (decoded) return LP_ERR_EOF;
+        Error e = f->resizeMat(width, height, PixelType{type});
+        if (e) return e;
+        if ((e = fill(f))) return e;
+        decoded = true;
+        f->blend = NoBlend;
+        f->dispose = DisposeToBackgroundColor;
+        f->xOffset = 0;
+        f->yOffset = 0;
+        f->duration_ns = 0;
+        return LP_OK;
+    }
+    Error SkipFrame() override { return LP_ERR_SKIP_NOT_SUPPORTED; }
+
+  private:
+    int width, height, type;
+    const FrameSink& fill;
+    bool decoded = false;
+};
+
+Error TransformFromFrame(int w, int h, int channels, const lp_image_options* opt, int max_size, const FrameSink& fill, uint8_t* dst,
+                         size_t dst_cap, size_t* out_len) {
+    try {
+        if (!opt || !dst || !out_len) return LP_ERR_BAD_ARGUMENT;
+        FrameDecoder d(w, h, channels, fill);
+        return thread_ops(max_size)->Transform(&d, fromC(opt), dst, dst_cap, out_len);
+    } catch (const std::bad_alloc&) {
+        return LP_ERR_BUF_TOO_SMALL;
+    } catch (...) {
+        return LP_ERR_BAD_ARGUMENT;
+    }
+}
+
 }  // namespace lilliput
 
 static int lp_decode_host_impl(const uint8_t* in, size_t in_len, uint8_t* pixels,

@@ -195,4 +195,10 @@ class ImageOps {  // ref ops.go:67-150
 using FrameSink = std::function<Error(Framebuffer*)>;
 Error TransformToFrame(const uint8_t* in, size_t in_len, const lp_image_options* opt, int max_size, const FrameSink& sink);
 
+// The mirror of TransformToFrame: lp_transform of an 8-bit PNG of a w x h frame of `channels` (3: BGR, 4: BGRA) into dst.
+// Transform runs with a FrameDecoder, which answers every Decoder call as OpenCVDecoder answers for such a PNG; its
+// DecodeTo sizes the framebuffer (resizeMat) and then calls fill, which writes the frame's pixels into it.
+Error TransformFromFrame(int w, int h, int channels, const lp_image_options* opt, int max_size, const FrameSink& fill, uint8_t* dst,
+                         size_t dst_cap, size_t* out_len);
+
 }  // namespace lilliput
