@@ -289,6 +289,35 @@ int lp_xbatch_decode_frames(lp_xbatch* x, const uint8_t* const* in, const size_t
                             const lp_image_options* opt, const lp_frame_tensor* dst, int* width, int* height,
                             int* status);
 
+/* Clips instead of one frame: up to T = frames_per_item frames of every item, spread over the whole animation, written
+ * into the caller's device tensor.  Slice i * T + t of dst (the same lp_frame_tensor as lp_xbatch_decode_frames, n * T
+ * slices; with nchw an N x T x C x H x W tensor) holds slot t of item i.
+ *   - item i's frames are the ones lp_transform(in[i], opt) hands its encoder, in order: decoded, tone-mapped if HDR,
+ *     oriented, composited as Transform composites them, with Fit / Resize / NoResize applied.  opt's width, height,
+ *     resize_method, normalize_orientation and force_sdr count; file_type, the encode options, max_encode_frames,
+ *     max_encode_duration_ns, disable_animated_output and encode_timeout_ns are ignored.  Frame 0 is exactly what
+ *     lp_xbatch_decode_frames writes for the item.
+ *   - F = nframes[i], the frame count the decoder's header reports: a GIF's record walk, a WebP's container frame
+ *     count, and 1 for every other source (an APNG included: Transform decodes its first frame only)
+ *   - sampling: when F <= T, slot t < F holds frame t; otherwise slot t holds frame floor(t * F / T), T distinct frames
+ *     with frame 0 first.  Decoding stops after the last selected frame L: nothing behind it is read, so damage behind
+ *     L is never seen
+ *   - frame_index[i * T + t]: the slot's frame index, -1 for an unused slot.  start_ms[i * T + t]: the sum of the
+ *     durations (in ms, as the decoder reports them) of frames 0 .. index - 1; 0 for an unused slot
+ *   - an unused slot is all zero, as is a slot whose frame the stream ended before delivering (its index is -1)
+ *   - width[i] x height[i]: the size of every frame of the item.  status[i]: Transform's status.  A frame larger than
+ *     the box in either dimension: LP_ERR_BUF_TOO_SMALL.  An item whose status is not LP_OK: T all-zero slices, 0 x 0,
+ *     nframes 0, every index -1
+ * Slices are packed as lp_xbatch_decode_frames packs them.  dst must stay allocated for the call, on the context's
+ * device; every write into it is complete when the call returns.  LP_ERR_BAD_ARGUMENT, with nothing written, for: the
+ * tensor checks of lp_xbatch_decode_frames with n * T slices in place of n; T outside 1..LP_XBATCH_MAX_CLIP_FRAMES;
+ * n < 0; a null in / in_len / opt / output array with n > 0.
+ * Stats: grid_items / fallback_items count items; ms_encode is the pack; d2h_bytes carries no pixels. */
+#define LP_XBATCH_MAX_CLIP_FRAMES 4096
+int lp_xbatch_decode_clips(lp_xbatch* x, const uint8_t* const* in, const size_t* in_len, int n,
+                           const lp_image_options* opt, int frames_per_item, const lp_frame_tensor* dst, int* width,
+                           int* height, int* nframes, int* frame_index, int64_t* start_ms, int* status);
+
 /* Files from pixels: slice i of the caller's device tensor src (the same lp_frame_tensor as lp_xbatch_decode_frames)
  * holds item i's frame at its top-left, width[i] x height[i].  The frame is converted to 8-bit BGR (channels 3) or BGRA
  * (channels 4) and goes through ImageOps.Transform with opt: status and bytes of item i are exactly those of

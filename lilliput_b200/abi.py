@@ -518,6 +518,10 @@ class XBatch:
         l.lp_xbatch_decode_frames.restype = C.c_int
         l.lp_xbatch_decode_frames.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.POINTER(_ImageOptions),
                                               C.POINTER(_FrameTensor), C.c_void_p, C.c_void_p, C.c_void_p]
+        l.lp_xbatch_decode_clips.restype = C.c_int
+        l.lp_xbatch_decode_clips.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.POINTER(_ImageOptions), C.c_int,
+                                             C.POINTER(_FrameTensor), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                             C.c_void_p, C.c_void_p]
         l.lp_xbatch_encode_frames.restype = C.c_int
         l.lp_xbatch_encode_frames.argtypes = [C.c_void_p, C.POINTER(_FrameTensor), C.c_int, C.c_void_p, C.c_void_p,
                                               C.POINTER(_ImageOptions), C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p]
@@ -570,6 +574,28 @@ class XBatch:
         if rc:
             raise LilliputError(rc)
         return list(w[:n]), list(h[:n]), list(status[:n])
+
+    def decode_clips(self, bufs, opt: ImageOptions, frames_per_item: int, data_ptr: int, bytes: int, height: int, width: int,
+                     channels: int = 3, nchw: bool = False, rgb: bool = True, dtype: str = "u8", scale=None, bias=None):
+        """lp_xbatch_decode_clips: up to T = frames_per_item frames of every file, spread over the animation (slot t of F > T
+        frames: frame t * F // T), written into slices i * T + t of the device tensor at data_ptr (laid out as for
+        decode_frames, N * T slices).  Returns (width, height, nframes, frame_index, start_ms, status): per item, per item,
+        per item, per slot (-1: unused), per slot (ms before the slot's frame), per item."""
+        n, T = len(bufs), frames_per_item
+        ptrs, lens, keep = Batch._ptr_arrays(bufs)
+        t = _FrameTensor(data_ptr, bytes, height, width, channels, int(bool(nchw)), int(bool(rgb)),
+                         FRAME_DTYPES.get(dtype, -1) if isinstance(dtype, str) else int(dtype),
+                         (C.c_float * 4)(*(list(scale) if scale is not None else [1.0] * 4)),
+                         (C.c_float * 4)(*(list(bias) if bias is not None else [0.0] * 4)))
+        w, h, nf, status = [(C.c_int * max(n, 1))() for _ in range(4)]
+        slots = max(n * max(T, 0), 1)
+        index, start = (C.c_int * slots)(), (C.c_int64 * slots)()
+        copt = opt._c()
+        rc = self.lib.l.lp_xbatch_decode_clips(self.h, ptrs, lens, n, C.byref(copt), T, C.byref(t), w, h, nf, index, start, status)
+        if rc:
+            raise LilliputError(rc)
+        m = n * T
+        return list(w[:n]), list(h[:n]), list(nf[:n]), list(index[:m]), list(start[:m]), list(status[:n])
 
     def encode_frames(self, data_ptr: int, bytes: int, widths, heights, opt: ImageOptions, height: int, width: int,
                       channels: int = 3, nchw: bool = False, rgb: bool = True, dtype: str = "u8", scale=None, bias=None,

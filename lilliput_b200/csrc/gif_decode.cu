@@ -449,7 +449,7 @@ struct GifFrameJob {
     int32_t fl, ft, fw, fh, interlace, transparent, ncolors;
     int32_t prev_disposal, pl, pt, pw, ph;
     int32_t status;
-    int32_t pad_;
+    int32_t canvas;  // canvas index the composited frame is stored at, from `canvases`; -1: composited, not stored
 };
 struct GifAnimJob {
     int32_t first_frame, nframes;
@@ -486,8 +486,11 @@ __global__ void __launch_bounds__(32) gif_lzw_kernel(GifFrameJob* jobs, uint8_t*
     if (threadIdx.x == 0) j.status = status;
 }
 
-__global__ void gif_compose_kernel(const GifAnimJob* anims, const GifFrameJob* jobs, const uint8_t* base, int cw, int chh,
-                                   uint8_t* canvases, size_t canvas_stride) {
+// (launched with 128 threads; the bound holds it at 32 registers, a full SM of warps, with no spill: the store slot's
+// address would otherwise take two more)
+__global__ void __launch_bounds__(128, 16)
+    gif_compose_kernel(const GifAnimJob* anims, const GifFrameJob* jobs, const uint8_t* base, int cw, int chh, uint8_t* canvases,
+                       size_t canvas_stride) {
     const int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y;
     if (x >= cw) return;
     const GifAnimJob a = anims[blockIdx.z];
@@ -497,37 +500,39 @@ __global__ void gif_compose_kernel(const GifAnimJob* anims, const GifFrameJob* j
         px = *reinterpret_cast<const uchar4*>(canvases + (size_t)a.first_frame * canvas_stride + at);
         snap = *reinterpret_cast<const uchar4*>(a.snap + at);
     }
-    const int fill_k = a.fill_bg ? 0 : -1;  // the frame that starts from the background fill, if any
-    for (int k = 0; k < a.nframes; k++) {
-        const GifFrameJob& c = jobs[a.first_frame + k];
-        if (k == fill_k) {
+    bool fill = a.fill_bg;  // the job's first frame starts from the background fill
+    for (const GifFrameJob *c = jobs + a.first_frame, *end = c + a.nframes; c < end; c++) {
+        if (fill) {
             px = a.bg;
+            fill = false;
         } else {
-            const bool in_prev = x >= c.pl && x < c.pl + c.pw && y >= c.pt && y < c.pt + c.ph;
-            if (in_prev && c.prev_disposal == 2) px = a.bg;
-            else if (in_prev && c.prev_disposal == 3) px = snap;
+            const bool in_prev = x >= c->pl && x < c->pl + c->pw && y >= c->pt && y < c->pt + c->ph;
+            if (in_prev && c->prev_disposal == 2) px = a.bg;
+            else if (in_prev && c->prev_disposal == 3) px = snap;
             snap = px;  // snapshot after disposal, before drawing
         }
-        const int fx = x - c.fl, fy = y - c.ft;
-        if (fx >= 0 && fx < c.fw && fy >= 0 && fy < c.fh) {
+        const int fx = x - c->fl, fy = y - c->ft;
+        if (fx >= 0 && fx < c->fw && fy >= 0 && fy < c->fh) {
             int row = fy;
-            if (c.interlace) {
-                const int h = c.fh;
+            if (c->interlace) {
+                const int h = c->fh;
                 const int n0 = (h + 7) / 8, n1 = (h + 3) / 8, n2 = (h + 1) / 4;
                 if ((fy & 7) == 0) row = fy / 8;
                 else if ((fy & 7) == 4) row = n0 + fy / 8;
                 else if ((fy & 3) == 2) row = n0 + n1 + fy / 4;
                 else row = n0 + n1 + n2 + fy / 2;
             }
-            const int idx = base[c.idx_off + (size_t)row * c.fw + fx];
-            if (idx != c.transparent && idx < c.ncolors) {
-                const uint8_t* pal = base + c.colors_off + (size_t)idx * 3;
+            const int idx = base[c->idx_off + (size_t)row * c->fw + fx];
+            if (idx != c->transparent && idx < c->ncolors) {
+                const uint8_t* pal = base + c->colors_off + (size_t)idx * 3;
                 px = make_uchar4(pal[2], pal[1], pal[0], 255);
             }
         }
-        *reinterpret_cast<uchar4*>(canvases + (size_t)(a.first_frame + k) * canvas_stride + at) = px;
+        if (c->canvas >= 0) *reinterpret_cast<uchar4*>(canvases + (size_t)c->canvas * canvas_stride + at) = px;
     }
-    if (a.snap) *reinterpret_cast<uchar4*>(a.snap + at) = snap;
+    // (re-read: the snapshot pointer is not held across the frame loop)
+    uint8_t* const sp = anims[blockIdx.z].snap;
+    if (sp) *reinterpret_cast<uchar4*>(sp + at) = snap;
 }
 
 // LZW and compositing of `nf` frame jobs, whose code streams are already contiguous, and `n` animation jobs, all in
@@ -556,6 +561,7 @@ struct GifFramePlan {
     bool local = false;
     std::vector<GifExt> ext;
     GifGcb enc_gcb;
+    size_t end_pos = 0;  // behind the frame's block terminator
 };
 struct GifAnimPlan {
     int sw = 0, sh = 0, loop_count = 1;
@@ -662,6 +668,7 @@ GifAnimPlan* gif_plan_parse(const uint8_t* data, size_t len, int max_frames, boo
         }
         if (total > 0xFFFFFF00u) return nullptr;
         f.lzw_len = (uint32_t)total;
+        f.end_pos = r.pos;
         const GifGcb g = gcbs.empty() ? GifGcb() : gcbs.back();
         f.transparent = g.transparent;
         f.disposal = g.disposal;
@@ -712,6 +719,17 @@ void gif_plan_info(const GifAnimPlan* p, int* width, int* height, int* nframes, 
     if (loop_count) *loop_count = p->loop_count;
 }
 size_t gif_plan_file_bytes(const GifAnimPlan* p) { return p->file_len; }
+// (a cut plan is decoded, never written: the writer's trailing extensions and palette runs stay the full walk's)
+size_t gif_plan_cut(GifAnimPlan* p, int last) {
+    p->frames.resize((size_t)last + 1);
+    p->lzw_total = p->idx_total = 0;
+    for (const GifFramePlan& f : p->frames) {
+        p->lzw_total += round_up((size_t)f.lzw_len + 32, (size_t)16);
+        p->idx_total += round_up((size_t)f.width * f.height + 64, (size_t)16);
+    }
+    p->file_len = p->frames.back().end_pos;
+    return p->file_len;
+}
 int gif_plan_delay_ms(const GifAnimPlan* p, int frame) { return p->frames[(size_t)frame].delay * 10; }  // ref giflib.go:212
 size_t gif_plan_device_bytes(const GifAnimPlan* p) {
     return round_up(p->file_len + 64, (size_t)256) + p->lzw_total + p->idx_total +
@@ -720,7 +738,7 @@ size_t gif_plan_device_bytes(const GifAnimPlan* p) {
 
 int gif_decode_batch(GifAnimPlan* const* plans, const uint8_t* const* files, const size_t* file_len, int n,
                      uint8_t* d_scratch, size_t scratch_bytes, uint8_t* d_canvases, size_t canvas_stride,
-                     const int* first_frame, int* h_status, cudaStream_t st) {
+                     const int* first_frame, int* h_status, cudaStream_t st, const int* canvas_of) {
     if (n <= 0) return LP_OK;
     const int nf = first_frame[n];
     std::vector<GifFrameJob> jobs((size_t)nf);
@@ -745,6 +763,7 @@ int gif_decode_batch(GifAnimPlan* const* plans, const uint8_t* const* files, con
             GifFrameJob& j = jobs[(size_t)first_frame[a] + k];
             j = gif_frame_job(f, file_off[a], prev_disposal, pl, pt, pw, ph, cw, chh);
             j.lzw_off = off;
+            j.canvas = canvas_of ? canvas_of[first_frame[a] + k] : first_frame[a] + (int)k;
             off += round_up((size_t)f.lzw_len + 32, (size_t)16);
             prev_disposal = f.disposal;
             pl = f.left; pt = f.top; pw = f.width; ph = f.height;
@@ -1312,6 +1331,7 @@ bool giflib_decoder_decode_frame(giflib_decoder d, opencv_mat mat) {  // ref gif
     GifFrameJob job = gif_frame_job(f, 0, d->prev_disposal, d->prev_left, d->prev_top, d->prev_width, d->prev_height,
                                     cw, chh);
     job.lzw_off = lzw_pos;
+    job.canvas = 0;  // (d_canvas: the one canvas the decoder keeps)
     job.idx_off = lzw_pos + round_up((size_t)f.lzw_len + 32, (size_t)16);  // the word reader may look past the end
     const size_t need = job.idx_off + round_up((size_t)job.npix + 64, (size_t)16);
     if (need > d->scratch_cap) {
@@ -1353,11 +1373,11 @@ bool giflib_decoder_decode_frame(giflib_decoder d, opencv_mat mat) {  // ref gif
 }
 
 // ref giflib.cpp:1308-1431: a second walk over the container
-struct GifAnimationInfo giflib_decoder_get_animation_info(const giflib_decoder d) {
+static GifAnimationInfo animation_info(const uint8_t* data, size_t len) {
     GifAnimationInfo info = {1, 0, 255, 255, 255, 0, 0};
     GifReader r;
-    r.p = d->rd.p;
-    r.n = d->rd.n;
+    r.p = data;
+    r.n = len;
     if (!r.open()) return info;
     bool found_loop = false, found_gcb = false;
     GifGcb first_gcb;
@@ -1422,6 +1442,8 @@ struct GifAnimationInfo giflib_decoder_get_animation_info(const giflib_decoder d
     }
     return info;
 }
+
+struct GifAnimationInfo giflib_decoder_get_animation_info(const giflib_decoder d) { return animation_info(d->rd.p, d->rd.n); }
 
 // ------------------------------------------------------------------ encoder (ref giflib.cpp:726-1306)
 
@@ -1572,3 +1594,7 @@ void giflib_encoder_release(giflib_encoder e) {
 int giflib_encoder_get_output_length(giflib_encoder e) { return (int)e->dst_offset; }
 
 }  // extern "C"
+
+namespace lp {
+int gif_header_frames(const uint8_t* data, size_t len) { return animation_info(data, len).frame_count; }
+}  // namespace lp

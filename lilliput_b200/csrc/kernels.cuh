@@ -292,9 +292,10 @@ struct WebpPlan {
     std::vector<WebpFramePlan> frames;
 };
 bool webp_plan_parse(const uint8_t* data, size_t len, WebpPlan* out);
-// the plan cut to its frame 0, as a Transform that stops after frame 0 decodes it (rectangle, blend and dispose onto the
-// canvas unchanged); returns the bytes at the start of the file that frame needs: through the end of its image data
-size_t webp_plan_first_frame(WebpPlan* p);
+// the plan cut after frame `last`, as a Transform that stops after that frame decodes it (rectangles, blend and dispose
+// onto the canvas unchanged); returns the bytes at the start of the file those frames need: through the end of frame
+// last's image data
+size_t webp_plan_cut(WebpPlan* p, int last);
 // device scratch webp_decode_batch lays out for one plan (uploaded file, VP8 work areas, lossless pixels, alpha planes,
 // job records), not counting the shared VP8L arena
 size_t webp_plan_device_bytes(const WebpPlan& p, size_t file_len);
@@ -303,23 +304,32 @@ size_t webp_plan_arena_bytes(const WebpPlan& p);
 // decodes + composites every frame of `n` WebP files: file a's composited canvas f (plan width x height x channels,
 // round_up(w * h * ch, 256) apart) lands at d_canvases + canvas_off[a] + f * that stride.  Lossless frames and ALPH
 // planes decode in waves of streams whose arena slices fit d_arena.  h_status per file: 0, or the frame failed.
-// ev_uploaded (optional) is recorded once the files are on the device.
+// ev_uploaded (optional) is recorded once the files are on the device.  canvas_of (optional, one entry per frame of
+// all files in order): the canvas each composited frame is stored at in place of f, -1 for none.
 int webp_decode_batch(const WebpPlan* const* plans, const uint8_t* const* files, const size_t* file_len, int n,
                       uint8_t* d_scratch, size_t scratch_bytes, uint8_t* d_arena, size_t arena_bytes, uint8_t* d_canvases,
-                      const uint64_t* canvas_off, int* h_status, cudaEvent_t ev_uploaded, cudaStream_t st);
+                      const uint64_t* canvas_off, int* h_status, cudaEvent_t ev_uploaded, cudaStream_t st,
+                      const int* canvas_of = nullptr);
 struct GifAnimPlan;
 GifAnimPlan* gif_plan_parse(const uint8_t* data, size_t len, int max_frames, bool first_frame_only = false);
 void gif_plan_free(GifAnimPlan* p);
-// bytes at the start of the file the plan reads (the whole file, or through frame 0's image data): what to upload
+// the plan cut after frame `last` (a full walk's plan, as a Transform that stops after that frame decodes it); returns
+// the bytes at the start of the file those frames need: through the end of frame last's image data
+size_t gif_plan_cut(GifAnimPlan* p, int last);
+// the frame count GifDecoder's Header() reports for the file: the reference's record walk (giflib_decoder_get_animation_info)
+int gif_header_frames(const uint8_t* data, size_t len);
+// bytes at the start of the file the plan reads (the whole file, or through the image data of its last frame when the
+// walk stopped at frame 0 or the plan was cut): what to upload
 size_t gif_plan_file_bytes(const GifAnimPlan* p);
 void gif_plan_info(const GifAnimPlan* p, int* width, int* height, int* nframes, uint32_t* bgcolor, int* loop_count);
 int gif_plan_delay_ms(const GifAnimPlan* p, int frame);
 size_t gif_plan_device_bytes(const GifAnimPlan* p);
 // decodes + composites every frame of `n` animations of one canvas size: animation a, frame f lands at
-// d_canvases + (first_frame[a] + f) * canvas_stride (BGRA); h_status per animation
+// d_canvases + (first_frame[a] + f) * canvas_stride (BGRA), or at canvas canvas_of[first_frame[a] + f] when canvas_of is
+// given (-1: composited, not stored); h_status per animation
 int gif_decode_batch(GifAnimPlan* const* plans, const uint8_t* const* files, const size_t* file_len, int n,
                      uint8_t* d_scratch, size_t scratch_bytes, uint8_t* d_canvases, size_t canvas_stride,
-                     const int* first_frame, int* h_status, cudaStream_t st);
+                     const int* first_frame, int* h_status, cudaStream_t st, const int* canvas_of = nullptr);
 // device scratch gif_encode_batch needs for one animation whose frames are resized to ow x oh
 size_t gif_plan_encode_bytes(const GifAnimPlan* p, int ow, int oh);
 // GIF files of `n` animations whose frames, resized to ow x oh BGRA, sit at d_frames + (first_frame[a] + f) * frame_stride:

@@ -370,7 +370,8 @@ struct WebpFrameJob {
     uint64_t work_off;   // lossy: VP8 work area, from the scratch base
     uint64_t px_off;     // lossless: ARGB words; lossy: ALPH plane (~0: none, alpha 255)
     int32_t x, y, w, h;
-    int32_t lossless, blend, dispose, mb_w, mb_h, pad_;
+    int32_t lossless, blend, dispose, mb_w, mb_h;
+    int32_t canvas;  // canvas of its file the composited frame is stored at; -1: composited, not stored
 };
 struct WebpAnimJob {
     uint64_t canvas_off, canvas_stride;
@@ -411,8 +412,10 @@ __global__ void webp_compose_kernel(const WebpAnimJob* anims, const WebpFrameJob
                 blend_px(s, ch, px, ch);
             }
         }
-        uint8_t* d = out + (size_t)k * a.canvas_stride;
-        for (int c = 0; c < ch; c++) d[c] = px[c];
+        if (f.canvas >= 0) {
+            uint8_t* d = out + (size_t)f.canvas * a.canvas_stride;
+            for (int c = 0; c < ch; c++) d[c] = px[c];
+        }
         if (inside && f.dispose) px[0] = px[1] = px[2] = px[3] = 0;
     }
 }
@@ -648,9 +651,9 @@ bool webp_plan_parse(const uint8_t* data, size_t len, WebpPlan* out) {
     return true;
 }
 
-size_t webp_plan_first_frame(WebpPlan* p) {
-    p->frames.resize(1);
-    const WebpFramePlan& f = p->frames[0];
+size_t webp_plan_cut(WebpPlan* p, int last) {
+    p->frames.resize((size_t)last + 1);
+    const WebpFramePlan& f = p->frames[(size_t)last];
     return std::max(f.img_off + f.img_len, f.has_alph ? f.alph_off + f.alph_len : 0);
 }
 
@@ -686,7 +689,8 @@ size_t webp_plan_arena_bytes(const WebpPlan& p) {
 // over every canvas pixel of every file (per run of equal canvas size).
 int webp_decode_batch(const WebpPlan* const* plans, const uint8_t* const* files, const size_t* file_len, int n,
                       uint8_t* d_scratch, size_t scratch_bytes, uint8_t* d_arena, size_t arena_bytes, uint8_t* d_canvases,
-                      const uint64_t* canvas_off, int* h_status, cudaEvent_t ev_uploaded, cudaStream_t st) {
+                      const uint64_t* canvas_off, int* h_status, cudaEvent_t ev_uploaded, cudaStream_t st,
+                      const int* canvas_of) {
     if (n <= 0) return LP_OK;
     int nf = 0;
     for (int a = 0; a < n; a++) nf += (int)plans[a]->frames.size();
@@ -733,6 +737,7 @@ int webp_decode_batch(const WebpPlan* const* plans, const uint8_t* const* files,
             j.mb_w = (f.width + 15) >> 4;
             j.mb_h = (f.height + 15) >> 4;
             j.px_off = ~0ull;
+            j.canvas = canvas_of ? canvas_of[k] : k - aj.first_frame;
             const size_t npix = (size_t)f.width * f.height;
             if (f.lossless) {
                 j.px_off = take(npix * 4);

@@ -32,7 +32,7 @@
 //                 gates of an 8-bit RGB / RGBA PNG (parse_frame_pair), and under NoResize its frame goes to the sink
 //                 unresized
 //        DisableAnimatedOutput (GIF and animated WebP to WebP, GIF to GIF): Transform stops after frame 0, so the plan
-//                 stops there too (gif_plan_parse's first-frame walk, webp_plan_first_frame); only the file up to the
+//                 stops there too (gif_plan_parse's first-frame walk, webp_plan_cut); only the file up to the
 //                 end of frame 0's image data is uploaded, the same kernels run over one frame per file, and the sink
 //                 writes a still WebP or a one-frame GIF
 //      and the sinks: JPEG (jpeg_encode.cu), lossy WebP still / animation (webp_encode.cu) carrying the ICC profile of
@@ -41,7 +41,8 @@
 //      from GIF sources (palette mapping + LZW of every frame of the task, gif_decode.cu; the container assembled on the
 //      host), PNG from JPEG, PNG and WebP stills (filter, DEFLATE, checksums and container of every frame of a run in
 //      three launches, png_encode.cu), and pixels instead of files (lp_xbatch_decode_frames: each run's frames packed
-//      into the caller's device tensor in one launch, frames_pack.cu).  Whatever the decoder kind, a task's decoded frames go through one run walk
+//      into the caller's device tensor in one launch, frames_pack.cu; lp_xbatch_decode_clips: T slots per item, an
+//      animation's plan cut after its last selected frame and only the selected frames' canvases stored).  Whatever the decoder kind, a task's decoded frames go through one run walk
 //      (task_runs: adjacent items that take a rendition and share a geometry), one resize launch per run, and one sink
 //      entry (sink_encode) per run of resized frames;
 //   3. anything the grid path does not cover (gray or over-budget multi-scan JPEGs, gray PNGs, EXIF-rotated sources,
@@ -121,6 +122,9 @@ struct XItem {
     std::shared_ptr<GifAnimPlan> gif;
     int gif_frames = 0;
     size_t span = 0;           // WebP, GIF: bytes at the start of the file the device reads (first-frame items: through frame 0)
+    int nframes = 0;                  // lp_xbatch_decode_clips: F, the frame count the decoder's header reports,
+    std::vector<int> clip;            // the frames of the slots in use (the only canvases stored, the plan cut after the last)
+    std::vector<int64_t> clip_ms;     // and each one's start (ms)
     std::vector<uint8_t> icc;  // WebP sink: the source's profile the WebP writer carries (empty: none, or not sane)
 };
 
@@ -181,6 +185,10 @@ struct lp_xbatch {
     lp_frame_tensor frames;  // lp_xbatch_decode_frames: the caller's tensor, and each item's frame size
     int* frame_w = nullptr;
     int* frame_h = nullptr;
+    int clip_t = 0;  // lp_xbatch_decode_clips: T slots per item (0: lp_xbatch_decode_frames, one), and the slots' outputs
+    int* clip_nframes = nullptr;
+    int* clip_index = nullptr;
+    int64_t* clip_ms = nullptr;
     const int* src_w = nullptr;  // lp_xbatch_encode_frames: the items are slices of `frames`, of these sizes (no files)
     const int* src_h = nullptr;
     int k = 1;              // renditions
@@ -282,14 +290,34 @@ struct ItemHeaders {
     std::shared_ptr<GifAnimPlan> gp[2];
 };
 
+// The slots of a clip of T frames over F (lp_xbatch_decode_clips' sampling rule): frame t while F <= T, otherwise frame
+// floor(t * F / T); each slot's start sums the durations (ms, duration_ms(j) of frame j) of the frames before its own
+template <class D>
+static void select_clip(XItem* it, int F, int T, D duration_ms) {
+    const int used = std::min(F, T);
+    it->nframes = F;
+    it->clip.resize((size_t)used);
+    it->clip_ms.resize((size_t)used);
+    int64_t ms = 0;
+    for (int t = 0, j = 0; t < used; t++) {
+        const int f = F <= T ? t : (int)((int64_t)t * F / T);
+        for (; j < f; j++) ms += duration_ms(j);
+        it->clip[t] = f;
+        it->clip_ms[t] = ms;
+    }
+}
+
 // The gates of an item of lp_xbatch_decode_frames: the frame Transform hands its still ".png" encoder, which answers at
 // once (no deadline, frame limit or flush follows it), so only MaxEncodeDuration -- held against a frame's duration
 // before the encode -- and NoResize send an item per image, besides what each decoder's gate refuses.  JPEG: rotated and
 // gray files too (the group's resize-only lp_batch context orients and decodes both; an item whose orientation swaps the
 // axes gets the turned frame's output size).  PNG: RGB / RGBA of 8 or 16 bits, HDR tone-mapped; an SDR cICP changes no
 // pixel and is written nowhere.  WebP: stills, and animations cut to frame 0.  GIF: the first-frame plan.
-static void parse_frames_pair(XItem& it, const lp_image_options& opt, const uint8_t* d, size_t n, int max_side) {
-    if (opt.max_encode_duration_ns != 0) return;
+// T > 0 (lp_xbatch_decode_clips, T slots): the same gates but MaxEncodeDuration, which the clip ignores.  An animation
+// takes its full plan, whose frame count is F (a GIF's only when it is the count GifDecoder's header walk gives, so both
+// routes agree on it), and is cut after the last selected frame: nothing behind it is uploaded or decoded.
+static void parse_frames_pair(XItem& it, const lp_image_options& opt, const uint8_t* d, size_t n, int max_side, int T) {
+    if (T == 0 && opt.max_encode_duration_ns != 0) return;
     static const uint8_t png_sig[8] = {0x89, 0x50, 0x4E, 0x47, 0x0D, 0x0A, 0x1A, 0x0A};
     if (d[0] == 0xFF && d[1] == 0xD8) {
         JpegHeader h;
@@ -338,8 +366,12 @@ static void parse_frames_pair(XItem& it, const lp_image_options& opt, const uint
             if (f0.x || f0.y || f0.width != p->width || f0.height != p->height) return;
             f0.blend = 1;
             f0.dispose = 0;
+        } else if (T == 0) {
+            it.span = webp_plan_cut(p.get(), 0);
         } else {
-            it.span = webp_plan_first_frame(p.get());
+            const WebpPlan& q = *p;
+            select_clip(&it, (int)q.frames.size(), T, [&](int j) { return (int64_t)q.frames[j].duration; });
+            it.span = webp_plan_cut(p.get(), it.clip.back());
         }
         it.w = p->width;
         it.h = p->height;
@@ -350,10 +382,16 @@ static void parse_frames_pair(XItem& it, const lp_image_options& opt, const uint
         return;
     }
     if (!memcmp(d, "GIF8", 4)) {
-        std::shared_ptr<GifAnimPlan> p(gif_plan_parse(d, n, 4096, true), gif_plan_free);
+        std::shared_ptr<GifAnimPlan> p(gif_plan_parse(d, n, 4096, T == 0), gif_plan_free);
         if (!p) return;
         int w = 0, h = 0, nf = 0;
         gif_plan_info(p.get(), &w, &h, &nf, nullptr, nullptr);
+        if (T > 0) {
+            if (nf != gif_header_frames(d, n)) return;
+            select_clip(&it, nf, T, [&](int j) { return (int64_t)gif_plan_delay_ms(p.get(), j); });
+            nf = it.clip.back() + 1;
+            gif_plan_cut(p.get(), nf - 1);
+        }
         it.w = w;
         it.h = h;
         it.ch = 4;
@@ -427,7 +465,8 @@ static void parse_pair(lp_xbatch* X, int i, int r, ItemHeaders* c) {
     it.span = n;
     if (!d || n < 16) return;
     if (R.sink == S_FRAMES) {
-        parse_frames_pair(it, opt, d, n, max_side);
+        parse_frames_pair(it, opt, d, n, max_side, X->clip_t);
+        if (X->clip_t && it.kind != K_FALLBACK && it.clip.empty()) select_clip(&it, 1, X->clip_t, [](int) { return (int64_t)0; });  // stills
         return;
     }
     static const uint8_t png_sig[8] = {0x89, 0x50, 0x4E, 0x47, 0x0D, 0x0A, 0x1A, 0x0A};
@@ -522,7 +561,7 @@ static void parse_pair(lp_xbatch* X, int i, int r, ItemHeaders* c) {
             // Transform encodes frame 0 and flushes before its deadline check, so whatever the budget, the file is a
             // still of the composited frame 0 and the device reads only that frame
             if (R.sink != S_WEBP || opt.max_encode_frames != 0 || opt.max_encode_duration_ns != 0) return;
-            if (opt.disable_animated_output) it.span = webp_plan_first_frame(p.get());
+            if (opt.disable_animated_output) it.span = webp_plan_cut(p.get(), 0);
             else if (opt.encode_timeout_ns <= 0) return;
         }
         it.w = p->width;
@@ -758,8 +797,9 @@ static size_t jpeg_batch_cap(const lp_xbatch* X, int ow, int oh) {
 }
 
 // resized frames of a pair: every frame of an animation (of its plan, which DisableAnimatedOutput cuts to frame 0), one
-// of a still
+// of a still; of a clip, its slots in use
 static int out_frames(const XItem& it) {
+    if (!it.clip.empty()) return (int)it.clip.size();
     if (it.kind == K_GIF) return it.gif_frames;
     return it.kind == K_WEBP ? (int)it.webp->frames.size() : 1;
 }
@@ -866,26 +906,36 @@ static FramePackLayout frames_layout(const lp_frame_tensor& t) {
     return o;
 }
 
-// lp_xbatch_decode_frames: every frame of the run into its item's slice of the caller's tensor in one launch.  The run's
-// items travel in a small device table, so items that are not neighbours in the batch land in their own slices, each
-// with its own frame size (a JPEG group's turned or gray items).  A frame larger than the box is refused; one whose
-// decode failed goes to the per-image path.  Nothing comes back to the host.
+// lp_xbatch_decode_frames and lp_xbatch_decode_clips: every frame of the run into its slot's slice of the caller's tensor
+// in one launch.  Item i has `slots` slices from i * slots (one for lp_xbatch_decode_frames, T for a clip); slot t holds
+// its t-th resized frame, and a slot past its frames is an entry of 0 x 0, which the kernel writes as zeros.  The table
+// travels to the device, so items that are not neighbours in the batch land in their own slices, each with its own
+// frame size (a JPEG group's turned or gray items).  A frame larger than the box is refused; an item whose decode failed
+// goes to the per-image path.  Nothing comes back to the host.
 static void frames_sink(lp_xbatch* X, Lane& L, Bump& bump, const std::vector<int>& pairs, const std::vector<int>& st,
                         const uint8_t* d_frames, size_t stride, std::vector<int>* failed) {
     const lp_frame_tensor& T = X->frames;
+    const int slots = std::max(1, X->clip_t);
     std::vector<FramePackItem> tab;
     std::vector<int> packed;
+    size_t at = 0;  // the pair's first frame in the run
     for (size_t q = 0; q < pairs.size(); q++) {
         const int i = pairs[q];  // (one rendition: the pair is the item)
         const XItem& it = X->items[i];
+        const int nf = out_frames(it);
         if (st[q] != LP_OK) {
             failed->push_back(i);
         } else if (it.ow > T.width || it.oh > T.height) {
             X->status[i] = LP_ERR_BUF_TOO_SMALL;
         } else {
-            tab.push_back(FramePackItem{d_frames + q * stride, (uint32_t)(it.ow * it.ch), it.ow, it.oh, it.ch, i});
+            for (int t = 0; t < slots; t++) {
+                const int64_t slice = (int64_t)i * slots + t;
+                tab.push_back(t < nf ? FramePackItem{d_frames + (at + t) * stride, (uint32_t)(it.ow * it.ch), it.ow, it.oh, it.ch, slice}
+                                     : FramePackItem{nullptr, 0, 0, 0, it.ch, slice});
+            }
             packed.push_back(i);
         }
+        at += nf;
     }
     if (tab.empty()) return;
     const size_t mark = bump.used;
@@ -902,10 +952,17 @@ static void frames_sink(lp_xbatch* X, Lane& L, Bump& bump, const std::vector<int
         return;
     }
     L.h2d += tab.size() * sizeof(FramePackItem);
-    for (const FramePackItem& f : tab) {
-        X->status[f.slice] = LP_OK;
-        X->frame_w[f.slice] = f.w;
-        X->frame_h[f.slice] = f.h;
+    for (int i : packed) {
+        const XItem& it = X->items[i];
+        X->status[i] = LP_OK;
+        X->frame_w[i] = it.ow;
+        X->frame_h[i] = it.oh;
+        if (!X->clip_t) continue;
+        X->clip_nframes[i] = it.nframes;
+        for (size_t t = 0; t < it.clip.size(); t++) {
+            X->clip_index[(size_t)i * slots + t] = it.clip[t];
+            X->clip_ms[(size_t)i * slots + t] = it.clip_ms[t];
+        }
     }
 }
 
@@ -1099,7 +1156,8 @@ static void run_webp(lp_xbatch* X, Lane& L, const Task& t) {
     std::vector<const uint8_t*> files((size_t)n);
     std::vector<size_t> flen((size_t)n);
     std::vector<uint64_t> canvas_off((size_t)n), out_off((size_t)n * K);  // out_off[k * K + r]
-    std::vector<int> first((size_t)n + 1, 0);
+    std::vector<int> first((size_t)n + 1, 0);  // canvases
+    std::vector<int> canvas_of;  // a clip's frames: the canvas each is stored at (-1: none)
     size_t scratch = 4096, arena = 0, canvas_bytes = 0, out_bytes = 0;
     for (int k = 0; k < n; k++) {
         const XItem& it = X->items[first_pair(X, idx[k], t.rm[k])];
@@ -1108,11 +1166,15 @@ static void run_webp(lp_xbatch* X, Lane& L, const Task& t) {
         flen[k] = it.span;
         scratch += webp_plan_device_bytes(*plans[k], flen[k]);
         arena += webp_plan_arena_bytes(*plans[k]);
-        const int nf = (int)plans[k]->frames.size();
+        const int nf = out_frames(it);  // (canvases stored: every frame, or a clip's slots)
         first[k + 1] = first[k] + nf;
         canvas_off[k] = canvas_bytes;
         canvas_bytes += (size_t)nf * round_up((size_t)it.w * it.h * it.ch, (size_t)256);
         L.h2d += flen[k];
+        if (!X->clip_t) continue;
+        const size_t j0 = canvas_of.size();
+        canvas_of.resize(j0 + plans[k]->frames.size(), -1);
+        for (size_t t = 0; t < it.clip.size(); t++) canvas_of[j0 + it.clip[t]] = (int)t;
     }
     for (int r = 0; r < K; r++)  // every rendition's resized frames, one area after another
         for (int k = 0; k < n; k++)
@@ -1130,7 +1192,7 @@ static void run_webp(lp_xbatch* X, Lane& L, const Task& t) {
     bool ok = d_scratch && d_canvases && d_out && (!arena || d_arena);
     if (ok)  // (the decode time starts once the files are on the device, as for the other kinds)
         ok = webp_decode_batch(plans.data(), files.data(), flen.data(), n, d_scratch, scratch, d_arena, arena, d_canvases,
-                               canvas_off.data(), st.data(), L.ev[0], L.st) == LP_OK;
+                               canvas_off.data(), st.data(), L.ev[0], L.st, canvas_of.empty() ? nullptr : canvas_of.data()) == LP_OK;
     cudaEventRecord(L.ev[1], L.st);
     for (int r = 0; r < K; r++)
         for (const Run& u : task_runs(X, t, r, 0, n, false))
@@ -1225,7 +1287,8 @@ static void run_gif(lp_xbatch* X, Lane& L, const Task& t) {
     Bump bump{L.dev, L.dev_bytes};
     const size_t canvas_stride = round_up((size_t)g.w * g.h * 4, (size_t)256);
     const size_t out_stride = round_up((size_t)g.ow * g.oh * 4, (size_t)256);
-    std::vector<int> first((size_t)na + 1, 0);
+    std::vector<int> first((size_t)na + 1, 0), cfirst((size_t)na + 1, 0);  // frame jobs, canvases (a clip stores its slots)
+    std::vector<int> canvas_of;  // a clip's frames: the canvas each is stored at (-1: none)
     size_t scratch_bytes = 0;
     std::vector<GifAnimPlan*> plans((size_t)na);
     std::vector<const uint8_t*> files((size_t)na);
@@ -1233,13 +1296,17 @@ static void run_gif(lp_xbatch* X, Lane& L, const Task& t) {
     for (int a = 0; a < na; a++) {
         const XItem& it = X->items[idx[a]];
         first[a + 1] = first[a] + it.gif_frames;
+        cfirst[a + 1] = cfirst[a] + out_frames(it);
         plans[a] = it.gif.get();
         files[a] = X->in[t.idx[a]];
         flen[a] = it.span;
         scratch_bytes += gif_plan_device_bytes(it.gif.get());
         L.h2d += flen[a];
+        if (!X->clip_t) continue;
+        canvas_of.resize((size_t)first[a + 1], -1);
+        for (size_t s = 0; s < it.clip.size(); s++) canvas_of[(size_t)first[a] + it.clip[s]] = cfirst[a] + (int)s;
     }
-    const int nf = first[na];
+    const int nf = cfirst[na];
     uint8_t* d_scratch = bump.take<uint8_t>(scratch_bytes + 4096);
     uint8_t* d_canvases = bump.take<uint8_t>((size_t)nf * canvas_stride + 256);
     uint8_t* d_resized = bump.take<uint8_t>((size_t)nf * out_stride + 256);
@@ -1248,12 +1315,12 @@ static void run_gif(lp_xbatch* X, Lane& L, const Task& t) {
     cudaEventRecord(L.ev[0], L.st);
     if (ok)
         ok = gif_decode_batch(plans.data(), files.data(), flen.data(), na, d_scratch, scratch_bytes + 4096, d_canvases,
-                              canvas_stride, first.data(), st.data(), L.st) == LP_OK;
+                              canvas_stride, first.data(), st.data(), L.st, canvas_of.empty() ? nullptr : canvas_of.data()) == LP_OK;
     cudaEventRecord(L.ev[1], L.st);
     const std::vector<Run> runs = task_runs(X, t, r, 0, na, false);
     for (const Run& u : runs)
-        ok = ok && resize_run(L, X->items[idx[u.k0]], d_canvases + (size_t)first[u.k0] * canvas_stride,
-                              d_resized + (size_t)first[u.k0] * out_stride, first[u.k1] - first[u.k0]);
+        ok = ok && resize_run(L, X->items[idx[u.k0]], d_canvases + (size_t)cfirst[u.k0] * canvas_stride,
+                              d_resized + (size_t)cfirst[u.k0] * out_stride, cfirst[u.k1] - cfirst[u.k0]);
     cudaEventRecord(L.ev[2], L.st);
     if (ok) ok = cudaStreamSynchronize(L.st) == cudaSuccess;
     if (!ok) {
@@ -1265,7 +1332,7 @@ static void run_gif(lp_xbatch* X, Lane& L, const Task& t) {
     lane_time(L, 1, 2, &L.ms_resize);
     std::vector<int> failed;
     for (const Run& u : runs)
-        sink_encode(X, L, bump, L.host, L.host_bytes, t, r, u, st.data(), d_resized + (size_t)first[u.k0] * out_stride, out_stride,
+        sink_encode(X, L, bump, L.host, L.host_bytes, t, r, u, st.data(), d_resized + (size_t)cfirst[u.k0] * out_stride, out_stride,
                     &failed);
     for (int p : failed) push_fallback(X, p);
 }
@@ -1536,9 +1603,9 @@ static size_t item_device_bytes(const lp_xbatch* X, int i, uint32_t rm) {
         }
         case K_WEBP:  // the VP8L arena (at most a quarter of the lane) is shared by the task (reserved by split_by_memory)
             return webp_plan_device_bytes(*it.webp, it.span) +
-                   it.webp->frames.size() * (round_up((size_t)it.w * it.h * it.ch, (size_t)256) + outb) + 8192;
-        case K_GIF:
-            return gif_plan_device_bytes(it.gif.get()) + (size_t)it.gif_frames * ((size_t)it.w * it.h * 4 + outb) + 8192 + gif_enc;
+                   (size_t)out_frames(it) * (round_up((size_t)it.w * it.h * it.ch, (size_t)256) + outb) + 8192;
+        case K_GIF:  // (canvases and resized frames: every frame, or a clip's slots)
+            return gif_plan_device_bytes(it.gif.get()) + (size_t)out_frames(it) * ((size_t)it.w * it.h * 4 + outb) + 8192 + gif_enc;
         case K_FRAME:  // the unpacked frame, its table entry and its output
             return round_up((size_t)it.w * it.h * it.ch, (size_t)256) + sizeof(FrameUnpackItem) + outb + 8192;
         default:
@@ -1570,28 +1637,54 @@ static Rendition make_rendition(const lp_image_options& opt) {
     return R;
 }
 
-// lp_xbatch_decode_frames' per-image route: Transform up to its encoder, whose frame (on the device already, or uploaded
-// by mat_device_view) is packed into slice i on this worker's stream by the grid path's kernel
-static int frames_transform(lp_xbatch* X, int i, const lp_image_options* opt, int max_size) {
+// A framebuffer Transform hands its encoder (on the device already, or uploaded by mat_device_view) packed into slice
+// `slice` of the call's tensor on this worker's stream by the grid path's kernel; item i's size is the frame's
+static int pack_framebuffer(lp_xbatch* X, int i, lilliput::Framebuffer* f, int64_t slice) {
     const lp_frame_tensor& T = X->frames;
-    return lilliput::TransformToFrame(X->in[i], X->in_len[i], opt, max_size, [&](lilliput::Framebuffer* f) -> int {
-        int cols = 0, rows = 0, type = 0;
-        const uint8_t* dev = nullptr;
-        size_t step = 0;
-        int rc = mat_device_view(f->mat, &cols, &rows, &type, &dev, &step);
-        if (rc) return rc;
-        const int ch = opencv_type_channels(type);
-        if (opencv_type_depth(type) != 8 || (ch != 1 && ch != 3 && ch != 4)) return LP_ERR_UNSUPPORTED;  // (framebuffers are 8-bit)
-        if (cols > T.width || rows > T.height) return LP_ERR_BUF_TOO_SMALL;
-        const FramePackItem one{dev, (uint32_t)step, cols, rows, ch, i};
-        cudaStream_t st = thread_stream();
-        rc = frames_pack_launch(nullptr, &one, 1, frames_layout(T), st);
-        if (!rc && cudaStreamSynchronize(st) != cudaSuccess) rc = LP_ERR_CUDA;
-        if (rc) return rc;
-        X->frame_w[i] = cols;
-        X->frame_h[i] = rows;
-        return LP_OK;
-    });
+    int cols = 0, rows = 0, type = 0;
+    const uint8_t* dev = nullptr;
+    size_t step = 0;
+    int rc = mat_device_view(f->mat, &cols, &rows, &type, &dev, &step);
+    if (rc) return rc;
+    const int ch = opencv_type_channels(type);
+    if (opencv_type_depth(type) != 8 || (ch != 1 && ch != 3 && ch != 4)) return LP_ERR_UNSUPPORTED;  // (framebuffers are 8-bit)
+    if (cols > T.width || rows > T.height) return LP_ERR_BUF_TOO_SMALL;
+    const FramePackItem one{dev, (uint32_t)step, cols, rows, ch, slice};
+    cudaStream_t st = thread_stream();
+    rc = frames_pack_launch(nullptr, &one, 1, frames_layout(T), st);
+    if (!rc && cudaStreamSynchronize(st) != cudaSuccess) rc = LP_ERR_CUDA;
+    if (rc) return rc;
+    X->frame_w[i] = cols;
+    X->frame_h[i] = rows;
+    return LP_OK;
+}
+
+// lp_xbatch_decode_frames' per-image route: Transform up to its encoder, whose frame goes to slice i
+static int frames_transform(lp_xbatch* X, int i, const lp_image_options* opt, int max_size) {
+    return lilliput::TransformToFrame(X->in[i], X->in_len[i], opt, max_size,
+                                      [&](lilliput::Framebuffer* f) -> int { return pack_framebuffer(X, i, f, i); });
+}
+
+// lp_xbatch_decode_clips' per-image route: Transform with every selected frame packed into its slot's slice; the slots
+// the stream ended before (the last ones) are zeroed
+static int clips_transform(lp_xbatch* X, int i, const lp_image_options* opt, int max_size) {
+    const int T = X->clip_t;
+    int filled = 0;
+    int rc = lilliput::TransformToClip(
+        X->in[i], X->in_len[i], opt, max_size, T,
+        [&](lilliput::Framebuffer* f, int t) -> int {
+            filled = t + 1;
+            return pack_framebuffer(X, i, f, (int64_t)i * T + t);
+        },
+        &X->clip_nframes[i], X->clip_index + (size_t)i * T, X->clip_ms + (size_t)i * T);
+    if (rc || filled == T) return rc;
+    const lp_frame_tensor& F = X->frames;
+    const size_t slice = (size_t)F.height * F.width * F.channels * frames_dtype_bytes(F.dtype);
+    cudaStream_t st = thread_stream();
+    if (cudaMemsetAsync((uint8_t*)F.data + ((size_t)i * T + filled) * slice, 0, (size_t)(T - filled) * slice, st) != cudaSuccess ||
+        cudaStreamSynchronize(st) != cudaSuccess)
+        return LP_ERR_CUDA;
+    return LP_OK;
 }
 
 // lp_xbatch_encode_frames' per-image route: Transform with a decoder that answers as a PNG of the frame would, whose
@@ -1808,7 +1901,7 @@ static int xbatch_call(lp_xbatch* X, const uint8_t* const* in, const size_t* in_
             const int p = fb[q], i = p / k;
             size_t len = 0;
             if (X->rend[p % k].sink == S_FRAMES) {
-                status[p] = frames_transform(X, i, &opts[p % k], max_size);
+                status[p] = X->clip_t ? clips_transform(X, i, &opts[p % k], max_size) : frames_transform(X, i, &opts[p % k], max_size);
             } else if (X->src_w) {
                 status[p] = transform_from_frame(X, i, &opts[p % k], max_size, out[p], &len);
                 out_len[p] = status[p] == LP_OK ? len : 0;
@@ -1895,13 +1988,12 @@ static int check_frame_tensor(const lp_xbatch* X, const lp_frame_tensor* t, int 
     return LP_OK;
 }
 
-extern "C" int lp_xbatch_decode_frames(lp_xbatch* X, const uint8_t* const* in, const size_t* in_len, int n,
-                                       const lp_image_options* opt, const lp_frame_tensor* dst, int* width, int* height,
-                                       int* status) {
-    if (!X || n < 0 || !opt || !dst || (n > 0 && (!in || !in_len || !width || !height || !status))) return LP_ERR_BAD_ARGUMENT;
-    size_t slice = 0;
-    if (check_frame_tensor(X, dst, n, &slice)) return LP_ERR_BAD_ARGUMENT;
-    const lp_frame_tensor T = *dst;
+// lp_xbatch_decode_frames (X->clip_t 0: one slice per item) and lp_xbatch_decode_clips (clip_t slices per item, its
+// outputs set up by the caller): the call over a checked tensor whose slices are `slice` bytes, then the slices of the
+// items that failed zeroed, as are their sizes
+static int decode_to_tensor(lp_xbatch* X, const uint8_t* const* in, const size_t* in_len, int n, const lp_image_options* opt,
+                            const lp_frame_tensor& T, size_t slice, int* width, int* height, int* status) {
+    const size_t per = (size_t)std::max(1, X->clip_t) * slice;  // an item's slices
     X->frames = T;
     X->frame_w = width;
     X->frame_h = height;
@@ -1911,7 +2003,6 @@ extern "C" int lp_xbatch_decode_frames(lp_xbatch* X, const uint8_t* const* in, c
     std::vector<uint8_t*> out((size_t)n, nullptr);  // (no files: every output of the call is in the tensor)
     std::vector<size_t> out_len((size_t)n, 0);
     int rc = xbatch_call(X, in, in_len, n, opt, &R, 1, out.data(), 0, out_len.data(), status);
-    // the slices of the items that failed: zero, as is their size
     DeviceGuard g(X->device);
     cudaStream_t st = X->lanes[0].st;
     for (int i = 0; i < n && !rc;) {
@@ -1921,11 +2012,54 @@ extern "C" int lp_xbatch_decode_frames(lp_xbatch* X, const uint8_t* const* in, c
         }
         int e = i;
         for (; e < n && status[e] != LP_OK; e++) width[e] = height[e] = 0;
-        if (cudaMemsetAsync((uint8_t*)T.data + (size_t)i * slice, 0, (size_t)(e - i) * slice, st) != cudaSuccess) rc = LP_ERR_CUDA;
+        if (cudaMemsetAsync((uint8_t*)T.data + (size_t)i * per, 0, (size_t)(e - i) * per, st) != cudaSuccess) rc = LP_ERR_CUDA;
         i = e;
     }
     if (!rc && cudaStreamSynchronize(st) != cudaSuccess) rc = LP_ERR_CUDA;
     X->frame_w = X->frame_h = nullptr;
+    return rc;
+}
+
+extern "C" int lp_xbatch_decode_frames(lp_xbatch* X, const uint8_t* const* in, const size_t* in_len, int n,
+                                       const lp_image_options* opt, const lp_frame_tensor* dst, int* width, int* height,
+                                       int* status) {
+    if (!X || n < 0 || !opt || !dst || (n > 0 && (!in || !in_len || !width || !height || !status))) return LP_ERR_BAD_ARGUMENT;
+    size_t slice = 0;
+    if (check_frame_tensor(X, dst, n, &slice)) return LP_ERR_BAD_ARGUMENT;
+    return decode_to_tensor(X, in, in_len, n, opt, *dst, slice, width, height, status);
+}
+
+extern "C" int lp_xbatch_decode_clips(lp_xbatch* X, const uint8_t* const* in, const size_t* in_len, int n,
+                                      const lp_image_options* opt, int frames_per_item, const lp_frame_tensor* dst, int* width,
+                                      int* height, int* nframes, int* frame_index, int64_t* start_ms, int* status) {
+    const int T = frames_per_item;
+    if (!X || n < 0 || !opt || !dst || T < 1 || T > LP_XBATCH_MAX_CLIP_FRAMES ||
+        (n > 0 && (!in || !in_len || !width || !height || !nframes || !frame_index || !start_ms || !status)))
+        return LP_ERR_BAD_ARGUMENT;
+    size_t slice = 0;
+    if ((int64_t)n * T > INT_MAX || check_frame_tensor(X, dst, n * T, &slice)) return LP_ERR_BAD_ARGUMENT;
+    const size_t slots = (size_t)n * T;
+    for (int i = 0; i < n; i++) nframes[i] = 0;
+    for (size_t s = 0; s < slots; s++) {
+        frame_index[s] = -1;
+        start_ms[s] = 0;
+    }
+    X->clip_t = T;
+    X->clip_nframes = nframes;
+    X->clip_index = frame_index;
+    X->clip_ms = start_ms;
+    const int rc = decode_to_tensor(X, in, in_len, n, opt, *dst, slice, width, height, status);
+    X->clip_t = 0;
+    X->clip_nframes = X->clip_index = nullptr;
+    X->clip_ms = nullptr;
+    for (int i = 0; i < n && !rc; i++) {  // an item that failed: no frames, and every slot unused
+        if (status[i] == LP_OK) continue;
+        nframes[i] = 0;
+        for (int t = 0; t < T; t++) {
+            frame_index[(size_t)i * T + t] = -1;
+            start_ms[(size_t)i * T + t] = 0;
+        }
+    }
     return rc;
 }
 

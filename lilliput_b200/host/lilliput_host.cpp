@@ -969,6 +969,77 @@ Error TransformToFrame(const uint8_t* in, size_t in_len, const lp_image_options*
     }
 }
 
+// Stands where the encoder stands in Transform for TransformToClip: every frame is counted and its duration summed; a
+// selected one goes to the sink.  The frame after which no slot is left completes the output; an end of stream completes
+// it too once a frame has arrived, and is LP_ERR_EOF before any (as FrameEncoder answers).
+class ClipEncoder : public Encoder {
+  public:
+    ClipEncoder(int F, int T, const ClipSink& s, int* index, int64_t* ms) : frames(F), slots(T), sink(s), frame_index(index), start_ms(ms) {}
+    Error Encode(Framebuffer* f, const std::map<int, int>&, bool* content, size_t* out_len) override {
+        *content = false;
+        *out_len = 0;
+        if (!f) {
+            if (k == 0) return LP_ERR_EOF;
+            *content = true;
+            return LP_OK;
+        }
+        const int used = std::min(frames, slots);
+        if (next < used && k == (frames <= slots ? next : (int)((int64_t)next * frames / slots))) {
+            Error e = sink(f, next);
+            if (e) return e;
+            frame_index[next] = k;
+            start_ms[next] = ms;
+            next++;
+        }
+        ms += f->duration_ns / 1000000;
+        k++;
+        *content = next >= used;
+        return LP_OK;
+    }
+
+  private:
+    int frames, slots;
+    const ClipSink& sink;
+    int* frame_index;
+    int64_t* start_ms;
+    int k = 0, next = 0;  // frames seen, slots filled
+    int64_t ms = 0;       // durations of the frames seen
+};
+
+Error TransformToClip(const uint8_t* in, size_t in_len, const lp_image_options* c_opt, int max_size, int T, const ClipSink& sink,
+                      int* nframes, int* frame_index, int64_t* start_ms) {
+    *nframes = 0;
+    for (int t = 0; t < T; t++) {
+        frame_index[t] = -1;
+        start_ms[t] = 0;
+    }
+    try {
+        if (!in || !c_opt || T < 1) return LP_ERR_BAD_ARGUMENT;
+        std::unique_ptr<Decoder> d;
+        Error e = NewDecoder(in, in_len, &d);
+        if (e) return e;
+        ImageHeader h;
+        if ((e = d->Header(&h))) return e;
+        // (an APNG's header says 2, but Transform decodes its first frame only)
+        const int F = dynamic_cast<OpenCVDecoder*>(d.get()) ? 1 : std::max(h.numFrames, 0);
+        ImageOptions opt = fromC(c_opt);
+        opt.MaxEncodeFrames = 0;
+        opt.MaxEncodeDuration_ns = 0;
+        opt.DisableAnimatedOutput = false;
+        opt.EncodeTimeout_ns = 1000000000000000000LL;  // (INT64_MAX would overflow Transform's now() + timeout)
+        ClipEncoder enc(F, T, sink, frame_index, start_ms);
+        size_t n = 0;
+        uint8_t none = 0;
+        e = thread_ops(max_size)->Transform(d.get(), opt, &none, 0, &n, &enc);
+        if (!e) *nframes = F;
+        return e;
+    } catch (const std::bad_alloc&) {
+        return LP_ERR_BUF_TOO_SMALL;
+    } catch (...) {
+        return LP_ERR_BAD_ARGUMENT;
+    }
+}
+
 // A decoder of one w x h frame of 3 (BGR) or 4 (BGRA) channels whose pixels `fill` writes, answering as OpenCVDecoder
 // answers for an 8-bit PNG of colour type 2 or 6 without ancillary chunks: orientation 1, one frame, no ICC profile, no
 // cICP, no GIF handle

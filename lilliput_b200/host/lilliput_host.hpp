@@ -195,6 +195,17 @@ class ImageOps {  // ref ops.go:67-150
 using FrameSink = std::function<Error(Framebuffer*)>;
 Error TransformToFrame(const uint8_t* in, size_t in_len, const lp_image_options* opt, int max_size, const FrameSink& sink);
 
+// Every frame Transform hands its encoder, offered in order, with clip slots given to a chosen few: lp_transform(in, opt)
+// with MaxEncodeFrames, MaxEncodeDuration and DisableAnimatedOutput off, no deadline, and a ClipEncoder in place of the
+// encoder.  F is the frame count the decoder's Header() reports (1 for every source the OpenCV decoder takes); slot s
+// of T holds frame s while F <= T, otherwise frame floor(s * F / T), and sink(frame, s) receives it (8-bit gray, BGR or
+// BGRA).  Transform stops after the last selected frame (the encoder answers with content), or at the end of the
+// stream.  *nframes = F; frame_index[s] and start_ms[s] (T entries each): the frame of slot s and the sum of the
+// durations (ms) of the frames before it, or -1 and 0 for a slot never filled.  Returns Transform's status.
+using ClipSink = std::function<Error(Framebuffer*, int slot)>;
+Error TransformToClip(const uint8_t* in, size_t in_len, const lp_image_options* opt, int max_size, int T, const ClipSink& sink,
+                      int* nframes, int* frame_index, int64_t* start_ms);
+
 // The mirror of TransformToFrame: lp_transform of an 8-bit PNG of a w x h frame of `channels` (3: BGR, 4: BGRA) into dst.
 // Transform runs with a FrameDecoder, which answers every Decoder call as OpenCVDecoder answers for such a PNG; its
 // DecodeTo sizes the framebuffer (resizeMat) and then calls fill, which writes the frame's pixels into it.
