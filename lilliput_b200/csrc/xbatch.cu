@@ -4,11 +4,12 @@
 //
 // Renditions (lp_xbatch_transform_renditions): k sets of options, each a Rendition record, and n * k (item, rendition)
 // pairs, each with lp_transform(in[i], opts[r])'s status and bytes; lp_xbatch_transform is k = 1.  A file's container
-// and header are parsed once; the gates below run per pair and give each item the mask of renditions it takes on the
-// grid.  A file is uploaded and decoded once for all of them: PNG and WebP stills resize each decoded frame window into
-// every rendition, JPEG groups with several renditions decode the bounding box of their crops through one resize-only
-// lp_batch context that resizes each chunk into every rendition's geometry, and each rendition's frames then go through
-// its own sink.  Animations (GIF, animated WebP) run each rendition as a task of its own.
+// and header are parsed once (ItemHeaders); one gate function per source format then runs per pair, for every sink, and
+// gives each item the mask of renditions it takes on the grid.  A file is uploaded and decoded once for all of them:
+// PNG and WebP stills resize each decoded frame window into every rendition, JPEG groups with several renditions decode
+// the bounding box of their crops through one resize-only lp_batch context that resizes each chunk into every
+// rendition's geometry, and each rendition's frames then go through its own sink.  Animations (GIF, animated WebP) run
+// each rendition as a task of its own.
 //
 // Per-item semantics are those of lp_transform (= lilliput's NewDecoder + ImageOps.Transform,
 // ref lilliput.go:129-164, ops.go:352-444).  What differs is the schedule:
@@ -45,12 +46,12 @@
 //      animation's plan cut after its last selected frame and only the selected frames' canvases stored).  Whatever the decoder kind, a task's decoded frames go through one run walk
 //      (task_runs: adjacent items that take a rendition and share a geometry), one resize launch per run, and one sink
 //      entry (sink_encode) per run of resized frames;
-//   3. anything the grid path does not cover (gray or over-budget multi-scan JPEGs, gray PNGs, EXIF-rotated sources,
-//      SDR-cICP PNGs to PNG (Transform re-attaches the chunk), lossless WebP output of JPEG and WebP sources, PNG
-//      output of animations, GIF output from other formats, animations under MaxEncodeFrames or MaxEncodeDuration,
-//      one-frame GIFs to WebP with no time to encode ...) and any item whose grid stage fails goes through lp_transform
-//      on a worker thread -- still this library's device kernels, one image per call -- so the status and bytes of
-//      EVERY item are what lp_transform would have returned.
+//   3. anything the grid path does not cover (over-budget multi-scan JPEGs, gray JPEGs and EXIF-rotated sources to
+//      files, gray PNGs, SDR-cICP PNGs to PNG (Transform re-attaches the chunk), lossless WebP output of JPEG and WebP
+//      sources, PNG output of animations, GIF output from other formats, animations under MaxEncodeFrames or
+//      MaxEncodeDuration, one-frame GIFs to WebP with no time to encode ...) and any item whose grid stage fails goes
+//      through lp_transform on a worker thread -- still this library's device kernels, one image per call -- so the
+//      status and bytes of EVERY item are what lp_transform would have returned.
 // Two worker lanes, each with half of the device arena and its own stream, process chunks of groups
 // concurrently, so one lane's PCIe copies and host-side container work overlap the other lane's kernels.
 // Nothing is exchanged between images, lanes or GPUs.
@@ -245,8 +246,10 @@ static bool plan_geometry(const lp_image_options& o, XItem* it) {
     return false;
 }
 
-// The profile WebpEncoder::Create hands to the WebP writer: what the decoder's ICC() read into its 32 KiB buffer
-// (ICCProfileBufferSize, ref lilliput.go:15; n <= 0: none), kept only when iccHeaderIsSane
+constexpr size_t kIccBufferBytes = 32768;  // ICCProfileBufferSize (ref lilliput.go:15)
+
+// The profile WebpEncoder::Create hands to the WebP writer: what the decoder's ICC() read into its buffer (n <= 0:
+// none), kept only when iccHeaderIsSane
 static void keep_icc(XItem* it, const uint8_t* icc, long n) {
     if (n > 0 && lilliput::iccHeaderIsSane(icc, (size_t)n)) it->icc.assign(icc, icc + n);
 }
@@ -274,19 +277,19 @@ static std::shared_ptr<const PngHeader> png_grid_header(const uint8_t* d, size_t
     return h;
 }
 
-// An item's container and header parse, shared by its renditions: each runs at most once per item, and a refusal is
-// remembered as well (-1: not parsed yet, 0: refused, 1: usable)
+// What an item's file is, parsed once for all its renditions when the first one needs it (-1: not parsed yet, 0: the
+// grid cannot decode it, 1: it can)
 struct ItemHeaders {
-    int jpeg = -1;
+    int jpeg = -1;  // a baseline or multi-scan header
     JpegHeader jh;
-    bool jpeg_multiscan = false;
+    int jpeg_budget = -1;  // multi-scan: the scans parse and stay within the serial decoder's budget (walked lazily)
     int png = -1;
     std::shared_ptr<const PngHeader> ph;
     bool png_cicp = false;
     uint8_t cicp[4];  // primaries, transfer, matrix, full range: the chunk Transform's decoder reports
-    int webp = -1;
+    int webp = -1;  // within max_side, and a still's frame is its canvas
     WebpPlan wp;
-    int gif[2] = {-1, -1};  // without, with DisableAnimatedOutput
+    int gif[2] = {-1, -1};  // the full plan, the first-frame plan
     std::shared_ptr<GifAnimPlan> gp[2];
 };
 
@@ -307,119 +310,176 @@ static void select_clip(XItem* it, int F, int T, D duration_ms) {
     }
 }
 
-// The gates of an item of lp_xbatch_decode_frames: the frame Transform hands its still ".png" encoder, which answers at
-// once (no deadline, frame limit or flush follows it), so only MaxEncodeDuration -- held against a frame's duration
-// before the encode -- and NoResize send an item per image, besides what each decoder's gate refuses.  JPEG: rotated and
-// gray files too (the group's resize-only lp_batch context orients and decodes both; an item whose orientation swaps the
-// axes gets the turned frame's output size).  PNG: RGB / RGBA of 8 or 16 bits, HDR tone-mapped; an SDR cICP changes no
-// pixel and is written nowhere.  WebP: stills, and animations cut to frame 0.  GIF: the first-frame plan.
-// T > 0 (lp_xbatch_decode_clips, T slots): the same gates but MaxEncodeDuration, which the clip ignores.  An animation
-// takes its full plan, whose frame count is F (a GIF's only when it is the count GifDecoder's header walk gives, so both
-// routes agree on it), and is cut after the last selected frame: nothing behind it is uploaded or decoded.
-static void parse_frames_pair(XItem& it, const lp_image_options& opt, const uint8_t* d, size_t n, int max_side, int T) {
-    if (T == 0 && opt.max_encode_duration_ns != 0) return;
-    static const uint8_t png_sig[8] = {0x89, 0x50, 0x4E, 0x47, 0x0D, 0x0A, 0x1A, 0x0A};
-    if (d[0] == 0xFF && d[1] == 0xD8) {
-        JpegHeader h;
-        if (jpeg_parse_header(d, n, &h) != LP_OK || (!h.supported && !h.multiscan)) return;
-        if ((h.ncomp != 3 && h.ncomp != 1) || h.width > max_side || h.height > max_side) return;
-        if (!h.supported && !multiscan_in_budget(d, n, h)) return;
-        it.jpeg_multiscan = !h.supported;
-        it.w = h.width;
-        it.h = h.height;
-        it.ch = h.ncomp;
-        it.jpeg_sampling = 0;
-        for (int q = 0; q < h.ncomp; q++) it.jpeg_sampling = (it.jpeg_sampling << 8) | (h.comp[q].h << 4) | h.comp[q].v;
-        if (!plan_geometry(opt, &it)) return;
-        // orientations 5..8: the requested size is the header's turned only under NormalizeOrientation, and Fit works on
-        // the turned frame (ops.go:449-470, as lp_batch sizes its class 2)
-        if (h.orientation >= 5 && h.orientation <= 8 && opt.resize_method == LP_OPS_FIT) {
-            const bool turn = opt.normalize_orientation != 0;
-            lilliput::calculateExpectedSize(turn ? h.height : h.width, turn ? h.width : h.height, opt.width, opt.height, &it.ow, &it.oh);
-        }
-        it.kind = K_JPEG;
-        return;
-    }
-    if (!memcmp(d, png_sig, 8)) {
-        std::shared_ptr<const PngHeader> ph = png_grid_header(d, n, max_side);
-        if (!ph) return;
-        uint8_t cicp[4];
-        if (png_extract_cicp(d, n, cicp)) {
-            it.hdr = cicp[1] == 16 || cicp[1] == 18;
-            it.transfer = cicp[1];
-            it.primaries = cicp[0];
-        }
-        it.w = ph->width;
-        it.h = ph->height;
-        it.ch = ph->out_channels;
-        if (!plan_geometry(opt, &it)) return;
-        it.png = std::move(ph);
-        it.kind = K_PNG;
-        return;
-    }
-    if (!memcmp(d, "RIFF", 4) && !memcmp(d + 8, "WEBP", 4)) {
-        std::unique_ptr<WebpPlan> p(new WebpPlan);
-        if (!webp_plan_parse(d, n, p.get()) || p->width > max_side || p->height > max_side) return;
-        WebpFramePlan& f0 = p->frames[0];
-        it.webp_animation = p->frames.size() > 1;
-        if (!it.webp_animation) {  // Transform does not composite a still: it resizes the decoded frame, which must be the canvas
-            if (f0.x || f0.y || f0.width != p->width || f0.height != p->height) return;
-            f0.blend = 1;
-            f0.dispose = 0;
-        } else if (T == 0) {
-            it.span = webp_plan_cut(p.get(), 0);
-        } else {
-            const WebpPlan& q = *p;
-            select_clip(&it, (int)q.frames.size(), T, [&](int j) { return (int64_t)q.frames[j].duration; });
-            it.span = webp_plan_cut(p.get(), it.clip.back());
-        }
-        it.w = p->width;
-        it.h = p->height;
-        it.ch = p->channels;
-        if (!plan_geometry(opt, &it)) return;
-        it.webp = std::move(p);
-        it.kind = K_WEBP;
-        return;
-    }
-    if (!memcmp(d, "GIF8", 4)) {
-        std::shared_ptr<GifAnimPlan> p(gif_plan_parse(d, n, 4096, T == 0), gif_plan_free);
-        if (!p) return;
-        int w = 0, h = 0, nf = 0;
-        gif_plan_info(p.get(), &w, &h, &nf, nullptr, nullptr);
-        if (T > 0) {
-            if (nf != gif_header_frames(d, n)) return;
-            select_clip(&it, nf, T, [&](int j) { return (int64_t)gif_plan_delay_ms(p.get(), j); });
-            nf = it.clip.back() + 1;
-            gif_plan_cut(p.get(), nf - 1);
-        }
-        it.w = w;
-        it.h = h;
-        it.ch = 4;
-        it.span = gif_plan_file_bytes(p.get());
-        if (w > max_side || h > max_side || !plan_geometry(opt, &it)) return;
-        it.gif = std::move(p);
-        it.gif_frames = nf;
-        it.kind = K_GIF;
-    }
+// A still written to WebP: Transform checks its deadline after the frame (a zero budget fails with ErrEncodeTimeout),
+// MaxEncodeFrames == 1 asks the decoder to skip to the end and a negative MaxEncodeDuration is exceeded at once (no
+// still decoder can skip: ErrSkipNotSupported).  The per-image path decides these after the frame.
+static bool webp_decides_after_frame(const lp_image_options& o) {
+    return o.encode_timeout_ns <= 0 || o.max_encode_frames == 1 || o.max_encode_duration_ns < 0;
 }
 
-// The option gates of a PNG still past its header gates (8-bit or 16-bit RGB / RGBA, no eXIf turn, no SDR cICP to PNG),
-// which a tensor item of lp_xbatch_encode_frames takes as a PNG with a profile.  GIF output needs a GIF source: per image
-// (ErrGifEncoderNeedsDecoder).  To WebP, PNGs with a profile stay per image, where they went before they could carry
-// it, under the options whose result the per-image path decides after the frame: a zero encode budget (the deadline
-// check, as for WebP stills), MaxEncodeFrames == 1 and a negative MaxEncodeDuration (the skip to the end a PNG decoder
-// refuses, as a JPEG's does).  To lossless output every PNG follows that rule.
-static bool png_option_gates(const Rendition& R, bool icc) {
+// The gates below serve every sink.  S_FRAMES (lp_xbatch_decode_frames and _clips) is the frame Transform hands its still
+// ".png" encoder, which answers at once: no deadline, frame limit or flush follows it, so only the decoders' gates apply.
+
+// JPEG: to JPEG, lossy WebP and PNG, and into the tensor.  The file sinks take three-component upright files; the tensor
+// also gray and rotated ones (the group's resize-only lp_batch context orients and decodes both).
+static void jpeg_gates(XItem& it, const Rendition& R, const uint8_t* d, size_t n, int max_side, ItemHeaders* c) {
     const lp_image_options& opt = R.opt;
-    if (R.sink == S_GIF) return false;
-    return !(R.sink == S_WEBP && (icc || R.lossless) &&
-             (opt.encode_timeout_ns <= 0 || opt.max_encode_frames == 1 || opt.max_encode_duration_ns < 0));
+    const bool frames = R.sink == S_FRAMES;
+    if (R.sink == S_GIF || (R.sink == S_WEBP && (R.lossless || webp_decides_after_frame(opt)))) return;
+    if (c->jpeg < 0) c->jpeg = jpeg_parse_header(d, n, &c->jh) == LP_OK && (c->jh.supported || c->jh.multiscan);
+    if (!c->jpeg) return;
+    const JpegHeader& h = c->jh;
+    const bool layout = frames ? h.ncomp == 3 || h.ncomp == 1 : h.ncomp == 3 && (h.orientation < 2 || h.orientation > 8);
+    if (!layout || h.width > max_side || h.height > max_side) return;
+    if (!h.supported) {  // multi-scan: damaged scans and files over the serial decoder's budget go per image
+        if (c->jpeg_budget < 0) c->jpeg_budget = multiscan_in_budget(d, n, h);
+        if (!c->jpeg_budget) return;
+    }
+    it.jpeg_multiscan = !h.supported;
+    it.w = h.width;
+    it.h = h.height;
+    it.ch = h.ncomp;
+    it.jpeg_sampling = 0;
+    for (int q = 0; q < h.ncomp; q++) it.jpeg_sampling = (it.jpeg_sampling << 8) | (h.comp[q].h << 4) | h.comp[q].v;
+    if (!plan_geometry(opt, &it)) return;
+    // orientations 5..8: the requested size is the header's turned only under NormalizeOrientation, and Fit works on the
+    // turned frame (ops.go:449-470, as lp_batch sizes its class 2)
+    if (h.orientation >= 5 && h.orientation <= 8 && opt.resize_method == LP_OPS_FIT) {
+        const bool turn = opt.normalize_orientation != 0;
+        lilliput::calculateExpectedSize(turn ? h.height : h.width, turn ? h.width : h.height, opt.width, opt.height, &it.ow, &it.oh);
+    }
+    thread_local std::vector<uint8_t> icc_buf(kIccBufferBytes);
+    if (R.sink == S_WEBP)  // (its APP2 segments concatenated: the item keeps its own copy)
+        keep_icc(&it, icc_buf.data(), opencv_decoder_get_jpeg_icc(const_cast<uint8_t*>(d), n, icc_buf.data(), icc_buf.size()));
+    it.kind = K_JPEG;
+}
+
+// PNG: a colour frame of 8 or 16 bits (png_grid_header), HDR tone-mapped.  An SDR cICP changes no pixel, but Transform
+// re-attaches it to a PNG output (ops.go:306-332): per image.  GIF output needs a GIF source: per image
+// (ErrGifEncoderNeedsDecoder).  To WebP, PNGs with a profile stay per image, where they went before they could carry it,
+// when the WebP encoder decides after the frame; to lossless output every PNG follows that rule.
+static void png_gates(XItem& it, const Rendition& R, const uint8_t* d, size_t n, int max_side, ItemHeaders* c) {
+    if (c->png < 0) {
+        c->ph = png_grid_header(d, n, max_side);
+        c->png = c->ph != nullptr;
+        if (c->png) c->png_cicp = png_extract_cicp(d, n, c->cicp);
+    }
+    if (!c->png) return;
+    if (c->png_cicp) {
+        it.hdr = c->cicp[1] == 16 || c->cicp[1] == 18;
+        if (!it.hdr && R.sink == S_PNG) return;
+        it.transfer = c->cicp[1];
+        it.primaries = c->cicp[0];
+    }
+    const PngHeader& h = *c->ph;
+    it.w = h.width;
+    it.h = h.height;
+    it.ch = h.out_channels;
+    if (!plan_geometry(R.opt, &it)) return;
+    thread_local std::vector<uint8_t> icc_buf(kIccBufferBytes);
+    const int icc_n = R.sink == S_WEBP ? png_extract_icc(d, n, icc_buf.data(), icc_buf.size()) : 0;
+    if (R.sink == S_GIF || (R.sink == S_WEBP && (icc_n > 0 || R.lossless) && webp_decides_after_frame(R.opt))) return;
+    if (R.sink == S_WEBP) keep_icc(&it, icc_buf.data(), icc_n);
+    it.png = c->ph;
+    it.kind = K_PNG;
+}
+
+// WebP: stills to lossy WebP, PNG and the tensor, animations to lossy WebP, cut to frame 0 under DisableAnimatedOutput
+// and for the tensor, or after a clip's last selected frame.  Lossless output of WebP sources: per image.
+static void webp_gates(XItem& it, const Rendition& R, const uint8_t* d, size_t n, int max_side, int T, ItemHeaders* c) {
+    const lp_image_options& opt = R.opt;
+    if (R.sink == S_GIF || R.lossless) return;
+    if (c->webp < 0) {  // damaged containers: per image
+        c->webp = webp_plan_parse(d, n, &c->wp) && c->wp.width <= max_side && c->wp.height <= max_side;
+        // Transform does not composite a still: it resizes the decoded frame, which must then be the canvas
+        if (c->webp && c->wp.frames.size() == 1) {
+            const WebpFramePlan& f0 = c->wp.frames[0];
+            if (f0.x || f0.y || f0.width != c->wp.width || f0.height != c->wp.height) c->webp = 0;
+        }
+    }
+    if (!c->webp) return;
+    std::unique_ptr<WebpPlan> p(new WebpPlan(c->wp));
+    WebpFramePlan& f0 = p->frames[0];
+    it.webp_animation = p->frames.size() > 1;
+    if (!it.webp_animation) {
+        // a still written to WebP with no time to encode: lp_transform's deadline check follows the frame.  Only the
+        // simple lossy stills the grid has always taken keep going there; the others stay with lp_transform
+        const bool simple = !f0.lossless && !f0.has_alph && !p->icc_len && !p->animated && p->channels == 3;
+        if (R.sink == S_WEBP && opt.encode_timeout_ns <= 0 && !simple) return;
+        // to PNG under MaxEncodeDuration: a WebP still's frame carries a duration, which Transform holds against the
+        // limit before it encodes the frame; lp_transform decides
+        if (R.sink == S_PNG && opt.max_encode_duration_ns != 0) return;
+        f0.blend = 1;  // copied onto a canvas of its own size, never disposed
+        f0.dispose = 0;
+    } else if (R.sink == S_FRAMES) {
+        if (T > 0) select_clip(&it, (int)p->frames.size(), T, [&](int j) { return (int64_t)p->frames[j].duration; });
+        it.span = webp_plan_cut(p.get(), T > 0 ? it.clip.back() : 0);
+    } else {
+        // to animated WebP, with the option gates of GIF -> WebP; Transform checks its deadline after every non-final
+        // frame, so a zero budget fails there (ErrEncodeTimeout): per image.  DisableAnimatedOutput: Transform encodes
+        // frame 0 and flushes before its deadline check, so whatever the budget, the file is a still of the composited
+        // frame 0 and the device reads only that frame
+        if (R.sink != S_WEBP || opt.max_encode_frames != 0 || opt.max_encode_duration_ns != 0) return;
+        if (opt.disable_animated_output) it.span = webp_plan_cut(p.get(), 0);
+        else if (opt.encode_timeout_ns <= 0) return;
+    }
+    it.w = p->width;
+    it.h = p->height;
+    it.ch = p->channels;
+    if (!plan_geometry(opt, &it)) return;
+    // (webp_decoder_get_icc reads no profile larger than the buffer)
+    if (R.sink == S_WEBP && p->icc_len <= kIccBufferBytes) keep_icc(&it, d + p->icc_off, (long)p->icc_len);
+    it.webp = std::move(p);
+    it.kind = K_WEBP;
+}
+
+// GIF: to GIF and WebP, and into the tensor.  DisableAnimatedOutput and the tensor take the first-frame plan: Transform
+// encodes frame 0 and flushes before its deadline check, and its decoder reads nothing behind that frame.  A clip takes
+// the full plan, whose frame count must be the one GifDecoder's header walk gives (so both routes agree on F), cut after
+// the last selected frame: nothing behind it is uploaded or decoded.
+static void gif_gates(XItem& it, const Rendition& R, const uint8_t* d, size_t n, int max_side, int T, ItemHeaders* c) {
+    const lp_image_options& opt = R.opt;
+    const bool frames = R.sink == S_FRAMES;
+    const bool first_only = frames ? T == 0 : opt.disable_animated_output != 0;
+    if (!frames) {
+        if ((R.sink != S_WEBP && R.sink != S_GIF) || opt.max_encode_frames != 0 || opt.max_encode_duration_ns != 0) return;
+        // a GIF written with no time to encode fails with ErrEncodeTimeout after its first frame (Transform's deadline):
+        // per image, to GIF and to lossless WebP
+        if (!first_only && (R.sink == S_GIF || R.lossless) && opt.encode_timeout_ns <= 0) return;
+    }
+    if (c->gif[first_only] < 0) {
+        c->gp[first_only].reset(gif_plan_parse(d, n, 4096, first_only), gif_plan_free);
+        c->gif[first_only] = c->gp[first_only] != nullptr;
+    }
+    if (!c->gif[first_only]) return;
+    std::shared_ptr<GifAnimPlan> p = c->gp[first_only];
+    int w = 0, h = 0, nf = 0;
+    gif_plan_info(p.get(), &w, &h, &nf, nullptr, nullptr);
+    if (T > 0) {
+        if (nf != gif_header_frames(d, n)) return;
+        select_clip(&it, nf, T, [&](int j) { return (int64_t)gif_plan_delay_ms(p.get(), j); });
+        nf = it.clip.back() + 1;
+        gif_plan_cut(p.get(), nf - 1);
+        c->gp[0].reset();  // (the cut plan is this pair's alone: another rendition would parse the file again)
+        c->gif[0] = -1;
+    }
+    it.w = w;
+    it.h = h;
+    it.ch = 4;
+    it.span = gif_plan_file_bytes(p.get());
+    // a one-frame file to WebP meets the same deadline check after its frame: with no time to encode, per image
+    if ((nf < 2 && R.sink == S_WEBP && !first_only && opt.encode_timeout_ns <= 0) || w > max_side || h > max_side ||
+        !plan_geometry(opt, &it))
+        return;
+    it.gif = std::move(p);
+    it.gif_frames = nf;
+    it.kind = K_GIF;
 }
 
 // A tensor item of lp_xbatch_encode_frames: its "header" is w x h x C, with no container, so no ICC profile and no cICP,
-// and it takes the gates of an 8-bit RGB / RGBA PNG (png_grid_header's size limit, png_option_gates) with three
-// differences.  Two send items per image where lp_transform fails them and the PNG gates keep an ICC-less PNG on the
-// grid, as they always have:
+// and it takes the gates of an 8-bit RGB / RGBA PNG (png_grid_header's size limit, png_gates) with three differences.
+// Two send items per image where lp_transform fails them and the PNG gates keep an ICC-less PNG on the grid, as they
+// always have:
 //   - the option gates are those of a PNG with a profile: Transform checks a still's deadline and MaxEncodeFrames after
 //     its frame goes to the .webp encoder (which waits for the end of the stream), and fails with ErrEncodeTimeout or
 //     ErrSkipNotSupported;
@@ -430,7 +490,7 @@ static bool png_option_gates(const Rendition& R, bool icc) {
 static void parse_frame_pair(const lp_xbatch* X, int i, XItem& it, const Rendition& R, int max_side) {
     const int w = X->src_w[i], h = X->src_h[i];
     if (w < 1 || h < 1 || w > X->frames.width || h > X->frames.height || w > max_side || h > max_side) return;
-    if (R.opt.max_encode_duration_ns < 0 || !png_option_gates(R, true)) return;
+    if (R.opt.max_encode_duration_ns < 0 || R.sink == S_GIF || (R.sink == S_WEBP && webp_decides_after_frame(R.opt))) return;
     it.w = w;
     it.h = h;
     it.ch = X->frames.channels;
@@ -462,147 +522,18 @@ static void parse_pair(lp_xbatch* X, int i, int r, ItemHeaders* c) {
     }
     const uint8_t* d = X->in[i];
     const size_t n = X->in_len[i];
+    const int T = X->clip_t;
     it.span = n;
     if (!d || n < 16) return;
-    if (R.sink == S_FRAMES) {
-        parse_frames_pair(it, opt, d, n, max_side, X->clip_t);
-        if (X->clip_t && it.kind != K_FALLBACK && it.clip.empty()) select_clip(&it, 1, X->clip_t, [](int) { return (int64_t)0; });  // stills
-        return;
-    }
+    // into the tensor, MaxEncodeDuration is held against a frame's duration before the encode; a clip ignores it
+    if (R.sink == S_FRAMES && T == 0 && opt.max_encode_duration_ns != 0) return;
     static const uint8_t png_sig[8] = {0x89, 0x50, 0x4E, 0x47, 0x0D, 0x0A, 0x1A, 0x0A};
-    thread_local std::vector<uint8_t> icc_buf(32768);
-    if (d[0] == 0xFF && d[1] == 0xD8) {
-        if (R.sink != S_JPEG && R.sink != S_WEBP && R.sink != S_PNG) return;
-        if (R.lossless) return;  // lossless WebP output of JPEG sources: per image
-        // A still to WebP: after its frame Transform checks its deadline (a zero budget fails with ErrEncodeTimeout),
-        // MaxEncodeFrames == 1 asks the decoder to skip to the end (a JPEG cannot: ErrSkipNotSupported), and a negative
-        // MaxEncodeDuration is exceeded at once (the same skip).  Those go per image.
-        if (R.sink == S_WEBP && (opt.encode_timeout_ns <= 0 || opt.max_encode_frames == 1 || opt.max_encode_duration_ns < 0))
-            return;
-        if (c->jpeg < 0) {
-            JpegHeader& h = c->jh;
-            c->jpeg = 0;
-            if (jpeg_parse_header(d, n, &h) != LP_OK || (!h.supported && !h.multiscan)) return;
-            if (h.ncomp != 3) return;
-            if (h.orientation >= 2 && h.orientation <= 8) return;
-            if (h.width > max_side || h.height > max_side) return;
-            if (!h.supported) {  // multi-scan: damaged scans and files over the serial decoder's budget go per image
-                if (!multiscan_in_budget(d, n, h)) return;
-                c->jpeg_multiscan = true;
-            }
-            c->jpeg = 1;
-        }
-        if (!c->jpeg) return;
-        const JpegHeader& h = c->jh;
-        it.jpeg_multiscan = c->jpeg_multiscan;
-        it.w = h.width;
-        it.h = h.height;
-        it.ch = 3;
-        it.jpeg_sampling = 0;
-        for (int q = 0; q < 3; q++) it.jpeg_sampling = (it.jpeg_sampling << 8) | (h.comp[q].h << 4) | h.comp[q].v;
-        if (!plan_geometry(opt, &it)) return;
-        if (R.sink == S_WEBP)  // (its APP2 segments concatenated: the item keeps its own copy)
-            keep_icc(&it, icc_buf.data(), opencv_decoder_get_jpeg_icc(const_cast<uint8_t*>(d), n, icc_buf.data(), icc_buf.size()));
-        it.kind = K_JPEG;
-        return;
-    }
-    if (!memcmp(d, png_sig, 8)) {
-        if (c->png < 0) {
-            c->ph = png_grid_header(d, n, max_side);
-            c->png = c->ph != nullptr;
-            if (c->png) c->png_cicp = png_extract_cicp(d, n, c->cicp);
-        }
-        if (!c->png) return;
-        if (c->png_cicp) {
-            it.hdr = c->cicp[1] == 16 || c->cicp[1] == 18;
-            // an SDR tag changes no pixel, but Transform re-attaches it to a PNG output (ops.go:306-332): per image
-            if (!it.hdr && R.sink == S_PNG) return;
-            it.transfer = c->cicp[1];
-            it.primaries = c->cicp[0];
-        }
-        const PngHeader& h = *c->ph;
-        it.w = h.width;
-        it.h = h.height;
-        it.ch = h.out_channels;
-        if (!plan_geometry(opt, &it)) return;
-        const int icc_n = R.sink == S_WEBP ? png_extract_icc(d, n, icc_buf.data(), icc_buf.size()) : 0;
-        if (!png_option_gates(R, icc_n > 0)) return;
-        if (R.sink == S_WEBP) keep_icc(&it, icc_buf.data(), icc_n);
-        it.png = c->ph;
-        it.kind = K_PNG;
-        return;
-    }
-    if (!memcmp(d, "RIFF", 4) && !memcmp(d + 8, "WEBP", 4)) {
-        if (R.sink == S_GIF || R.lossless) return;  // (lossless WebP output of WebP sources: per image)
-        if (c->webp < 0) {  // damaged containers: per image
-            c->webp = webp_plan_parse(d, n, &c->wp) && c->wp.width <= max_side && c->wp.height <= max_side;
-            // Transform does not composite a still: it resizes the decoded frame, which must then be the canvas
-            if (c->webp && c->wp.frames.size() == 1) {
-                const WebpFramePlan& f0 = c->wp.frames[0];
-                if (f0.x || f0.y || f0.width != c->wp.width || f0.height != c->wp.height) c->webp = 0;
-            }
-        }
-        if (!c->webp) return;
-        std::unique_ptr<WebpPlan> p(new WebpPlan(c->wp));
-        WebpFramePlan& f0 = p->frames[0];
-        if (p->frames.size() == 1) {
-            // a still written to WebP with no time to encode: lp_transform's deadline check follows the frame.  Only the
-            // simple lossy stills the grid has always taken keep going there; the others stay with lp_transform
-            const bool simple = !f0.lossless && !f0.has_alph && !p->icc_len && !p->animated && p->channels == 3;
-            if (R.sink == S_WEBP && opt.encode_timeout_ns <= 0 && !simple) return;
-            // to PNG under MaxEncodeDuration: a WebP still's frame carries a duration, which Transform holds against the
-            // limit before it encodes the frame; lp_transform decides
-            if (R.sink == S_PNG && opt.max_encode_duration_ns != 0) return;
-            f0.blend = 1;  // copied onto a canvas of its own size, never disposed
-            f0.dispose = 0;
-        } else {
-            // animations -> animated WebP, with the option gates of GIF -> WebP; Transform checks its deadline after
-            // every non-final frame, so a zero budget fails there (ErrEncodeTimeout): per image.  DisableAnimatedOutput:
-            // Transform encodes frame 0 and flushes before its deadline check, so whatever the budget, the file is a
-            // still of the composited frame 0 and the device reads only that frame
-            if (R.sink != S_WEBP || opt.max_encode_frames != 0 || opt.max_encode_duration_ns != 0) return;
-            if (opt.disable_animated_output) it.span = webp_plan_cut(p.get(), 0);
-            else if (opt.encode_timeout_ns <= 0) return;
-        }
-        it.w = p->width;
-        it.h = p->height;
-        it.ch = p->channels;
-        if (!plan_geometry(opt, &it)) return;
-        // (webp_decoder_get_icc reads no profile larger than the 32 KiB buffer)
-        if (R.sink == S_WEBP && p->icc_len <= icc_buf.size()) keep_icc(&it, d + p->icc_off, (long)p->icc_len);
-        it.webp_animation = c->wp.frames.size() > 1;
-        it.webp = std::move(p);
-        it.kind = K_WEBP;
-        return;
-    }
-    if (!memcmp(d, "GIF8", 4)) {
-        if ((R.sink != S_WEBP && R.sink != S_GIF) || opt.max_encode_frames != 0 || opt.max_encode_duration_ns != 0) return;
-        // DisableAnimatedOutput: Transform encodes frame 0 and flushes before its deadline check, and its decoder reads
-        // nothing behind that frame.  Otherwise a GIF written with no time to encode fails with ErrEncodeTimeout after
-        // its first frame (Transform's deadline): per image, to GIF and to lossless WebP
-        const bool first_only = opt.disable_animated_output != 0;
-        if (!first_only && (R.sink == S_GIF || R.lossless) && opt.encode_timeout_ns <= 0) return;
-        if (c->gif[first_only] < 0) {
-            c->gp[first_only].reset(gif_plan_parse(d, n, 4096, first_only), gif_plan_free);
-            c->gif[first_only] = c->gp[first_only] != nullptr;
-        }
-        if (!c->gif[first_only]) return;
-        const std::shared_ptr<GifAnimPlan>& p = c->gp[first_only];
-        int w = 0, h = 0, nf = 0;
-        gif_plan_info(p.get(), &w, &h, &nf, nullptr, nullptr);
-        it.w = w;
-        it.h = h;
-        it.ch = 4;
-        it.span = gif_plan_file_bytes(p.get());
-        // a one-frame file to WebP meets the same deadline check after its frame: with no time to encode, per image
-        if ((nf < 2 && R.sink == S_WEBP && !first_only && opt.encode_timeout_ns <= 0) || w > max_side || h > max_side ||
-            !plan_geometry(opt, &it))
-            return;
-        it.gif = p;
-        it.gif_frames = nf;
-        it.kind = K_GIF;
-        return;
-    }
+    if (d[0] == 0xFF && d[1] == 0xD8) jpeg_gates(it, R, d, n, max_side, c);
+    else if (!memcmp(d, png_sig, 8)) png_gates(it, R, d, n, max_side, c);
+    else if (!memcmp(d, "RIFF", 4) && !memcmp(d + 8, "WEBP", 4)) webp_gates(it, R, d, n, max_side, T, c);
+    else if (!memcmp(d, "GIF8", 4)) gif_gates(it, R, d, n, max_side, T, c);
+    if (R.sink == S_FRAMES && T > 0 && it.kind != K_FALLBACK && it.clip.empty())  // a still: one slot
+        select_clip(&it, 1, T, [](int) { return (int64_t)0; });
 }
 
 // every rendition of item i; the pairs that take the grid set their bits in X->mask[i]
@@ -1637,6 +1568,15 @@ static Rendition make_rendition(const lp_image_options& opt) {
     return R;
 }
 
+// the one rendition of lp_xbatch_decode_frames and lp_xbatch_decode_clips: pixels into the caller's tensor
+// (none of the file sinks' fields: a ".webp" at quality 101 must not read as lossless output)
+static Rendition frames_rendition(const lp_image_options& opt) {
+    Rendition R;
+    R.opt = opt;
+    R.sink = S_FRAMES;
+    return R;
+}
+
 // A framebuffer Transform hands its encoder (on the device already, or uploaded by mat_device_view) packed into slice
 // `slice` of the call's tensor on this worker's stream by the grid path's kernel; item i's size is the frame's
 static int pack_framebuffer(lp_xbatch* X, int i, lilliput::Framebuffer* f, int64_t slice) {
@@ -1998,8 +1938,7 @@ static int decode_to_tensor(lp_xbatch* X, const uint8_t* const* in, const size_t
     X->frame_w = width;
     X->frame_h = height;
     for (int i = 0; i < n; i++) width[i] = height[i] = 0;
-    Rendition R = make_rendition(*opt);
-    R.sink = S_FRAMES;
+    Rendition R = frames_rendition(*opt);
     std::vector<uint8_t*> out((size_t)n, nullptr);  // (no files: every output of the call is in the tensor)
     std::vector<size_t> out_len((size_t)n, 0);
     int rc = xbatch_call(X, in, in_len, n, opt, &R, 1, out.data(), 0, out_len.data(), status);
