@@ -336,6 +336,30 @@ int lp_xbatch_encode_frames(lp_xbatch* x, const lp_frame_tensor* src, int n, con
                             const lp_image_options* opt, uint8_t* const* out, size_t out_cap, size_t* out_len,
                             int* status);
 
+/* Animations from clips: slice i * T + t of src (T = frames_per_item; the lp_frame_tensor of lp_xbatch_decode_clips,
+ * n * T slices; with nchw an N x T x C x H x W tensor) holds frame t of item i at its top-left, width[i] x height[i]
+ * (every frame of an item has that size).  Frames 0 .. nframes[i] - 1 are used; later slots are not read.  Frames are
+ * converted as lp_xbatch_encode_frames converts them.
+ *   - nframes[i] == 1: the item is the lp_xbatch_encode_frames item of slice i * T (same status and bytes); its
+ *     duration is ignored
+ *   - nframes[i] >= 2: status and bytes are those of lp_transform(A_i, opt, out[i], out_cap, ..., max_size), where A_i
+ *     is an animated WebP of width[i] x height[i]: a VP8X chunk with the animation flag (and the alpha flag exactly
+ *     when channels == 4), an ANIM chunk with background 0xFFFFFFFF and loop_count, then nframes[i] ANMF chunks, each
+ *     the whole canvas at 0, 0 with no blending and no disposal, lasting duration_ms[i * T + t], whose image is a
+ *     lossless VP8L frame that keeps every value (colour under alpha 0 included)
+ *   - nframes[i] outside 1..T, width[i] or height[i] outside 1..box, or (nframes[i] >= 2) a duration of a used frame
+ *     outside 0..0xFFFFFF: that item gets LP_ERR_BAD_ARGUMENT and out_len 0; the others go on
+ * The tensor's contents must be complete before the call; the call only reads the tensor.  LP_ERR_BAD_ARGUMENT, with
+ * nothing written, for: the tensor checks of lp_xbatch_decode_frames with n * T slices; T outside
+ * 1..LP_XBATCH_MAX_CLIP_FRAMES; loop_count outside 0..65535; n < 0; a null opt / nframes / width / height /
+ * duration_ms / out / out_len / status with n > 0.
+ * Stats: grid_items / fallback_items count items; ms_decode is the unpack; h2d_bytes carries no pixels (the item table
+ * only); d2h_bytes is the files.  lp_xbatch_encode_frames is this call with T = 1. */
+int lp_xbatch_encode_clips(lp_xbatch* x, const lp_frame_tensor* src, int n, int frames_per_item, const int* nframes,
+                           const int* width, const int* height, const int* duration_ms, int loop_count,
+                           const lp_image_options* opt, uint8_t* const* out, size_t out_cap, size_t* out_len,
+                           int* status);
+
 /* ---- the same call over several GPUs of one node (SURVEY 8(e): shard by image index, no collective) ----
  * One lp_xbatch per device behind one call: the batch is cut into contiguous blocks balanced by compressed bytes,
  * every block runs on its own GPU from its own host thread, results land in the caller's arrays by index. */

@@ -525,6 +525,10 @@ class XBatch:
         l.lp_xbatch_encode_frames.restype = C.c_int
         l.lp_xbatch_encode_frames.argtypes = [C.c_void_p, C.POINTER(_FrameTensor), C.c_int, C.c_void_p, C.c_void_p,
                                               C.POINTER(_ImageOptions), C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p]
+        l.lp_xbatch_encode_clips.restype = C.c_int
+        l.lp_xbatch_encode_clips.argtypes = [C.c_void_p, C.POINTER(_FrameTensor), C.c_int, C.c_int, C.c_void_p, C.c_void_p,
+                                             C.c_void_p, C.c_void_p, C.c_int, C.POINTER(_ImageOptions), C.c_void_p, C.c_size_t,
+                                             C.c_void_p, C.c_void_p]
         cfg = _XBatchConfig(device, arena_bytes, host_threads, max_size)
         self.h = l.lp_xbatch_create(C.byref(cfg))
         if not self.h:
@@ -615,6 +619,32 @@ class XBatch:
         status = (C.c_int * max(n, 1))()
         copt = opt._c()
         rc = self.lib.l.lp_xbatch_encode_frames(self.h, C.byref(t), n, ws, hs, C.byref(copt), out_ptrs, out_cap, out_lens, status)
+        if rc:
+            raise LilliputError(rc)
+        return [out[i, : out_lens[i]].tobytes() for i in range(n)], list(status[:n])
+
+    def encode_clips(self, data_ptr: int, bytes: int, frames_per_item: int, nframes, widths, heights, durations_ms,
+                     opt: ImageOptions, height: int, width: int, loop_count: int = 0, channels: int = 3, nchw: bool = False,
+                     rgb: bool = True, dtype: str = "u8", scale=None, bias=None, out_cap: int = 1 << 20):
+        """lp_xbatch_encode_clips: animations from clips of the device tensor at data_ptr (laid out as for decode_clips,
+        N * T slices): item i's frame t is the top-left widths[i] x heights[i] of slice i * T + t, for t < nframes[i],
+        lasting durations_ms[i * T + t].  An item of several frames equals lp_transform of an animated WebP of lossless
+        full-canvas frames with those durations and loop_count; one of a single frame is an encode_frames item.
+        Returns (outs, status)."""
+        n, T = len(widths), frames_per_item
+        t = _FrameTensor(data_ptr, bytes, height, width, channels, int(bool(nchw)), int(bool(rgb)),
+                         FRAME_DTYPES.get(dtype, -1) if isinstance(dtype, str) else int(dtype),
+                         (C.c_float * 4)(*(list(scale) if scale is not None else [1.0] * 4)),
+                         (C.c_float * 4)(*(list(bias) if bias is not None else [0.0] * 4)))
+        nf, ws, hs = (C.c_int * max(n, 1))(*nframes), (C.c_int * max(n, 1))(*widths), (C.c_int * max(n, 1))(*heights)
+        ms = (C.c_int * max(n * max(T, 0), 1))(*durations_ms)
+        out = np.empty((max(n, 1), out_cap), dtype=np.uint8)
+        out_ptrs = (C.c_void_p * max(n, 1))(*[out[i].ctypes.data for i in range(n)])
+        out_lens = (C.c_size_t * max(n, 1))()
+        status = (C.c_int * max(n, 1))()
+        copt = opt._c()
+        rc = self.lib.l.lp_xbatch_encode_clips(self.h, C.byref(t), n, T, nf, ws, hs, ms, loop_count, C.byref(copt), out_ptrs,
+                                               out_cap, out_lens, status)
         if rc:
             raise LilliputError(rc)
         return [out[i, : out_lens[i]].tobytes() for i in range(n)], list(status[:n])

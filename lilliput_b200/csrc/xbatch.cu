@@ -31,7 +31,8 @@
 //        frames -> lp_xbatch_encode_frames: no file but slice i of a caller's device tensor, w[i] x h[i] at its top-left,
 //                 unpacked into u8 BGR / BGRA frames by one launch over the task (frames_pack.cu); the item passes the
 //                 gates of an 8-bit RGB / RGBA PNG (parse_frame_pair), and under NoResize its frame goes to the sink
-//                 unresized
+//                 unresized.  lp_xbatch_encode_clips: T slices per item, a clip of nframes >= 2 passing the gates of its
+//                 animated WebP A_i (clip_gates); the frames its output reads are unpacked as an animation's canvases
 //        DisableAnimatedOutput (GIF and animated WebP to WebP, GIF to GIF): Transform stops after frame 0, so the plan
 //                 stops there too (gif_plan_parse's first-frame walk, webp_plan_cut); only the file up to the
 //                 end of frame 0's image data is uploaded, the same kernels run over one frame per file, and the sink
@@ -126,6 +127,7 @@ struct XItem {
     int nframes = 0;                  // lp_xbatch_decode_clips: F, the frame count the decoder's header reports,
     std::vector<int> clip;            // the frames of the slots in use (the only canvases stored, the plan cut after the last)
     std::vector<int64_t> clip_ms;     // and each one's start (ms)
+    int src_frames = 1;  // K_FRAME: the item's frames the output reads, slices i * T .. (nframes to an animated .webp)
     std::vector<uint8_t> icc;  // WebP sink: the source's profile the WebP writer carries (empty: none, or not sane)
 };
 
@@ -192,6 +194,10 @@ struct lp_xbatch {
     int64_t* clip_ms = nullptr;
     const int* src_w = nullptr;  // lp_xbatch_encode_frames: the items are slices of `frames`, of these sizes (no files)
     const int* src_h = nullptr;
+    int src_t = 1;  // lp_xbatch_encode_clips: T slices per item (1 for lp_xbatch_encode_frames), the frames each item
+    const int* src_nframes = nullptr;  // uses (null: one each), their durations (ms, T per item) and the loop count
+    const int* src_ms = nullptr;
+    int src_loops = 0;
     int k = 1;              // renditions
     std::vector<Rendition> rend;
     std::vector<XItem> items;   // pairs: item i, rendition r at i * k + r
@@ -487,10 +493,63 @@ static void gif_gates(XItem& it, const Rendition& R, const uint8_t* d, size_t n,
 //     which it refuses (ErrSkipNotSupported).
 // The third is NoResize: Transform hands a still's frame straight to the encoder, so the item takes the grid and its
 // unpacked frame goes to the sink unresized.  A size outside the box stays per image, which refuses it.
+//
+// A clip item of lp_xbatch_encode_clips with nframes >= 2 takes the gates of what Transform does with A_i, its animated
+// WebP of full-canvas, no-blend, no-dispose frames (clip_gates); one of a single frame is the tensor item above.
+static bool frame_args_ok(const lp_xbatch* X, int i) {
+    const int w = X->src_w[i], h = X->src_h[i];
+    if (w < 1 || h < 1 || w > X->frames.width || h > X->frames.height) return false;
+    if (!X->src_nframes) return true;
+    const int nf = X->src_nframes[i];
+    if (nf < 1 || nf > X->src_t) return false;
+    for (int t = 0; nf > 1 && t < nf; t++) {  // (ANMF holds 24 bits of duration)
+        const int ms = X->src_ms[(size_t)i * X->src_t + t];
+        if (ms < 0 || ms > 0xFFFFFF) return false;
+    }
+    return true;
+}
+
+// The clip gates (nframes >= 2).  Transform decodes A_i's frames in order; each one covers the canvas without blending,
+// so the composite it fits is the frame itself, and Transform fits an animation even under NoResize, to its own size
+// (a copy: the resize of an unchanged size copies).  What the item's output reads, and when Transform decides after a
+// frame in ways the per-image route reports:
+//   - .webp: every frame goes to the encoder, which writes each with its duration, A_i's background and loop count.
+//     Transform checks its deadline after every non-final frame, so a zero EncodeTimeout fails there
+//     (ErrEncodeTimeout): per image.  DisableAnimatedOutput: Transform encodes frame 0 and flushes before that check,
+//     so the file is a still of frame 0 and only frame 0 is read, whatever the budget.  A non-zero MaxEncodeFrames
+//     makes Transform ask the decoder to skip to the end, which it cannot (ErrSkipNotSupported), unless the stream
+//     ends first: per image.
+//   - .jpeg and .png: the still encoder answers on frame 0, so only frame 0 is read; no deadline, frame limit or
+//     DisableAnimatedOutput is consulted.
+//   - any file sink: a non-zero MaxEncodeDuration is held against the frames' durations before each encode, and
+//     exceeding it ends in a skip to the end: per image.
+//   - .gif: per image (ErrGifEncoderNeedsDecoder).
+static bool clip_gates(XItem& it, const Rendition& R, int nf) {
+    const lp_image_options& opt = R.opt;
+    if (R.sink == S_GIF || opt.max_encode_duration_ns != 0) return false;
+    if (R.sink != S_WEBP) {
+        it.src_frames = 1;
+        return true;
+    }
+    if (opt.max_encode_frames != 0) return false;
+    if (opt.disable_animated_output) {
+        it.src_frames = 1;
+        return true;
+    }
+    if (opt.encode_timeout_ns <= 0) return false;
+    it.src_frames = nf;
+    return true;
+}
+
 static void parse_frame_pair(const lp_xbatch* X, int i, XItem& it, const Rendition& R, int max_side) {
     const int w = X->src_w[i], h = X->src_h[i];
-    if (w < 1 || h < 1 || w > X->frames.width || h > X->frames.height || w > max_side || h > max_side) return;
-    if (R.opt.max_encode_duration_ns < 0 || R.sink == S_GIF || (R.sink == S_WEBP && webp_decides_after_frame(R.opt))) return;
+    if (!frame_args_ok(X, i) || w > max_side || h > max_side) return;
+    const int nf = X->src_nframes ? X->src_nframes[i] : 1;
+    if (nf > 1) {
+        if (!clip_gates(it, R, nf)) return;
+    } else if (R.opt.max_encode_duration_ns < 0 || R.sink == S_GIF || (R.sink == S_WEBP && webp_decides_after_frame(R.opt))) {
+        return;
+    }
     it.w = w;
     it.h = h;
     it.ch = X->frames.channels;
@@ -728,16 +787,19 @@ static size_t jpeg_batch_cap(const lp_xbatch* X, int ow, int oh) {
 }
 
 // resized frames of a pair: every frame of an animation (of its plan, which DisableAnimatedOutput cuts to frame 0), one
-// of a still; of a clip, its slots in use
+// of a still; of a clip, its slots in use; of a tensor item, the frames its output reads
 static int out_frames(const XItem& it) {
     if (!it.clip.empty()) return (int)it.clip.size();
     if (it.kind == K_GIF) return it.gif_frames;
+    if (it.kind == K_FRAME) return it.src_frames;
     return it.kind == K_WEBP ? (int)it.webp->frames.size() : 1;
 }
 
 // WebP (stills and animations): one encode of every frame of the run, then each pair's file around its frames with the
-// metadata WebpEncoder takes from the decoder: the ICC profile the pair kept and, from a WebP or GIF source, background,
-// loop count and frame durations (webp_assemble writes none of these three into a one-frame file)
+// metadata WebpEncoder takes from the decoder: the ICC profile the pair kept and, from a WebP or GIF source or a tensor
+// clip (A_i: background 0xFFFFFFFF, the call's loop count, the caller's durations), background, loop count and frame
+// durations (webp_assemble writes none of these three into a one-frame file).  Every frame is written full-canvas with
+// no blending and no disposal, as the per-image encoder writes whatever blend and dispose it receives.
 static void webp_sink(lp_xbatch* X, const Rendition& R, Lane& L, const std::vector<int>& pairs, const std::vector<int>& st,
                       const uint8_t* d_frames, size_t stride, std::vector<int>* failed) {
     const XItem& g = X->items[pairs[0]];
@@ -768,10 +830,13 @@ static void webp_sink(lp_xbatch* X, const Rendition& R, Lane& L, const std::vect
             int n = 0;
             gif_plan_info(it.gif.get(), nullptr, nullptr, nullptr, &bg, &n);
             loops = (uint32_t)n;
+        } else if (it.kind == K_FRAME && nf > 1) {
+            loops = (uint32_t)X->src_loops;
         }
         for (int j = 0; j < nf; j++) {
             if (it.kind == K_WEBP) f[j].duration = it.webp->frames[j].duration;
             if (it.kind == K_GIF) f[j].duration = gif_plan_delay_ms(it.gif.get(), j);
+            if (it.kind == K_FRAME && nf > 1) f[j].duration = X->src_ms[(size_t)(i / X->k) * X->src_t + j];
             L.d2h += f[j].image.size() + f[j].alph.size();
         }
         webp_assemble(f, nf, it.icc.data(), it.icc.size(), bg, loops, &file);
@@ -1148,27 +1213,32 @@ static void run_webp(lp_xbatch* X, Lane& L, const Task& t) {
     for (int p : failed) push_fallback(X, p);
 }
 
-// Tensor task (lp_xbatch_encode_frames, one rendition): one unpack launch turns every item's slice into a packed u8 frame
-// (its "decode"), then the PNG task's path: per run of equal geometry one resize and the sink.  Under NoResize no resize
-// runs and the sink reads the unpacked frames.  Only the item table crosses PCIe on the way in.
+// Tensor task (lp_xbatch_encode_frames and _clips, one rendition): one unpack launch turns the slices every item's output
+// reads (one, or a clip's frames to an animated .webp) into packed u8 frames, laid out as an animation's canvases: an
+// item's frames back to back, items in task order (its "decode").  Then the path of the other kinds: per run of equal
+// geometry one resize and the sink.  Under NoResize no resize runs and the sink reads the unpacked frames.  Only the item
+// table crosses PCIe on the way in.
 static void run_frame(lp_xbatch* X, Lane& L, const Task& t) {
     const std::vector<int>& idx = t.idx;
     const int n = (int)idx.size();
     const bool resize = X->rend[0].opt.resize_method != LP_OPS_NO_RESIZE;
     Bump bump{L.dev, L.dev_bytes};
     std::vector<uint64_t> frame_off((size_t)n), out_off((size_t)n);
+    std::vector<int> first((size_t)n + 1, 0);  // frames
     size_t frame_bytes = 0, out_bytes = 0;
     uint64_t max_frame = 0;
     for (int k = 0; k < n; k++) {
         const XItem& it = X->items[idx[k]];
         const size_t fb = (size_t)it.w * it.h * it.ch;
+        first[k + 1] = first[k] + it.src_frames;
         frame_off[k] = frame_bytes;
-        frame_bytes += round_up(fb, (size_t)256);
+        frame_bytes += (size_t)it.src_frames * round_up(fb, (size_t)256);
         max_frame = std::max<uint64_t>(max_frame, fb);
         out_off[k] = out_bytes;
-        out_bytes += round_up((size_t)it.ow * it.oh * it.ch, (size_t)256);
+        out_bytes += (size_t)it.src_frames * round_up((size_t)it.ow * it.oh * it.ch, (size_t)256);
     }
-    FrameUnpackItem* d_tab = bump.take<FrameUnpackItem>((size_t)n * sizeof(FrameUnpackItem));
+    const int nf = first[n];
+    FrameUnpackItem* d_tab = bump.take<FrameUnpackItem>((size_t)nf * sizeof(FrameUnpackItem));
     uint8_t* d_frames = bump.take<uint8_t>(frame_bytes + 256);
     uint8_t* d_out = resize ? bump.take<uint8_t>(out_bytes + 256) : d_frames;
     if (!d_tab || !d_frames || !d_out) {
@@ -1176,19 +1246,21 @@ static void run_frame(lp_xbatch* X, Lane& L, const Task& t) {
         return;
     }
     if (!resize) out_off = frame_off;
-    std::vector<FrameUnpackItem> tab((size_t)n);
+    std::vector<FrameUnpackItem> tab((size_t)nf);
     for (int k = 0; k < n; k++) {
         const XItem& it = X->items[idx[k]];
-        tab[k] = FrameUnpackItem{d_frames + frame_off[k], it.w, it.h, idx[k]};
+        const size_t fs = round_up((size_t)it.w * it.h * it.ch, (size_t)256);
+        for (int f = 0; f < it.src_frames; f++)
+            tab[(size_t)first[k] + f] = FrameUnpackItem{d_frames + frame_off[k] + f * fs, it.w, it.h, (int64_t)idx[k] * X->src_t + f};
     }
     bool ok = cudaMemcpyAsync(d_tab, tab.data(), tab.size() * sizeof(FrameUnpackItem), cudaMemcpyHostToDevice, L.st) == cudaSuccess;
     L.h2d += tab.size() * sizeof(FrameUnpackItem);
     cudaEventRecord(L.ev[0], L.st);
-    if (ok) ok = frames_unpack_launch(d_tab, nullptr, n, max_frame, frames_layout(X->frames), L.st) == LP_OK;
+    if (ok) ok = frames_unpack_launch(d_tab, nullptr, nf, max_frame, frames_layout(X->frames), L.st) == LP_OK;
     cudaEventRecord(L.ev[1], L.st);
     if (resize)
         for (const Run& u : task_runs(X, t, 0, 0, n, false))
-            ok = ok && resize_run(L, X->items[idx[u.k0]], d_frames + frame_off[u.k0], d_out + out_off[u.k0], u.k1 - u.k0);
+            ok = ok && resize_run(L, X->items[idx[u.k0]], d_frames + frame_off[u.k0], d_out + out_off[u.k0], first[u.k1] - first[u.k0]);
     cudaEventRecord(L.ev[2], L.st);
     if (ok) ok = cudaStreamSynchronize(L.st) == cudaSuccess;
     if (!ok) {
@@ -1537,8 +1609,8 @@ static size_t item_device_bytes(const lp_xbatch* X, int i, uint32_t rm) {
                    (size_t)out_frames(it) * (round_up((size_t)it.w * it.h * it.ch, (size_t)256) + outb) + 8192;
         case K_GIF:  // (canvases and resized frames: every frame, or a clip's slots)
             return gif_plan_device_bytes(it.gif.get()) + (size_t)out_frames(it) * ((size_t)it.w * it.h * 4 + outb) + 8192 + gif_enc;
-        case K_FRAME:  // the unpacked frame, its table entry and its output
-            return round_up((size_t)it.w * it.h * it.ch, (size_t)256) + sizeof(FrameUnpackItem) + outb + 8192;
+        case K_FRAME:  // the unpacked frames (one, or a clip's to an animated .webp), their table entries and outputs
+            return (size_t)it.src_frames * (round_up((size_t)it.w * it.h * it.ch, (size_t)256) + sizeof(FrameUnpackItem) + outb) + 8192;
         default:
             return 0;
     }
@@ -1627,19 +1699,21 @@ static int clips_transform(lp_xbatch* X, int i, const lp_image_options* opt, int
     return LP_OK;
 }
 
-// lp_xbatch_encode_frames' per-image route: Transform with a decoder that answers as a PNG of the frame would, whose
-// DecodeTo unpacks slice i with the grid path's kernel into the framebuffer's device mirror on this worker's stream.
-// A size outside the box is refused here.
+// lp_xbatch_encode_frames' and _clips' per-image route: Transform with a decoder that answers as a PNG of the frame
+// would (one frame) or as WebpDecoder would for A_i (a clip), whose DecodeTo unpacks frame k's slice with the grid path's
+// kernel into the framebuffer's device mirror on this worker's stream.  The per-item argument errors are refused here.
 static int transform_from_frame(lp_xbatch* X, int i, const lp_image_options* opt, int max_size, uint8_t* dst, size_t* len) {
     const lp_frame_tensor& T = X->frames;
     const int w = X->src_w[i], h = X->src_h[i];
-    if (w < 1 || h < 1 || w > T.width || h > T.height) return LP_ERR_BAD_ARGUMENT;
-    return lilliput::TransformFromFrame(w, h, T.channels, opt, max_size, [&](lilliput::Framebuffer* f) -> int {
+    if (!frame_args_ok(X, i)) return LP_ERR_BAD_ARGUMENT;
+    const int nf = X->src_nframes ? X->src_nframes[i] : 1;
+    const int* ms = X->src_ms ? X->src_ms + (size_t)i * X->src_t : nullptr;
+    return lilliput::TransformFromClip(w, h, T.channels, nf, ms, X->src_loops, opt, max_size, [&](lilliput::Framebuffer* f, int k) -> int {
         uint8_t* dev = nullptr;
         size_t step = 0;
         int rc = mat_bind_device_frame(f->mat, w, h, f->Type().v, &dev, &step);
         if (rc) return rc;
-        const FrameUnpackItem one{dev, w, h, i};
+        const FrameUnpackItem one{dev, w, h, (int64_t)i * X->src_t + k};
         cudaStream_t st = thread_stream();
         rc = frames_unpack_launch(nullptr, &one, 1, (uint64_t)w * h * T.channels, frames_layout(T), st);
         if (!rc && cudaStreamSynchronize(st) != cudaSuccess) rc = LP_ERR_CUDA;
@@ -2002,19 +2076,47 @@ extern "C" int lp_xbatch_decode_clips(lp_xbatch* X, const uint8_t* const* in, co
     return rc;
 }
 
+// lp_xbatch_encode_frames (T 1, nframes null: one frame each) and lp_xbatch_encode_clips: files from the items' slices of
+// a checked tensor, T per item
+static int encode_tensor(lp_xbatch* X, const lp_frame_tensor& src, int n, int T, const int* nframes, const int* width,
+                         const int* height, const int* duration_ms, int loop_count, const lp_image_options* opt,
+                         uint8_t* const* out, size_t out_cap, size_t* out_len, int* status) {
+    X->frames = src;
+    X->src_w = width;
+    X->src_h = height;
+    X->src_t = T;
+    X->src_nframes = nframes;
+    X->src_ms = duration_ms;
+    X->src_loops = loop_count;
+    const Rendition R = opt ? make_rendition(*opt) : Rendition();  // (opt may be null when n == 0)
+    const int rc = xbatch_call(X, nullptr, nullptr, n, opt, &R, 1, out, out_cap, out_len, status);
+    X->src_w = X->src_h = nullptr;
+    X->src_t = 1;
+    X->src_nframes = X->src_ms = nullptr;
+    X->src_loops = 0;
+    return rc;
+}
+
+extern "C" int lp_xbatch_encode_clips(lp_xbatch* X, const lp_frame_tensor* src, int n, int frames_per_item, const int* nframes,
+                                      const int* width, const int* height, const int* duration_ms, int loop_count,
+                                      const lp_image_options* opt, uint8_t* const* out, size_t out_cap, size_t* out_len,
+                                      int* status) {
+    const int T = frames_per_item;
+    if (!X || n < 0 || T < 1 || T > LP_XBATCH_MAX_CLIP_FRAMES || loop_count < 0 || loop_count > 65535 ||
+        (n > 0 && (!opt || !nframes || !width || !height || !duration_ms || !out || !out_len || !status)))
+        return LP_ERR_BAD_ARGUMENT;
+    size_t slice = 0;
+    if ((int64_t)n * T > INT_MAX || check_frame_tensor(X, src, n * T, &slice)) return LP_ERR_BAD_ARGUMENT;
+    return encode_tensor(X, *src, n, T, nframes, width, height, duration_ms, loop_count, opt, out, out_cap, out_len, status);
+}
+
 extern "C" int lp_xbatch_encode_frames(lp_xbatch* X, const lp_frame_tensor* src, int n, const int* width, const int* height,
                                        const lp_image_options* opt, uint8_t* const* out, size_t out_cap, size_t* out_len,
                                        int* status) {
     if (!X || n < 0 || (n > 0 && (!opt || !width || !height || !out || !out_len || !status))) return LP_ERR_BAD_ARGUMENT;
     size_t slice = 0;
     if (check_frame_tensor(X, src, n, &slice)) return LP_ERR_BAD_ARGUMENT;
-    X->frames = *src;
-    X->src_w = width;
-    X->src_h = height;
-    const Rendition R = opt ? make_rendition(*opt) : Rendition();  // (opt may be null when n == 0)
-    const int rc = xbatch_call(X, nullptr, nullptr, n, opt, &R, 1, out, out_cap, out_len, status);
-    X->src_w = X->src_h = nullptr;
-    return rc;
+    return encode_tensor(X, *src, n, 1, nullptr, width, height, nullptr, 0, opt, out, out_cap, out_len, status);
 }
 
 // ------------------------------------------------------------------ library-level multi-GPU dispatch

@@ -1040,53 +1040,71 @@ Error TransformToClip(const uint8_t* in, size_t in_len, const lp_image_options* 
     }
 }
 
-// A decoder of one w x h frame of 3 (BGR) or 4 (BGRA) channels whose pixels `fill` writes, answering as OpenCVDecoder
-// answers for an 8-bit PNG of colour type 2 or 6 without ancillary chunks: orientation 1, one frame, no ICC profile, no
-// cICP, no GIF handle
+// A decoder of `nframes` w x h frames of 3 (BGR) or 4 (BGRA) channels whose pixels `fill` writes.  One frame: it answers
+// as OpenCVDecoder answers for an 8-bit PNG of colour type 2 or 6 without ancillary chunks (orientation 1, no ICC
+// profile, no cICP, no GIF handle).  Several: as WebpDecoder answers for an animated WebP of full-canvas frames with no
+// blending or disposal, frame k lasting duration_ms[k], background 0xFFFFFFFF and loop count `loops` (webp.go:50-59,
+// 139-176; the alpha flag gives the channel count), with no ICC profile either.
 class FrameDecoder : public Decoder {
   public:
-    FrameDecoder(int w, int h, int channels, const FrameSink& f) : width(w), height(h), type(channels == 4 ? CV_8UC4 : CV_8UC3), fill(f) {}
+    FrameDecoder(int w, int h, int channels, int nframes, const int* duration_ms, int loops, const ClipFill& f)
+        : width(w), height(h), type(channels == 4 ? CV_8UC4 : CV_8UC3), frames(nframes), ms(duration_ms), loops(loops), fill(f) {}
     Error Header(ImageHeader* h) override {
         h->width = width;
         h->height = height;
         h->pixelType.v = type;
         h->orientation = 1;
-        h->numFrames = 1;
+        h->numFrames = frames;
         return LP_OK;
     }
-    std::string Description() override { return "PNG"; }
-    Error DecodeTo(Framebuffer* f) override {  // as OpenCVDecoder::DecodeTo
-        if (decoded) return LP_ERR_EOF;
+    std::string Description() override { return frames > 1 ? "WEBP" : "PNG"; }
+    Error DecodeTo(Framebuffer* f) override {  // as OpenCVDecoder::DecodeTo, or WebpDecoder::DecodeTo
+        if (next >= frames) return LP_ERR_EOF;
         Error e = f->resizeMat(width, height, PixelType{type});
         if (e) return e;
-        if ((e = fill(f))) return e;
-        decoded = true;
+        if ((e = fill(f, next))) return e;
+        const bool anim = frames > 1;
         f->blend = NoBlend;
-        f->dispose = DisposeToBackgroundColor;
+        f->dispose = anim ? NoDispose : DisposeToBackgroundColor;
         f->xOffset = 0;
         f->yOffset = 0;
-        f->duration_ns = 0;
+        f->duration_ns = anim ? (int64_t)ms[next] * 1000000 : 0;
+        next++;
         return LP_OK;
     }
     Error SkipFrame() override { return LP_ERR_SKIP_NOT_SUPPORTED; }
+    int LoopCount() override { return frames > 1 ? loops : 0; }
+    int64_t Duration_ns() override {
+        int64_t total = 0;
+        for (int k = 0; frames > 1 && k < frames; k++) total += ms[k];
+        return total * 1000000;
+    }
 
   private:
-    int width, height, type;
-    const FrameSink& fill;
-    bool decoded = false;
+    int width, height, type, frames;
+    const int* ms;
+    int loops;
+    const ClipFill& fill;
+    int next = 0;  // the frame DecodeTo delivers next
 };
 
-Error TransformFromFrame(int w, int h, int channels, const lp_image_options* opt, int max_size, const FrameSink& fill, uint8_t* dst,
-                         size_t dst_cap, size_t* out_len) {
+Error TransformFromClip(int w, int h, int channels, int nframes, const int* duration_ms, int loop_count, const lp_image_options* opt,
+                        int max_size, const ClipFill& fill, uint8_t* dst, size_t dst_cap, size_t* out_len) {
     try {
-        if (!opt || !dst || !out_len) return LP_ERR_BAD_ARGUMENT;
-        FrameDecoder d(w, h, channels, fill);
+        if (!opt || !dst || !out_len || nframes < 1 || (nframes > 1 && !duration_ms)) return LP_ERR_BAD_ARGUMENT;
+        FrameDecoder d(w, h, channels, nframes, duration_ms, loop_count, fill);
         return thread_ops(max_size)->Transform(&d, fromC(opt), dst, dst_cap, out_len);
     } catch (const std::bad_alloc&) {
         return LP_ERR_BUF_TOO_SMALL;
     } catch (...) {
         return LP_ERR_BAD_ARGUMENT;
     }
+}
+
+Error TransformFromFrame(int w, int h, int channels, const lp_image_options* opt, int max_size, const FrameSink& fill, uint8_t* dst,
+                         size_t dst_cap, size_t* out_len) {
+    return TransformFromClip(w, h, channels, 1, nullptr, 0, opt, max_size, [&](Framebuffer* f, int) { return fill(f); }, dst, dst_cap,
+                             out_len);
 }
 
 }  // namespace lilliput

@@ -212,4 +212,12 @@ Error TransformToClip(const uint8_t* in, size_t in_len, const lp_image_options* 
 Error TransformFromFrame(int w, int h, int channels, const lp_image_options* opt, int max_size, const FrameSink& fill, uint8_t* dst,
                          size_t dst_cap, size_t* out_len);
 
+// The animated form: lp_transform of A, an animated WebP of `nframes` (>= 2) full-canvas w x h frames of `channels`,
+// with no blending or disposal, frame k lasting duration_ms[k], background 0xFFFFFFFF and loop_count, whose frames are
+// lossless.  The FrameDecoder then answers as WebpDecoder answers for A, and its DecodeTo calls fill(framebuffer, k)
+// for frame k.  nframes == 1 is TransformFromFrame (durations and loop count unused).
+using ClipFill = std::function<Error(Framebuffer*, int frame)>;
+Error TransformFromClip(int w, int h, int channels, int nframes, const int* duration_ms, int loop_count, const lp_image_options* opt,
+                        int max_size, const ClipFill& fill, uint8_t* dst, size_t dst_cap, size_t* out_len);
+
 }  // namespace lilliput
