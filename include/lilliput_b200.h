@@ -289,6 +289,32 @@ int lp_xbatch_decode_frames(lp_xbatch* x, const uint8_t* const* in, const size_t
                             const lp_image_options* opt, const lp_frame_tensor* dst, int* width, int* height,
                             int* status);
 
+/* Files and pixels of the same uploads in one call: k file renditions (opts[0..k-1], as lp_xbatch_transform_renditions)
+ * and m frame renditions (frames[0..m-1], as lp_xbatch_decode_frames), 0 <= k, 0 <= m, 1 <= k + m <=
+ * LP_XBATCH_MAX_RENDITIONS.
+ *   - out, out_len and status have n * k item-major entries, each exactly what lp_xbatch_transform_renditions(in, in_len,
+ *     n, opts, k, ...) writes there
+ *   - frames[j].dst, width, height and status hold exactly what lp_xbatch_decode_frames(in, in_len, n, &frames[j].opt,
+ *     &frames[j].dst, ...) writes; the slices of failed items are zero
+ * Each file is uploaded and decoded once for all the renditions it takes on the grid path, file and frame alike; an
+ * animation decodes once per rendition, and an EXIF-rotated or gray JPEG (which only frame renditions take there) once
+ * per frame rendition.  LP_ERR_BAD_ARGUMENT, with nothing written, for: a bad k or m; n < 0; a null in / in_len with
+ * n > 0; a null opts with k > 0, or null out / out_len / status with n > 0 and k > 0; a null frames with m > 0; any
+ * frame rendition failing lp_xbatch_decode_frames' argument checks; two tensors whose n slices overlap.  Stats:
+ * grid_items and fallback_items count all n * (k + m) pairs; d2h_bytes counts files only; h2d_bytes is the file
+ * renditions' call's plus the frame renditions' pack tables.  lp_xbatch_transform_renditions is this call with m = 0,
+ * lp_xbatch_decode_frames with k = 0 and m = 1. */
+typedef struct lp_frame_rendition {
+    lp_image_options opt; /* as lp_xbatch_decode_frames' opt (file_type and encode options ignored) */
+    lp_frame_tensor dst;  /* n slices, as lp_xbatch_decode_frames' dst */
+    int* width;           /* n entries each */
+    int* height;
+    int* status;
+} lp_frame_rendition;
+int lp_xbatch_transform_frames(lp_xbatch* x, const uint8_t* const* in, const size_t* in_len, int n,
+                               const lp_image_options* opts, int k, uint8_t* const* out, size_t out_cap,
+                               size_t* out_len, int* status, const lp_frame_rendition* frames, int m);
+
 /* Clips instead of one frame: up to T = frames_per_item frames of every item, spread over the whole animation, written
  * into the caller's device tensor.  Slice i * T + t of dst (the same lp_frame_tensor as lp_xbatch_decode_frames, n * T
  * slices; with nchw an N x T x C x H x W tensor) holds slot t of item i.

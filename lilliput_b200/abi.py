@@ -480,6 +480,19 @@ class _FrameTensor(C.Structure):
                 ("scale", C.c_float * 4), ("bias", C.c_float * 4)]
 
 
+def _frame_tensor(data_ptr: int, bytes: int, height: int, width: int, channels: int = 3, nchw: bool = False,
+                  rgb: bool = True, dtype: str = "u8", scale=None, bias=None) -> _FrameTensor:
+    return _FrameTensor(data_ptr, bytes, height, width, channels, int(bool(nchw)), int(bool(rgb)),
+                        FRAME_DTYPES.get(dtype, -1) if isinstance(dtype, str) else int(dtype),
+                        (C.c_float * 4)(*(list(scale) if scale is not None else [1.0] * 4)),
+                        (C.c_float * 4)(*(list(bias) if bias is not None else [0.0] * 4)))
+
+
+class _FrameRendition(C.Structure):
+    _fields_ = [("opt", _ImageOptions), ("dst", _FrameTensor), ("width", C.c_void_p), ("height", C.c_void_p),
+                ("status", C.c_void_p)]
+
+
 def _renditions(fn, h, bufs, opts, out_cap):
     """lp_xbatch_transform_renditions / lp_multi_transform_renditions: every file through every ImageOptions of
     `opts`.  Returns (outs, status), both indexed [item][rendition]."""
@@ -518,6 +531,10 @@ class XBatch:
         l.lp_xbatch_decode_frames.restype = C.c_int
         l.lp_xbatch_decode_frames.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.POINTER(_ImageOptions),
                                               C.POINTER(_FrameTensor), C.c_void_p, C.c_void_p, C.c_void_p]
+        l.lp_xbatch_transform_frames.restype = C.c_int
+        l.lp_xbatch_transform_frames.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.POINTER(_ImageOptions),
+                                                 C.c_int, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p,
+                                                 C.POINTER(_FrameRendition), C.c_int]
         l.lp_xbatch_decode_clips.restype = C.c_int
         l.lp_xbatch_decode_clips.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.POINTER(_ImageOptions), C.c_int,
                                              C.POINTER(_FrameTensor), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
@@ -568,16 +585,42 @@ class XBatch:
         Float dtypes store sample * scale[c] + bias[c] per output channel.  Returns (width, height, status) lists."""
         n = len(bufs)
         ptrs, lens, keep = Batch._ptr_arrays(bufs)
-        t = _FrameTensor(data_ptr, bytes, height, width, channels, int(bool(nchw)), int(bool(rgb)),
-                         FRAME_DTYPES.get(dtype, -1) if isinstance(dtype, str) else int(dtype),
-                         (C.c_float * 4)(*(list(scale) if scale is not None else [1.0] * 4)),
-                         (C.c_float * 4)(*(list(bias) if bias is not None else [0.0] * 4)))
+        t = _frame_tensor(data_ptr, bytes, height, width, channels, nchw, rgb, dtype, scale, bias)
         w, h, status = (C.c_int * max(n, 1))(), (C.c_int * max(n, 1))(), (C.c_int * max(n, 1))()
         copt = opt._c()
         rc = self.lib.l.lp_xbatch_decode_frames(self.h, ptrs, lens, n, C.byref(copt), C.byref(t), w, h, status)
         if rc:
             raise LilliputError(rc)
         return list(w[:n]), list(h[:n]), list(status[:n])
+
+    def transform_frames(self, bufs, opts, frame_specs, out_cap: int = 1 << 20):
+        """lp_xbatch_transform_frames: every file through every ImageOptions of `opts` (as transform_renditions) and into
+        every frame rendition of `frame_specs` (as decode_frames) in one call, each file decoded once.  A frame spec is a
+        dict of decode_frames' arguments: opt, data_ptr, bytes, height, width, and optionally channels, nchw, rgb, dtype,
+        scale, bias.  Returns (outs, status, frames): outs and status indexed [item][rendition], and one
+        (width, height, status) of lists per frame spec."""
+        n, k, m = len(bufs), len(opts), len(frame_specs)
+        ptrs, lens, keep = Batch._ptr_arrays(bufs)
+        out = np.empty((max(n * k, 1), out_cap), dtype=np.uint8)
+        out_ptrs = (C.c_void_p * max(n * k, 1))(*[out[p].ctypes.data for p in range(n * k)])
+        out_lens = (C.c_size_t * max(n * k, 1))()
+        status = (C.c_int * max(n * k, 1))()
+        cs = [o._c() for o in opts]  # (they own the strings and option arrays the copies point at)
+        copts = (_ImageOptions * max(k, 1))(*cs)
+        fcs = [f["opt"]._c() for f in frame_specs]
+        sizes = [[(C.c_int * max(n, 1))() for _ in range(3)] for _ in range(m)]
+        tensor_args = ("data_ptr", "bytes", "height", "width", "channels", "nchw", "rgb", "dtype", "scale", "bias")
+        frs = (_FrameRendition * max(m, 1))(*[
+            _FrameRendition(fcs[j], _frame_tensor(**{a: f[a] for a in tensor_args if a in f}),
+                            C.cast(sizes[j][0], C.c_void_p), C.cast(sizes[j][1], C.c_void_p), C.cast(sizes[j][2], C.c_void_p))
+            for j, f in enumerate(frame_specs)])
+        rc = self.lib.l.lp_xbatch_transform_frames(self.h, ptrs, lens, n, copts, k, out_ptrs, out_cap, out_lens, status,
+                                                   frs, m)
+        if rc:
+            raise LilliputError(rc)
+        return ([[out[i * k + r, : out_lens[i * k + r]].tobytes() for r in range(k)] for i in range(n)],
+                [[status[i * k + r] for r in range(k)] for i in range(n)],
+                [(list(w[:n]), list(h[:n]), list(st[:n])) for w, h, st in sizes])
 
     def decode_clips(self, bufs, opt: ImageOptions, frames_per_item: int, data_ptr: int, bytes: int, height: int, width: int,
                      channels: int = 3, nchw: bool = False, rgb: bool = True, dtype: str = "u8", scale=None, bias=None):
@@ -587,10 +630,7 @@ class XBatch:
         per item, per slot (-1: unused), per slot (ms before the slot's frame), per item."""
         n, T = len(bufs), frames_per_item
         ptrs, lens, keep = Batch._ptr_arrays(bufs)
-        t = _FrameTensor(data_ptr, bytes, height, width, channels, int(bool(nchw)), int(bool(rgb)),
-                         FRAME_DTYPES.get(dtype, -1) if isinstance(dtype, str) else int(dtype),
-                         (C.c_float * 4)(*(list(scale) if scale is not None else [1.0] * 4)),
-                         (C.c_float * 4)(*(list(bias) if bias is not None else [0.0] * 4)))
+        t = _frame_tensor(data_ptr, bytes, height, width, channels, nchw, rgb, dtype, scale, bias)
         w, h, nf, status = [(C.c_int * max(n, 1))() for _ in range(4)]
         slots = max(n * max(T, 0), 1)
         index, start = (C.c_int * slots)(), (C.c_int64 * slots)()
@@ -608,10 +648,7 @@ class XBatch:
         item i the top-left widths[i] x heights[i] of slice i, each file equal to lp_transform of an 8-bit PNG of that
         frame with opt.  Float dtypes read round(x * scale[c] + bias[c]) clamped to 0..255.  Returns (outs, status)."""
         n = len(widths)
-        t = _FrameTensor(data_ptr, bytes, height, width, channels, int(bool(nchw)), int(bool(rgb)),
-                         FRAME_DTYPES.get(dtype, -1) if isinstance(dtype, str) else int(dtype),
-                         (C.c_float * 4)(*(list(scale) if scale is not None else [1.0] * 4)),
-                         (C.c_float * 4)(*(list(bias) if bias is not None else [0.0] * 4)))
+        t = _frame_tensor(data_ptr, bytes, height, width, channels, nchw, rgb, dtype, scale, bias)
         ws, hs = (C.c_int * max(n, 1))(*widths), (C.c_int * max(n, 1))(*heights)
         out = np.empty((max(n, 1), out_cap), dtype=np.uint8)
         out_ptrs = (C.c_void_p * max(n, 1))(*[out[i].ctypes.data for i in range(n)])
@@ -632,10 +669,7 @@ class XBatch:
         full-canvas frames with those durations and loop_count; one of a single frame is an encode_frames item.
         Returns (outs, status)."""
         n, T = len(widths), frames_per_item
-        t = _FrameTensor(data_ptr, bytes, height, width, channels, int(bool(nchw)), int(bool(rgb)),
-                         FRAME_DTYPES.get(dtype, -1) if isinstance(dtype, str) else int(dtype),
-                         (C.c_float * 4)(*(list(scale) if scale is not None else [1.0] * 4)),
-                         (C.c_float * 4)(*(list(bias) if bias is not None else [0.0] * 4)))
+        t = _frame_tensor(data_ptr, bytes, height, width, channels, nchw, rgb, dtype, scale, bias)
         nf, ws, hs = (C.c_int * max(n, 1))(*nframes), (C.c_int * max(n, 1))(*widths), (C.c_int * max(n, 1))(*heights)
         ms = (C.c_int * max(n * max(T, 0), 1))(*durations_ms)
         out = np.empty((max(n, 1), out_cap), dtype=np.uint8)

@@ -80,7 +80,7 @@ namespace lp {
 lp_batch* batch_create_in(const lp_batch_config* cfg, uint8_t* dev_arena, size_t dev_bytes, uint8_t* host_arena,
                           size_t host_bytes, bool progressive_jpeg, bool multiscan_sources, bool resize_only,
                           bool oriented_sources = false,  // (rotated and gray JPEGs are handed to lp_transform before
-                          bool gray_sources = false,      // grouping, except by lp_xbatch_decode_frames)
+                          bool gray_sources = false,      // grouping, except by frame renditions)
                           const BatchGeom* geoms = nullptr, int n_geoms = 0);
 int batch_resized_status(lp_batch* b, int* status);
 const uint8_t* batch_resized_geom(const lp_batch* b, int g, size_t* image_stride);
@@ -93,7 +93,7 @@ int mat_bind_device_frame(void* mat, int cols, int rows, int type, uint8_t** dev
 namespace {
 
 enum Kind { K_FALLBACK = 0, K_JPEG = 1, K_PNG = 2, K_WEBP = 3, K_GIF = 4, K_FRAME = 5 };  // K_FRAME: lp_xbatch_encode_frames
-enum Sink { S_NONE = 0, S_JPEG = 1, S_WEBP = 2, S_GIF = 3, S_PNG = 4, S_FRAMES = 5 };  // S_FRAMES: lp_xbatch_decode_frames
+enum Sink { S_NONE = 0, S_JPEG = 1, S_WEBP = 2, S_GIF = 3, S_PNG = 4, S_FRAMES = 5 };  // S_FRAMES: a frame rendition
 constexpr int kMaxRenditions = LP_XBATCH_MAX_RENDITIONS;  // (a rendition mask is one 32-bit word)
 
 // One output the call asks of every item: its options and what the sink takes from them
@@ -105,6 +105,9 @@ struct Rendition {
     bool progressive = false;  // S_JPEG: progressive files (JpegProgressive)
     int png_level = 1;         // S_PNG: zlib level and filter policy (png_encode_policy)
     bool png_adaptive = false;
+    lp_frame_tensor dst{};     // S_FRAMES: the caller's tensor (item i's slices from i * max(1, clip_t)) and each item's
+    int* frame_w = nullptr;    // frame size (its status is the pair's)
+    int* frame_h = nullptr;
 };
 
 // One (item, rendition) pair.  The source fields (kind, frame, JPEG layout, PNG header, HDR tags) are the item's and
@@ -116,6 +119,7 @@ struct XItem {
     int cx = 0, cy = 0, cw = 0, chh = 0;  // crop rectangle fed to the resize
     int jpeg_sampling = 0;          // (h0<<12)|(v0<<8)|... groups JPEGs of one component layout
     bool jpeg_multiscan = false;    // progressive, or one scan per component
+    bool jpeg_frames_only = false;  // rotated (EXIF 2..8) or gray: only frame renditions take it on the grid
     std::shared_ptr<const PngHeader> png;
     bool hdr = false;                 // PNG: a cICP chunk with a PQ (16) or HLG (18) transfer, tone-mapped after the decode
     int transfer = 0, primaries = 0;  // (its code points)
@@ -185,10 +189,8 @@ struct lp_xbatch {
     size_t out_cap = 0;
     size_t* out_len = nullptr;
     int* status = nullptr;  // (out, out_len and status: one entry per pair, item-major)
-    lp_frame_tensor frames;  // lp_xbatch_decode_frames: the caller's tensor, and each item's frame size
-    int* frame_w = nullptr;
-    int* frame_h = nullptr;
-    int clip_t = 0;  // lp_xbatch_decode_clips: T slots per item (0: lp_xbatch_decode_frames, one), and the slots' outputs
+    lp_frame_tensor frames;  // lp_xbatch_encode_frames and _clips: the caller's source tensor
+    int clip_t = 0;  // lp_xbatch_decode_clips: T slots per item (0: one, any other call), and the slots' outputs
     int* clip_nframes = nullptr;
     int* clip_index = nullptr;
     int64_t* clip_ms = nullptr;
@@ -198,7 +200,7 @@ struct lp_xbatch {
     const int* src_nframes = nullptr;  // uses (null: one each), their durations (ms, T per item) and the loop count
     const int* src_ms = nullptr;
     int src_loops = 0;
-    int k = 1;              // renditions
+    int k = 1;              // renditions (lp_xbatch_transform_frames: the file renditions, then the frame renditions)
     std::vector<Rendition> rend;
     std::vector<XItem> items;   // pairs: item i, rendition r at i * k + r
     std::vector<uint32_t> mask;  // per item: the renditions it takes on the grid
@@ -601,7 +603,9 @@ static void parse_item(lp_xbatch* X, int i) {
     uint32_t m = 0;
     for (int r = 0; r < X->k; r++) {
         parse_pair(X, i, r, &c);
-        if (X->items[(size_t)i * X->k + r].kind != K_FALLBACK) m |= 1u << r;
+        XItem& it = X->items[(size_t)i * X->k + r];
+        if (it.kind != K_FALLBACK) m |= 1u << r;
+        if (it.kind == K_JPEG) it.jpeg_frames_only = c.jh.ncomp == 1 || (c.jh.orientation >= 2 && c.jh.orientation <= 8);
     }
     X->mask[i] = m;
 }
@@ -902,34 +906,34 @@ static FramePackLayout frames_layout(const lp_frame_tensor& t) {
     return o;
 }
 
-// lp_xbatch_decode_frames and lp_xbatch_decode_clips: every frame of the run into its slot's slice of the caller's tensor
-// in one launch.  Item i has `slots` slices from i * slots (one for lp_xbatch_decode_frames, T for a clip); slot t holds
-// its t-th resized frame, and a slot past its frames is an entry of 0 x 0, which the kernel writes as zeros.  The table
-// travels to the device, so items that are not neighbours in the batch land in their own slices, each with its own
-// frame size (a JPEG group's turned or gray items).  A frame larger than the box is refused; an item whose decode failed
+// A frame rendition (lp_xbatch_transform_frames, _decode_frames, _decode_clips): every frame of the run into its slot's
+// slice of the rendition's tensor in one launch.  Item i has `slots` slices from i * slots (one, or T for a clip); slot t
+// holds its t-th resized frame, and a slot past its frames is an entry of 0 x 0, which the kernel writes as zeros.  The
+// table travels to the device, so items that are not neighbours in the batch land in their own slices, each with its own
+// frame size (a JPEG group's turned or gray items).  A frame larger than the box is refused; a pair whose decode failed
 // goes to the per-image path.  Nothing comes back to the host.
-static void frames_sink(lp_xbatch* X, Lane& L, Bump& bump, const std::vector<int>& pairs, const std::vector<int>& st,
+static void frames_sink(lp_xbatch* X, const Rendition& R, Lane& L, Bump& bump, const std::vector<int>& pairs, const std::vector<int>& st,
                         const uint8_t* d_frames, size_t stride, std::vector<int>* failed) {
-    const lp_frame_tensor& T = X->frames;
+    const lp_frame_tensor& T = R.dst;
     const int slots = std::max(1, X->clip_t);
     std::vector<FramePackItem> tab;
-    std::vector<int> packed;
+    std::vector<int> packed;  // pairs
     size_t at = 0;  // the pair's first frame in the run
     for (size_t q = 0; q < pairs.size(); q++) {
-        const int i = pairs[q];  // (one rendition: the pair is the item)
-        const XItem& it = X->items[i];
+        const int p = pairs[q], i = p / X->k;
+        const XItem& it = X->items[p];
         const int nf = out_frames(it);
         if (st[q] != LP_OK) {
-            failed->push_back(i);
+            failed->push_back(p);
         } else if (it.ow > T.width || it.oh > T.height) {
-            X->status[i] = LP_ERR_BUF_TOO_SMALL;
+            X->status[p] = LP_ERR_BUF_TOO_SMALL;
         } else {
             for (int t = 0; t < slots; t++) {
                 const int64_t slice = (int64_t)i * slots + t;
                 tab.push_back(t < nf ? FramePackItem{d_frames + (at + t) * stride, (uint32_t)(it.ow * it.ch), it.ow, it.oh, it.ch, slice}
                                      : FramePackItem{nullptr, 0, 0, 0, it.ch, slice});
             }
-            packed.push_back(i);
+            packed.push_back(p);
         }
         at += nf;
     }
@@ -948,12 +952,13 @@ static void frames_sink(lp_xbatch* X, Lane& L, Bump& bump, const std::vector<int
         return;
     }
     L.h2d += tab.size() * sizeof(FramePackItem);
-    for (int i : packed) {
-        const XItem& it = X->items[i];
-        X->status[i] = LP_OK;
-        X->frame_w[i] = it.ow;
-        X->frame_h[i] = it.oh;
-        if (!X->clip_t) continue;
+    for (int p : packed) {
+        const XItem& it = X->items[p];
+        const int i = p / X->k;
+        X->status[p] = LP_OK;
+        R.frame_w[i] = it.ow;
+        R.frame_h[i] = it.oh;
+        if (!X->clip_t) continue;  // (a clip: the call's one rendition)
         X->clip_nframes[i] = it.nframes;
         for (size_t t = 0; t < it.clip.size(); t++) {
             X->clip_index[(size_t)i * slots + t] = it.clip[t];
@@ -984,7 +989,7 @@ static void sink_encode(lp_xbatch* X, Lane& L, Bump& bump, uint8_t* h_stage, siz
     cudaEventRecord(L.ev[2], L.st);
     if (R.sink == S_WEBP) webp_sink(X, R, L, pairs, pst, d_frames, stride, failed);
     else if (R.sink == S_GIF) gif_sink(X, L, bump, pairs, pst, d_frames, stride, failed);
-    else if (R.sink == S_FRAMES) frames_sink(X, L, bump, pairs, pst, d_frames, stride, failed);
+    else if (R.sink == S_FRAMES) frames_sink(X, R, L, bump, pairs, pst, d_frames, stride, failed);
     else slot_sink(X, R, L, bump, h_stage, h_stage_bytes, pairs, pst, d_frames, stride, jpeg_cap, failed);
     cudaEventRecord(L.ev[3], L.st);
     cudaEventSynchronize(L.ev[3]);
@@ -1418,6 +1423,9 @@ static void run_jpeg(lp_xbatch* X, Lane& L, const Task& t) {
     const XItem& g = X->items[(size_t)idx[0] * K + rs[0]];  // (the source fields are the group's; the output fields rs[0]'s)
     const bool several = rs.size() > 1;
     const bool resize_only = several || R.sink != S_JPEG;  // WebP, PNG, or several renditions: the frames go to the sinks' encoders
+    // a context of one frame rendition takes rotated and gray files (lp_xbatch_decode_frames' contexts, and each task of a
+    // rotated or gray group); a multi-geometry context takes orientation class 0 only, and the file sinks never get them
+    const bool turned = !several && R.sink == S_FRAMES;
     size_t in_bytes = 0;
     for (int i : idx) in_bytes += X->in_len[i];
     lp_batch_config c;
@@ -1429,7 +1437,7 @@ static void run_jpeg(lp_xbatch* X, Lane& L, const Task& t) {
     c.dst_width = R.opt.width;
     c.dst_height = R.opt.height;
     c.resize_method = R.opt.resize_method;
-    c.normalize_orientation = R.opt.normalize_orientation;  // (sizes only the turned items lp_xbatch_decode_frames hands it)
+    c.normalize_orientation = R.opt.normalize_orientation;  // (sizes only the turned items a frame rendition hands it)
     c.jpeg_quality = R.quality;
     c.max_in_bytes = in_bytes + (1 << 20);
     // slot per output: never larger than the callers' buffers (lp_batch copies a whole result into out[i])
@@ -1438,7 +1446,7 @@ static void run_jpeg(lp_xbatch* X, Lane& L, const Task& t) {
     const size_t mcus = (size_t)ceil_div(g.w, 8) * ceil_div(g.h, 8);
     // multi-scan groups: + the nonzero masks per block, + the scan and table-set pools (batch.cu)
     // (a context that takes rotated files: + each chunk slot's oriented crop, at most the frame)
-    const size_t per_img = (mcus * 3 + 64) * (128 + 64 + 2 + (g.jpeg_multiscan ? 8 : 0)) + (size_t)g.w * g.h * 3 * (R.sink == S_FRAMES ? 2 : 1) + 65536;
+    const size_t per_img = (mcus * 3 + 64) * (128 + 64 + 2 + (g.jpeg_multiscan ? 8 : 0)) + (size_t)g.w * g.h * 3 * (turned ? 2 : 1) + 65536;
     const size_t pools = g.jpeg_multiscan ? batch_multiscan_pool_bytes((size_t)n) : 0;
     // every rendition's resized frames stay resident for the group; the sinks run one after another, so the largest
     // sink's room is kept
@@ -1462,9 +1470,8 @@ static void run_jpeg(lp_xbatch* X, Lane& L, const Task& t) {
     int chunk = (int)std::min<long>(fit, 3L * std::max(slots, 1));
     if (slots > 0 && chunk > slots) chunk = chunk / slots * slots;
     c.chunk = std::max(1, std::min(chunk, n));
-    const bool frames = R.sink == S_FRAMES;  // (a call with one rendition: the context may take rotated and gray files)
     lp_batch* b = batch_create_in(&c, L.dev, L.dev_bytes, L.host, L.host_bytes, R.progressive, g.jpeg_multiscan, resize_only,
-                                  frames, frames, several ? geoms.data() : nullptr, several ? (int)geoms.size() : 0);
+                                  turned, turned, several ? geoms.data() : nullptr, several ? (int)geoms.size() : 0);
     if (!b) {
         push_task_fallback(X, t);
         return;
@@ -1640,7 +1647,7 @@ static Rendition make_rendition(const lp_image_options& opt) {
     return R;
 }
 
-// the one rendition of lp_xbatch_decode_frames and lp_xbatch_decode_clips: pixels into the caller's tensor
+// a frame rendition (lp_xbatch_transform_frames, _decode_frames, _decode_clips): pixels into a caller's tensor
 // (none of the file sinks' fields: a ".webp" at quality 101 must not read as lossless output)
 static Rendition frames_rendition(const lp_image_options& opt) {
     Rendition R;
@@ -1650,9 +1657,9 @@ static Rendition frames_rendition(const lp_image_options& opt) {
 }
 
 // A framebuffer Transform hands its encoder (on the device already, or uploaded by mat_device_view) packed into slice
-// `slice` of the call's tensor on this worker's stream by the grid path's kernel; item i's size is the frame's
-static int pack_framebuffer(lp_xbatch* X, int i, lilliput::Framebuffer* f, int64_t slice) {
-    const lp_frame_tensor& T = X->frames;
+// `slice` of frame rendition R's tensor on this worker's stream by the grid path's kernel; item i's size is the frame's
+static int pack_framebuffer(const Rendition& R, int i, lilliput::Framebuffer* f, int64_t slice) {
+    const lp_frame_tensor& T = R.dst;
     int cols = 0, rows = 0, type = 0;
     const uint8_t* dev = nullptr;
     size_t step = 0;
@@ -1666,31 +1673,35 @@ static int pack_framebuffer(lp_xbatch* X, int i, lilliput::Framebuffer* f, int64
     rc = frames_pack_launch(nullptr, &one, 1, frames_layout(T), st);
     if (!rc && cudaStreamSynchronize(st) != cudaSuccess) rc = LP_ERR_CUDA;
     if (rc) return rc;
-    X->frame_w[i] = cols;
-    X->frame_h[i] = rows;
+    R.frame_w[i] = cols;
+    R.frame_h[i] = rows;
     return LP_OK;
 }
 
-// lp_xbatch_decode_frames' per-image route: Transform up to its encoder, whose frame goes to slice i
-static int frames_transform(lp_xbatch* X, int i, const lp_image_options* opt, int max_size) {
-    return lilliput::TransformToFrame(X->in[i], X->in_len[i], opt, max_size,
-                                      [&](lilliput::Framebuffer* f) -> int { return pack_framebuffer(X, i, f, i); });
+// A frame pair's per-image route: Transform up to its encoder, whose frame goes to the item's slice of the rendition's
+// tensor
+static int frames_transform(lp_xbatch* X, int p, int max_size) {
+    const Rendition& R = X->rend[p % X->k];
+    const int i = p / X->k;
+    return lilliput::TransformToFrame(X->in[i], X->in_len[i], &R.opt, max_size,
+                                      [&](lilliput::Framebuffer* f) -> int { return pack_framebuffer(R, i, f, i); });
 }
 
-// lp_xbatch_decode_clips' per-image route: Transform with every selected frame packed into its slot's slice; the slots
-// the stream ended before (the last ones) are zeroed
-static int clips_transform(lp_xbatch* X, int i, const lp_image_options* opt, int max_size) {
+// lp_xbatch_decode_clips' per-image route (one rendition: the pair is the item): Transform with every selected frame
+// packed into its slot's slice; the slots the stream ended before (the last ones) are zeroed
+static int clips_transform(lp_xbatch* X, int i, int max_size) {
+    const Rendition& R = X->rend[0];
     const int T = X->clip_t;
     int filled = 0;
     int rc = lilliput::TransformToClip(
-        X->in[i], X->in_len[i], opt, max_size, T,
+        X->in[i], X->in_len[i], &R.opt, max_size, T,
         [&](lilliput::Framebuffer* f, int t) -> int {
             filled = t + 1;
-            return pack_framebuffer(X, i, f, (int64_t)i * T + t);
+            return pack_framebuffer(R, i, f, (int64_t)i * T + t);
         },
         &X->clip_nframes[i], X->clip_index + (size_t)i * T, X->clip_ms + (size_t)i * T);
     if (rc || filled == T) return rc;
-    const lp_frame_tensor& F = X->frames;
+    const lp_frame_tensor& F = R.dst;
     const size_t slice = (size_t)F.height * F.width * F.channels * frames_dtype_bytes(F.dtype);
     cudaStream_t st = thread_stream();
     if (cudaMemsetAsync((uint8_t*)F.data + ((size_t)i * T + filled) * slice, 0, (size_t)(T - filled) * slice, st) != cudaSuccess ||
@@ -1721,9 +1732,10 @@ static int transform_from_frame(lp_xbatch* X, int i, const lp_image_options* opt
     }, dst, X->out_cap, len);
 }
 
-// One call over n items and k renditions (rends: each one's sink, made from opts[r]); the arguments are checked
-static int xbatch_call(lp_xbatch* X, const uint8_t* const* in, const size_t* in_len, int n, const lp_image_options* opts,
-                       const Rendition* rends, int k, uint8_t* const* out, size_t out_cap, size_t* out_len, int* status) {
+// One call over n items and k renditions (rends: each one's options and sink); out, out_len and status have n * k
+// item-major entries, one per pair (a frame pair's out is null); the arguments are checked
+static int xbatch_call(lp_xbatch* X, const uint8_t* const* in, const size_t* in_len, int n, const Rendition* rends, int k,
+                       uint8_t* const* out, size_t out_cap, size_t* out_len, int* status) {
     int prev = 0;
     cudaGetDevice(&prev);
     LP_CUDA_OK(cudaSetDevice(X->device));
@@ -1761,7 +1773,9 @@ static int xbatch_call(lp_xbatch* X, const uint8_t* const* in, const size_t* in_
             if (!(X->mask[i] >> r & 1)) X->fallback.push_back(i * k + r);
         if (!X->mask[i]) continue;
         const XItem& it = X->items[first_pair(X, i, X->mask[i])];
-        groups[std::make_tuple((int)it.kind, it.w, it.h, it.ch, it.jpeg_sampling | (it.jpeg_multiscan ? 1 << 24 : 0))].push_back(i);
+        // rotated and gray JPEGs form groups of their own when the call has several renditions (below)
+        const int apart = k > 1 && it.jpeg_frames_only ? 1 << 25 : 0;
+        groups[std::make_tuple((int)it.kind, it.w, it.h, it.ch, it.jpeg_sampling | (it.jpeg_multiscan ? 1 << 24 : 0) | apart)].push_back(i);
     }
     std::vector<Task> tasks;
     std::vector<double> cost;  // rough device time: the longest tasks start first
@@ -1846,22 +1860,34 @@ static int xbatch_call(lp_xbatch* X, const uint8_t* const* in, const size_t* in_
         const std::vector<int>& g = kv.second;
         if (kind == K_PNG || kind == K_WEBP || kind == K_FRAME) continue;
         if (kind == K_JPEG) {
-            // host staging bounds a JPEG task: out slots (the pipelined JPEG path only) + item mirrors come from the lane's
-            // pinned arena
+            // A rotated or gray group (only frame renditions take it, and only a context of one rendition orients and
+            // decodes it) runs each rendition as tasks of its own, as animations do; any other group all its renditions
+            // in one context
             uint32_t all = 0;
             for (int i : g) all |= X->mask[i];
-            const int r0 = __builtin_ctz(all);
-            const XItem& it0 = X->items[(size_t)g[0] * k + r0];
-            const bool pipelined = (all & (all - 1)) == 0 && X->rend[r0].sink == S_JPEG;
-            const size_t slot = (pipelined ? round_up(std::min(out_cap, std::max((size_t)65536, (size_t)it0.ow * it0.oh * 3)), (size_t)256) : 0) +
-                                sizeof(JpegDecodeItem) + 64;
-            const size_t per = std::max<size_t>(1, X->lanes[0].host_bytes / slot);
-            const size_t want = std::min(per, std::max<size_t>(1, (g.size() + 1) / 2));  // two tasks at least: both lanes work
-            for (size_t a = 0; a < g.size(); a += want) {
-                Task t{kind, std::vector<int>(g.begin() + a, g.begin() + std::min(g.size(), a + want)), {}};
-                for (int i : t.idx) t.rm.push_back(X->mask[i]);
-                tasks.push_back(std::move(t));
-                cost.push_back((double)tasks.back().idx.size() * it0.w * it0.h * 0.05);
+            std::vector<uint32_t> passes;
+            for (int r = 0; r < k; r++)
+                if ((std::get<4>(kv.first) & 1 << 25) && (all >> r & 1)) passes.push_back(1u << r);
+            if (passes.empty()) passes.push_back(all);
+            for (uint32_t pass : passes) {
+                std::vector<int> gp;
+                for (int i : g)
+                    if (X->mask[i] & pass) gp.push_back(i);
+                // host staging bounds a JPEG task: out slots (the pipelined JPEG path only) + item mirrors come from the
+                // lane's pinned arena
+                const int r0 = __builtin_ctz(pass);
+                const XItem& it0 = X->items[(size_t)gp[0] * k + r0];
+                const bool pipelined = (pass & (pass - 1)) == 0 && X->rend[r0].sink == S_JPEG;
+                const size_t slot = (pipelined ? round_up(std::min(out_cap, std::max((size_t)65536, (size_t)it0.ow * it0.oh * 3)), (size_t)256) : 0) +
+                                    sizeof(JpegDecodeItem) + 64;
+                const size_t per = std::max<size_t>(1, X->lanes[0].host_bytes / slot);
+                const size_t want = std::min(per, std::max<size_t>(1, (gp.size() + 1) / 2));  // two tasks at least: both lanes work
+                for (size_t a = 0; a < gp.size(); a += want) {
+                    Task t{kind, std::vector<int>(gp.begin() + a, gp.begin() + std::min(gp.size(), a + want)), {}};
+                    for (int i : t.idx) t.rm.push_back(X->mask[i] & pass);
+                    tasks.push_back(std::move(t));
+                    cost.push_back((double)tasks.back().idx.size() * it0.w * it0.h * 0.05);
+                }
             }
             continue;
         }
@@ -1913,14 +1939,15 @@ static int xbatch_call(lp_xbatch* X, const uint8_t* const* in, const size_t* in_
             cudaSetDevice(X->device);
             const long l0 = g_launches;
             const int p = fb[q], i = p / k;
+            const lp_image_options* opt = &X->rend[p % k].opt;
             size_t len = 0;
             if (X->rend[p % k].sink == S_FRAMES) {
-                status[p] = X->clip_t ? clips_transform(X, i, &opts[p % k], max_size) : frames_transform(X, i, &opts[p % k], max_size);
+                status[p] = X->clip_t ? clips_transform(X, i, max_size) : frames_transform(X, p, max_size);
             } else if (X->src_w) {
-                status[p] = transform_from_frame(X, i, &opts[p % k], max_size, out[p], &len);
+                status[p] = transform_from_frame(X, i, opt, max_size, out[p], &len);
                 out_len[p] = status[p] == LP_OK ? len : 0;
             } else {
-                status[p] = lp_transform(in[i], in_len[i], &opts[p % k], out[p], out_cap, &len, max_size);
+                status[p] = lp_transform(in[i], in_len[i], opt, out[p], out_cap, &len, max_size);
                 out_len[p] = status[p] == LP_OK ? len : 0;
             }
             fb_launches += g_launches - l0;
@@ -1954,11 +1981,8 @@ static int xbatch_call(lp_xbatch* X, const uint8_t* const* in, const size_t* in_
 extern "C" int lp_xbatch_transform_renditions(lp_xbatch* X, const uint8_t* const* in, const size_t* in_len, int n,
                                               const lp_image_options* opts, int k, uint8_t* const* out, size_t out_cap,
                                               size_t* out_len, int* status) {
-    if (!X || n < 0 || !opts || k < 1 || k > kMaxRenditions || (n > 0 && (!in || !in_len || !out || !out_len || !status)))
-        return LP_ERR_BAD_ARGUMENT;
-    std::vector<Rendition> rends;
-    for (int r = 0; r < k; r++) rends.push_back(make_rendition(opts[r]));
-    return xbatch_call(X, in, in_len, n, opts, rends.data(), k, out, out_cap, out_len, status);
+    if (k < 1) return LP_ERR_BAD_ARGUMENT;
+    return lp_xbatch_transform_frames(X, in, in_len, n, opts, k, out, out_cap, out_len, status, nullptr, 0);
 }
 
 extern "C" int lp_xbatch_transform(lp_xbatch* X, const uint8_t* const* in, const size_t* in_len, int n,
@@ -2002,44 +2026,85 @@ static int check_frame_tensor(const lp_xbatch* X, const lp_frame_tensor* t, int 
     return LP_OK;
 }
 
-// lp_xbatch_decode_frames (X->clip_t 0: one slice per item) and lp_xbatch_decode_clips (clip_t slices per item, its
-// outputs set up by the caller): the call over a checked tensor whose slices are `slice` bytes, then the slices of the
-// items that failed zeroed, as are their sizes
-static int decode_to_tensor(lp_xbatch* X, const uint8_t* const* in, const size_t* in_len, int n, const lp_image_options* opt,
-                            const lp_frame_tensor& T, size_t slice, int* width, int* height, int* status) {
-    const size_t per = (size_t)std::max(1, X->clip_t) * slice;  // an item's slices
-    X->frames = T;
-    X->frame_w = width;
-    X->frame_h = height;
-    for (int i = 0; i < n; i++) width[i] = height[i] = 0;
-    Rendition R = frames_rendition(*opt);
-    std::vector<uint8_t*> out((size_t)n, nullptr);  // (no files: every output of the call is in the tensor)
-    std::vector<size_t> out_len((size_t)n, 0);
-    int rc = xbatch_call(X, in, in_len, n, opt, &R, 1, out.data(), 0, out_len.data(), status);
+// lp_xbatch_transform_frames over checked arguments (slice[j]: the bytes of one slice of frames[j].dst; X->clip_t slices
+// per item, or one).  The pairs go to the callers' arrays directly when every rendition is a file's; otherwise through
+// one item-major pair array of n * (k + m) entries, scattered when the call ends.  Then every frame rendition's failed
+// items get all-zero slices and 0 x 0.
+static int transform_frames_call(lp_xbatch* X, const uint8_t* const* in, const size_t* in_len, int n, const lp_image_options* opts,
+                                 int k, uint8_t* const* out, size_t out_cap, size_t* out_len, int* status,
+                                 const lp_frame_rendition* frames, int m, const size_t* slice) {
+    const int K = k + m;
+    std::vector<Rendition> rends;
+    for (int r = 0; r < k; r++) rends.push_back(make_rendition(opts[r]));
+    for (int j = 0; j < m; j++) {
+        Rendition R = frames_rendition(frames[j].opt);
+        R.dst = frames[j].dst;
+        R.frame_w = frames[j].width;
+        R.frame_h = frames[j].height;
+        for (int i = 0; i < n; i++) R.frame_w[i] = R.frame_h[i] = 0;
+        rends.push_back(R);
+    }
+    if (!m) return xbatch_call(X, in, in_len, n, rends.data(), K, out, out_cap, out_len, status);
+    const size_t np = (size_t)n * K;
+    std::vector<uint8_t*> pout(np, nullptr);
+    std::vector<size_t> plen(np, 0);
+    std::vector<int> pst(np, LP_ERR_UNSUPPORTED);
+    for (size_t i = 0; i < (size_t)n; i++)
+        for (int r = 0; r < k; r++) pout[i * K + r] = out[i * k + r];
+    int rc = xbatch_call(X, in, in_len, n, rends.data(), K, pout.data(), out_cap, plen.data(), pst.data());
+    if (rc) return rc;
+    for (size_t i = 0; i < (size_t)n; i++) {
+        for (int r = 0; r < k; r++) {
+            status[i * k + r] = pst[i * K + r];
+            out_len[i * k + r] = plen[i * K + r];
+        }
+        for (int j = 0; j < m; j++) frames[j].status[i] = pst[i * K + k + j];
+    }
     DeviceGuard g(X->device);
     cudaStream_t st = X->lanes[0].st;
-    for (int i = 0; i < n && !rc;) {
-        if (status[i] == LP_OK) {
-            i++;
-            continue;
+    for (int j = 0; j < m && !rc; j++) {
+        const lp_frame_rendition& F = frames[j];
+        const size_t per = (size_t)std::max(1, X->clip_t) * slice[j];  // an item's slices
+        for (int i = 0; i < n && !rc;) {
+            if (F.status[i] == LP_OK) {
+                i++;
+                continue;
+            }
+            int e = i;
+            for (; e < n && F.status[e] != LP_OK; e++) F.width[e] = F.height[e] = 0;
+            if (cudaMemsetAsync((uint8_t*)F.dst.data + (size_t)i * per, 0, (size_t)(e - i) * per, st) != cudaSuccess) rc = LP_ERR_CUDA;
+            i = e;
         }
-        int e = i;
-        for (; e < n && status[e] != LP_OK; e++) width[e] = height[e] = 0;
-        if (cudaMemsetAsync((uint8_t*)T.data + (size_t)i * per, 0, (size_t)(e - i) * per, st) != cudaSuccess) rc = LP_ERR_CUDA;
-        i = e;
     }
     if (!rc && cudaStreamSynchronize(st) != cudaSuccess) rc = LP_ERR_CUDA;
-    X->frame_w = X->frame_h = nullptr;
     return rc;
+}
+
+extern "C" int lp_xbatch_transform_frames(lp_xbatch* X, const uint8_t* const* in, const size_t* in_len, int n,
+                                          const lp_image_options* opts, int k, uint8_t* const* out, size_t out_cap,
+                                          size_t* out_len, int* status, const lp_frame_rendition* frames, int m) {
+    if (!X || n < 0 || k < 0 || m < 0 || k + m < 1 || k + m > kMaxRenditions || (n > 0 && (!in || !in_len)) ||
+        (k > 0 && (!opts || (n > 0 && (!out || !out_len || !status)))) || (m > 0 && !frames))
+        return LP_ERR_BAD_ARGUMENT;
+    size_t slice[kMaxRenditions] = {};
+    for (int j = 0; j < m; j++) {
+        const lp_frame_rendition& F = frames[j];
+        if ((n > 0 && (!F.width || !F.height || !F.status)) || check_frame_tensor(X, &F.dst, n, &slice[j])) return LP_ERR_BAD_ARGUMENT;
+        const uintptr_t a0 = (uintptr_t)F.dst.data, a1 = a0 + slice[j] * (size_t)n;
+        for (int q = 0; q < j; q++) {  // (no two tensors share a byte of their n slices)
+            const uintptr_t b0 = (uintptr_t)frames[q].dst.data, b1 = b0 + slice[q] * (size_t)n;
+            if (a0 < b1 && b0 < a1) return LP_ERR_BAD_ARGUMENT;
+        }
+    }
+    return transform_frames_call(X, in, in_len, n, opts, k, out, out_cap, out_len, status, frames, m, slice);
 }
 
 extern "C" int lp_xbatch_decode_frames(lp_xbatch* X, const uint8_t* const* in, const size_t* in_len, int n,
                                        const lp_image_options* opt, const lp_frame_tensor* dst, int* width, int* height,
                                        int* status) {
-    if (!X || n < 0 || !opt || !dst || (n > 0 && (!in || !in_len || !width || !height || !status))) return LP_ERR_BAD_ARGUMENT;
-    size_t slice = 0;
-    if (check_frame_tensor(X, dst, n, &slice)) return LP_ERR_BAD_ARGUMENT;
-    return decode_to_tensor(X, in, in_len, n, opt, *dst, slice, width, height, status);
+    if (!opt || !dst) return LP_ERR_BAD_ARGUMENT;
+    const lp_frame_rendition F{*opt, *dst, width, height, status};
+    return lp_xbatch_transform_frames(X, in, in_len, n, nullptr, 0, nullptr, 0, nullptr, nullptr, &F, 1);
 }
 
 extern "C" int lp_xbatch_decode_clips(lp_xbatch* X, const uint8_t* const* in, const size_t* in_len, int n,
@@ -2061,7 +2126,8 @@ extern "C" int lp_xbatch_decode_clips(lp_xbatch* X, const uint8_t* const* in, co
     X->clip_nframes = nframes;
     X->clip_index = frame_index;
     X->clip_ms = start_ms;
-    const int rc = decode_to_tensor(X, in, in_len, n, opt, *dst, slice, width, height, status);
+    const lp_frame_rendition F{*opt, *dst, width, height, status};
+    const int rc = transform_frames_call(X, in, in_len, n, nullptr, 0, nullptr, 0, nullptr, nullptr, &F, 1, &slice);
     X->clip_t = 0;
     X->clip_nframes = X->clip_index = nullptr;
     X->clip_ms = nullptr;
@@ -2089,7 +2155,7 @@ static int encode_tensor(lp_xbatch* X, const lp_frame_tensor& src, int n, int T,
     X->src_ms = duration_ms;
     X->src_loops = loop_count;
     const Rendition R = opt ? make_rendition(*opt) : Rendition();  // (opt may be null when n == 0)
-    const int rc = xbatch_call(X, nullptr, nullptr, n, opt, &R, 1, out, out_cap, out_len, status);
+    const int rc = xbatch_call(X, nullptr, nullptr, n, &R, 1, out, out_cap, out_len, status);
     X->src_w = X->src_h = nullptr;
     X->src_t = 1;
     X->src_nframes = X->src_ms = nullptr;
